@@ -1,12 +1,12 @@
-"""fiesta_b200 -- B200-native (sm_100a) implementation of FIESTA's incremental ESDF hot path.
+"""fiesta_b200 -- H100-native (sm_90a) implementation of FIESTA's incremental ESDF hot path.
 
 The product is the C-ABI shared library `fiesta_b200/lib/libfiesta_b200.so` (declared in include/fiesta_b200.h,
 built from fiesta_b200/csrc/*.cu by `fiesta_b200.build.build()`); C++ callers use the drop-in facade
 include/fiesta_b200/ESDFMap.h.  This module is only the ctypes binding that tests/ and bench.py drive it with:
-`ESDFMap` mirrors the reference class's public surface (/root/reference/include/ESDFMap.h:111-164) method for method.
+`ESDFMap` mirrors the reference class's public surface (FIESTA include/ESDFMap.h:111-164) method for method.
 
 There is no CPU fallback: importing works anywhere, but creating a map without the compiled library or without an
-sm_100 GPU raises.
+sm_90 GPU raises.
 """
 import ctypes as C
 import os
@@ -82,7 +82,7 @@ def load_library():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise FiestaError("%s is missing: run `python -m fiesta_b200.build` (nvcc, sm_100a). There is no CPU "
+            raise FiestaError("%s is missing: run `python -m fiesta_b200.build` (nvcc, sm_90a). There is no CPU "
                               "fallback." % LIB_PATH)
         L = C.CDLL(LIB_PATH)
         L.fiesta_last_error.restype = C.c_char_p

@@ -1,4 +1,4 @@
-"""In-tree build of libfiesta_b200.so (sm_100a only) with nvcc.  No CPU fallback is built or exists."""
+"""In-tree build of libfiesta_b200.so (sm_90a only) with nvcc.  No CPU fallback is built or exists."""
 import os
 import subprocess
 import sys
@@ -11,7 +11,8 @@ SOURCES = ["fb_map.cu", "fb_esdf.cu", "fb_raycast.cu", "fb_exact.cu", "fb_xrelax
 HEADERS = ["fb_common.cuh", "fb_exact.h", "fb_divmagic.h", os.path.join("..", "..", "include", "fiesta_b200.h")]
 # -fmad=false: the ray-casting, query and occupancy code must round every fp64 operation exactly like the reference's
 # separate multiply and add (ESDFMap.cpp:122-123, 519-537; raycast.cpp:100-107).
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [ "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O2"]
 
 
@@ -30,7 +31,7 @@ def _stale(target, deps):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a and link fiesta_b200/lib/libfiesta_b200.so.  Returns the library path."""
+    """Compile every CUDA source for sm_90a and link fiesta_b200/lib/libfiesta_b200.so.  Returns the library path."""
     os.makedirs(LIBDIR, exist_ok=True)
     hdrs = [os.path.join(CSRC, h) for h in HEADERS]
     objs = []
@@ -44,7 +45,7 @@ def build(force=False, verbose=False):
             subprocess.check_call(cmd)
         objs.append(o)
     if force or _stale(LIB, objs):
-        subprocess.check_call([_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        subprocess.check_call([_nvcc(), "-shared", "-o", LIB] + objs + ARCH)
     return LIB
 
 

@@ -1,4 +1,4 @@
-// fiesta_b200 -- shared device/host definitions for the sm_100a kernels.
+// fiesta_b200 -- shared device/host definitions for the sm_90a kernels.
 //
 // HBM layout (all arrays dense, z fastest, index ii = (x*Gy + y)*Pz + z with Pz = Gz rounded up to 4 so that the
 // TMA global strides are 16-byte multiples; ii equals the reference's linear index (ESDFMap.cpp:91) when Gz % 4 == 0):
@@ -20,6 +20,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+// SMs of an H100 SXM: fixed-size grid-stride launches are sized to a multiple of it.
+#define FB_SMS 132
 #define FB_UNKNOWN 0u
 #define FB_INF 1u
 #define FB_TILE 8

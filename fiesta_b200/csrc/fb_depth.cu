@@ -1,5 +1,5 @@
 // fiesta_b200 -- depth image -> point cloud on the device (SURVEY.md 8(f) "next #1": the step right before the hot path).
-// Replaces Fiesta::DepthConversion (/root/reference/include/Fiesta.h:319-382): pin-hole back-projection of a uint16
+// Replaces Fiesta::DepthConversion (FIESTA include/Fiesta.h:319-382): pin-hole back-projection of a uint16
 // millimetre depth image and the temporal consistency filter against the previous image; the surviving points are
 // compacted IN PIXEL ORDER (the order defines the ray indices of the serial ray casting that follows) and handed to the
 // ray-casting kernels without leaving HBM: one 0.6 MB image goes up instead of a 3.7 MB cloud.

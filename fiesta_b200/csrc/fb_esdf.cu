@@ -1,4 +1,4 @@
-// fiesta_b200 -- incremental ESDF update kernels (replaces ESDFMap::UpdateESDF, /root/reference/src/ESDFMap.cpp:273-398).
+// fiesta_b200 -- incremental ESDF update kernels (replaces ESDFMap::UpdateESDF, FIESTA src/ESDFMap.cpp:273-398).
 //
 // E1 insert seeds   (ESDFMap.cpp:278-291)  k_seed_inserts : record := {0, self}, activate the tiles within reach.
 // E2 delete         (ESDFMap.cpp:292-337)  k_delete_scan  : the per-obstacle doubly linked lists (ESDFMap.cpp:24-42) are
@@ -499,12 +499,12 @@ __global__ void k_halo_retire(FbGeom g, uint32_t *cobs, int x_first, int nlayers
 }
 cudaError_t fb_esdf_halo_ingest(const FbGeom &g, const FbEsdfArgs &a, const uint32_t *recv, int x_first, int nlayers, int own_tile_x, unsigned *d_nchanged, cudaStream_t s) {
   if (nlayers <= 0) return cudaSuccess;
-  k_halo_ingest<<<148 * 4, 256, 0, s>>>(g, a, recv, x_first, nlayers, own_tile_x, d_nchanged);
+  k_halo_ingest<<<FB_SMS * 4, 256, 0, s>>>(g, a, recv, x_first, nlayers, own_tile_x, d_nchanged);
   return cudaGetLastError();
 }
 cudaError_t fb_esdf_halo_retire(const FbGeom &g, uint32_t *cobs, int x_first, int nlayers, cudaStream_t s) {
   if (nlayers <= 0) return cudaSuccess;
-  k_halo_retire<<<148 * 4, 256, 0, s>>>(g, cobs, x_first, nlayers);
+  k_halo_retire<<<FB_SMS * 4, 256, 0, s>>>(g, cobs, x_first, nlayers);
   return cudaGetLastError();
 }
 
@@ -537,7 +537,7 @@ cudaError_t fb_esdf_seed_inserts(const FbGeom &g, const FbEsdfArgs &a, const uin
 cudaError_t fb_esdf_delete_scan(const FbGeom &g, const FbEsdfArgs &a, cudaStream_t s) {
   long long nvec = g.ptotal >> 2;
   long long blocks = (nvec + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;                   // grid-stride, a multiple of the SM count
+  if (blocks > FB_SMS * 16) blocks = FB_SMS * 16;                   // grid-stride, a multiple of the SM count
   k_delete_scan<<<(unsigned)blocks, 256, 0, s>>>(g, a);
   return cudaGetLastError();
 }

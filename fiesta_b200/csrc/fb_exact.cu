@@ -1,6 +1,6 @@
 // fiesta_b200 -- ORDER-EXACT mode of UpdateOccupancy / UpdateESDF (FIESTA_MODE_EXACT).
 //
-// The reference result is a function of its sequential FIFO order (/root/reference/src/ESDFMap.cpp:273-398): seeds in
+// The reference result is a function of its sequential FIFO order (FIESTA src/ESDFMap.cpp:273-398): seeds in
 // insert_queue_/delete_queue_ order, dependants of a deleted obstacle in LIFO list order (:301-334), neighbours in dirs_
 // order, strict improvement, and every queue element seeing the writes of all earlier elements.  This file reproduces
 // that order with data-parallel kernels (the CPU model of exactly this formulation is oracle/exact_model.c, which matches
@@ -186,7 +186,7 @@ cudaError_t fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t 
   XCK(cudaMalloc((void **)&X->d_count, 16)); XCK(cudaMalloc((void **)&X->d_flag, 16));
   XCK(cudaMallocHost((void **)&X->h_count, 16));
   XCK(cudaMemsetAsync(X->d_count, 0, 16, s)); XCK(cudaMemsetAsync(X->d_flag, 0, 16, s));
-  k_x_fill64<<<148 * 8, 256, 0, s>>>(X->MB, P, XMB_NONE);
+  k_x_fill64<<<FB_SMS * 8, 256, 0, s>>>(X->MB, P, XMB_NONE);
   XCK(cudaMemsetAsync(X->tkey, 0, P * 8, s));
   XCK(cudaMemsetAsync(X->LS, 0, P * 8, s));
   X->tclock = 1; X->key_base = 0; X->key_epoch = 1; X->key_hi = 1ull << FB_KEY_BITS; X->gen_id = 0; X->wclock = 0; X->sclock = 0;
@@ -266,7 +266,7 @@ cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, ui
     if ((e = x_ensure(X, &X->sel, &X->cap_sel, (size_t)n_del + 16))) return e;
     // `scratch` (one word per voxel) is all-XNONE between uses: every sparse use below undoes its own writes instead of
     // refilling 4 bytes per voxel of the grid three times per call
-    if (!X->scratch_clean) { k_x_fill32<<<148 * 8, 256, 0, s>>>(scratch, P, XNONE); *launches += 1; }
+    if (!X->scratch_clean) { k_x_fill32<<<FB_SMS * 8, 256, 0, s>>>(scratch, P, XNONE); *launches += 1; }
     scratch_ok = true;
     X->scratch_clean = false;                                  // until the undo kernels below are queued (an error return leaves it false)
     k_x_del_minpos<<<nblk(n_del), 256, 0, s>>>(del, n_del, occ, l_occ, scratch);
@@ -288,7 +288,7 @@ cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, ui
       for (int attempt = 0; attempt < 2; ++attempt) {
         size_t cap = X->cap_dv;
         XCK(cudaMemsetAsync(X->d_count, 0, 4, s));
-        k_x_scan_deps<<<148 * 16, 256, 0, s>>>(g, cobs, occbits, scratch, X->LS, X->k1, X->k2, X->dv, X->d_count, (unsigned)((cap < X->cap_k1 ? cap : X->cap_k1) < X->cap_k2 ? (cap < X->cap_k1 ? cap : X->cap_k1) : X->cap_k2), shift);
+        k_x_scan_deps<<<FB_SMS * 16, 256, 0, s>>>(g, cobs, occbits, scratch, X->LS, X->k1, X->k2, X->dv, X->d_count, (unsigned)((cap < X->cap_k1 ? cap : X->cap_k1) < X->cap_k2 ? (cap < X->cap_k1 ? cap : X->cap_k1) : X->cap_k2), shift);
         XCK(cudaMemcpyAsync(X->h_count, X->d_count, 4, cudaMemcpyDeviceToHost, s));
         XCK(cudaStreamSynchronize(s));
         ndep = *X->h_count;

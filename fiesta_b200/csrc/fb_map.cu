@@ -1,8 +1,8 @@
 // fiesta_b200 -- C ABI (include/fiesta_b200.h), host-side map state, and the occupancy / query / export kernels.
 //
 // Host code mirrors what the reference does on the caller's thread with pure arithmetic (index conversions,
-// update-range bookkeeping, sentinel returns: /root/reference/src/ESDFMap.cpp:46-118, 401-421, 792-824) and hands every
-// per-voxel operation to the device.  There is NO CPU fallback: fiesta_create fails without an sm_100 device.
+// update-range bookkeeping, sentinel returns: FIESTA src/ESDFMap.cpp:46-118, 401-421, 792-824) and hands every
+// per-voxel operation to the device.  There is NO CPU fallback: fiesta_create fails without an sm_90 device.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -398,7 +398,7 @@ int fiesta_create(const fiesta_config *cfg, fiesta_map **out) {
   }
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) { set_error("fiesta_create: device is not sm_100 (%s); this build only contains sm_100a code", prop.name); return FIESTA_ERR_NO_DEVICE; }
+  if (prop.major != 9) { set_error("fiesta_create: device is not sm_90 (%s); this build only contains sm_90a code", prop.name); return FIESTA_ERR_NO_DEVICE; }
   CK(cudaSetDevice(cfg->device));
   fiesta_map *m = new (std::nothrow) fiesta_map();
   if (!m) { set_error("out of host memory"); return FIESTA_ERR_INVALID; }
@@ -729,7 +729,7 @@ int fiesta_update_occupancy(fiesta_map *m, int global_map) {
       FbExact &X = m->X;
       k_reset_touched<<<1, 1, 0, m->stream>>>(m->d_ctr);
       cudaMemsetAsync(X.d_count, 0, 8, m->stream);
-      const unsigned blocks = n < 148u * 16u ? n : 148u * 16u;
+      const unsigned blocks = n < FB_SMS * 16u ? n : FB_SMS * 16u;
       // crossings are staged (voxel, first-observation time) in arrays that are scratch between two k_x_relax launches
       unsigned long long *ikey = reinterpret_cast<unsigned long long *>(X.SUM), *dkey = ikey + m->g.ptotal;
       k_integrate<true><<<blocks, 128, 0, m->stream>>>(m->g, m->touch_list, n, m->cnt, m->occ, m->cobs, m->occbits, X.touched, X.emask, X.d_count, X.d_count + 1,
@@ -755,7 +755,7 @@ int fiesta_update_occupancy(fiesta_map *m, int global_map) {
     if ((r = ensure(&m->ins, &m->cap_ins, (size_t)m->n_ins + (size_t)n * 512, true, m->stream))) return -r;
     if ((r = ensure(&m->del, &m->cap_del, (size_t)m->n_del + (size_t)n * 512, true, m->stream))) return -r;
     k_reset_touched<<<1, 1, 0, m->stream>>>(m->d_ctr);
-    const unsigned blocks = n < 148u * 16u ? n : 148u * 16u;
+    const unsigned blocks = n < FB_SMS * 16u ? n : FB_SMS * 16u;
     k_integrate<false><<<blocks, 128, 0, m->stream>>>(m->g, m->touch_list, n, m->cnt, m->occ, m->cobs, m->occbits, m->ins, m->del, &m->d_ctr->n_ins, &m->d_ctr->n_del,
                                                      m->d_ctr, nullptr, nullptr, nullptr, global_map, m->l_hit, m->l_miss, m->l_min, m->l_max, m->l_occ);
     k_reset_queues<<<1, 1, 0, m->stream>>>(m->d_ctr, 1, 0);
@@ -1096,7 +1096,7 @@ int fiesta_host_mirror_refresh(fiesta_host_mirror *p, int64_t *n_changed) {
   p->last_scanned = vol;
   CK(cudaMemsetAsync(p->d_n, 0, 4, m->stream));
   const long long want = (vol + 255) / 256;
-  const unsigned blocks = (unsigned)(want < 148ll * 16 ? want : 148ll * 16);
+  const unsigned blocks = (unsigned)(want < FB_SMS * 16ll ? want : FB_SMS * 16ll);
   k_mirror_diff<<<blocks, 256, 0, m->stream>>>(g, m->cobs, p->d_shadow, lo[0], lo[1], lo[2], ex[0], ex[1], ex[2], p->d_chg, (unsigned)p->cap_chg, p->d_n);
   m->st.kernel_launches++;
   CK(cudaGetLastError());

@@ -1,8 +1,8 @@
 // fiesta_b200 -- per-frame ray casting into the hit/miss counters.
 //
-// Replaces Fiesta::RaycastMultithread + RaycastProcess (/root/reference/include/Fiesta.h:194-303), Raycast()
-// (/root/reference/src/raycast.cpp:56-158) and the counter half of ESDFMap::SetOccupancy
-// (/root/reference/src/ESDFMap.cpp:401-437) with results identical to the reference's SERIAL mode
+// Replaces Fiesta::RaycastMultithread + RaycastProcess (FIESTA include/Fiesta.h:194-303), Raycast()
+// (FIESTA src/raycast.cpp:56-158) and the counter half of ESDFMap::SetOccupancy
+// (FIESTA src/ESDFMap.cpp:401-437) with results identical to the reference's SERIAL mode
 // (ray_cast_num_thread = 0, the only deterministic one).
 //
 // The serial loop is order dependent: a ray's back-to-front free-space marking stops at the first voxel an EARLIER

@@ -1,5 +1,5 @@
 // fiesta_b200 -- device-side visualisation extraction (SURVEY.md 8(f) "next #2"): the step right after the hot path.
-// Replaces the full-box triple loops of ESDFMap::GetPointCloud (/root/reference/src/ESDFMap.cpp:544-582) and
+// Replaces the full-box triple loops of ESDFMap::GetPointCloud (FIESTA src/ESDFMap.cpp:544-582) and
 // ESDFMap::GetSliceMarker + RainbowColorMap (:584-699) with a flag pass + ordered stream compaction (CUB), so only the
 // selected points cross PCIe.  Output order = the reference's loop order (x, then y, then z = increasing linear index).
 #include <cub/cub.cuh>

@@ -1,5 +1,5 @@
 // fiesta_b200 -- ORDER-EXACT mode, E2 (second half) + E3: the re-seeding of the delete loop and the FIFO relaxation loop of
-// UpdateESDF (/root/reference/src/ESDFMap.cpp:301-334, 338-392) as ONE persistent kernel, k_x_relax: every FIFO generation,
+// UpdateESDF (FIESTA src/ESDFMap.cpp:301-334, 338-392) as ONE persistent kernel, k_x_relax: every FIFO generation,
 // every round of its behaviour fixpoint and the ordered hand-over to the next generation run on the device, separated by
 // grid barriers; the host launches it once per UpdateESDF and reads one control block back.
 // (CPU model of exactly this formulation, checked against the sequential reference: oracle/exact_model.c.)
@@ -52,7 +52,7 @@ static __constant__ int x_dirs[24][3] = {
     {-2, 0, 0}, {2, 0, 0}, {0, -2, 0}, {0, 2, 0}, {0, 0, -2}, {0, 0, 2}};
 static __constant__ int x_off_c[X_NOFF];     // the distinct sums a+b, packed (dx+4) | (dy+4)<<4 | (dz+4)<<8 (filled by fb_xrelax_init)
 
-// Index arithmetic is a third of this kernel's instruction stream (ncu source view, profiles/r02_xrelax_ncu.md): 64-bit linear
+// Index arithmetic was a third of this kernel's instruction stream (ncu source view): 64-bit linear
 // indices, six-compare box tests and divisions by the run-time pitch.  The forms below are exact for every grid the library
 // accepts (< 2^30 voxels): 32-bit indices, unsigned range tests, multiply-high divisions with host-made constants.
 __device__ __forceinline__ unsigned x_vi(const FbGeom &g, int x, int y, int z) { return (unsigned)((x * g.gy + y) * g.pz + z); }
@@ -684,7 +684,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       const unsigned nf = (big && r > 1u) ? __ldcg(&ctl->nF[in]) : 0u;
       if (gtid == 0) { ctl->nW[zz] = 0; ctl->nF[zz] = 0; }
       if (r > 1u && nw == 0u && nf == 0u) break;
-      if (r > X_MAX_ROUNDS) { if (gtid == 0) ctl->err = 2u; break; }   // cannot happen (element i is final after i+1 rounds at the latest); never spin forever on a B200
+      if (r > X_MAX_ROUNDS) { if (gtid == 0) ctl->err = 2u; break; }   // cannot happen (element i is final after i+1 rounds at the latest); never spin forever on the GPU
       ++rounds; ++wclock;
       const bool dense = big && r > 1u && nw > a.dense_min;   // more than one wave of warps: evaluate through the summaries
       if (dense) {                                             // bring the summaries up to date first, then evaluate through them

@@ -2,7 +2,7 @@
 
 Every rank integrates every frame identically (ray casting / UpdateOccupancy are replicated); only the distance-field
 relaxation is partitioned: rank r relaxes the tile columns of its x-slab and the 2-voxel ghost layers on the internal faces
-(dirs_ reaches 2 voxels, /root/reference/include/parameters.h:66-68) travel between neighbouring ranks after every local
+(dirs_ reaches 2 voxels, FIESTA include/parameters.h:66-68) travel between neighbouring ranks after every local
 relaxation -- over NVLink with NCCL on GPUs (gloo in the CPU protocol test) -- until no rank sees a changed ghost record.
 A ghost x-layer is Gy*Pz contiguous records, so layers are exchanged exactly as they lie in HBM (no packing kernel).
 """

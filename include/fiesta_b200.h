@@ -1,5 +1,5 @@
 /*
- * fiesta_b200 -- C ABI of the B200-native FIESTA hot path.
+ * fiesta_b200 -- C ABI of the H100-native FIESTA hot path.
  *
  * This is the drop-in boundary: every entry point below replaces one method of the reference's
  * `fiesta::ESDFMap` (or the one `Fiesta` member that drives it) and keeps its argument meaning, return
@@ -29,7 +29,7 @@ enum {
   FIESTA_OK = 0,
   FIESTA_ERR_INVALID = 1,   /* bad argument */
   FIESTA_ERR_CUDA = 2,      /* CUDA runtime/driver error, see fiesta_last_error() */
-  FIESTA_ERR_NO_DEVICE = 3, /* no usable sm_100 device: there is NO CPU fallback */
+  FIESTA_ERR_NO_DEVICE = 3, /* no usable sm_90 device: there is NO CPU fallback */
   FIESTA_ERR_LIMIT = 4      /* grid or frame exceeds a documented limit */
 };
 

@@ -1,10 +1,10 @@
 // fiesta_b200 -- header-compatible C++ facade for the reference class `fiesta::ESDFMap`.
 //
 // Put this directory BEFORE the reference's include/ on the include path and `#include "ESDFMap.h"` in Fiesta.h
-// resolves here: same namespace, class name, constructor and public methods as /root/reference/include/ESDFMap.h:111-164
+// resolves here: same namespace, class name, constructor and public methods as FIESTA include/ESDFMap.h:111-164
 // (dense-array + PROBABILISTIC build, the shipped configuration: parameters.h:9-14), same public field
 // `grid_total_size_`, same sentinel returns.  Every method forwards 1:1 to the C ABI in include/fiesta_b200.h, which runs
-// on the B200.  Ownership matches the reference (Fiesta.h:96,137): `new ESDFMap(...)` / `delete`.
+// on the H100.  Ownership matches the reference (Fiesta.h:96,137): `new ESDFMap(...)` / `delete`.
 //
 // Differences a maintainer should know (see INTEGRATION.md):
 //  * RaycastFrame() is an ADDITION: one call replaces the whole Fiesta::RaycastMultithread loop (Fiesta.h:281-303) and is
@@ -12,7 +12,7 @@
 //    at the next UpdateOccupancy), so Fiesta.h compiles and runs without edits.
 //  * SetOccupancy() is not thread-safe; the reference's threaded ray casting (ray_cast_num_thread > 0) is itself racy
 //    (Fiesta.h:294-300, ESDFMap.cpp:430-433).  Use RaycastFrame() instead of host threads.
-//  * A failed construction (no sm_100 GPU, out of memory) throws std::runtime_error -- there is no CPU fallback.
+//  * A failed construction (no sm_90 GPU, out of memory) throws std::runtime_error -- there is no CPU fallback.
 #ifndef ESDF_MAP_H
 #define ESDF_MAP_H
 

@@ -1,4 +1,4 @@
-/* TEST INFRASTRUCTURE ONLY -- restatement of Fiesta::DepthConversion (/root/reference/include/Fiesta.h:319-382), shared by
+/* TEST INFRASTRUCTURE ONLY -- restatement of Fiesta::DepthConversion (FIESTA include/Fiesta.h:319-382), shared by
  * both oracles (the header needs cv_bridge/OpenCV/PCL and cannot be compiled here).  Fills `cloud` (3 floats per point, pixel
  * order) from a uint16 millimetre depth image; returns the number of points.
  *   image_cnt : value of image_cnt_ AFTER the increment at :321 (1 for the first image)

@@ -1,7 +1,7 @@
 /* TEST INFRASTRUCTURE ONLY -- never linked into, imported by or executed from the product path.
  *
  * CPU model of fiesta_b200's FAST-mode UpdateESDF (fiesta_b200/csrc/fb_esdf.cu): the order-free tile wavefront that
- * replaces ESDFMap::UpdateESDF (/root/reference/src/ESDFMap.cpp:273-398) on the throughput path.  It restates, sequentially
+ * replaces ESDFMap::UpdateESDF (FIESTA src/ESDFMap.cpp:273-398) on the throughput path.  It restates, sequentially
  * and without any CUDA, exactly the schedule-independent semantics of the kernels:
  *   E1  insert seeds            record := self | FRESH, tiles within reach 2 queued           (k_seed_inserts)
  *   E2  delete scan             records whose obstacle no longer exists := INF | FRESH         (k_delete_scan)

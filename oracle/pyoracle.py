@@ -23,7 +23,16 @@ D3 = C.c_double * 3
 I3 = C.c_int * 3
 
 
-def build(reference="/root/reference"):
+# Checkout of the upstream FIESTA sources that oracle/_ref is compiled from.  Optional: tests/golden holds what the
+# tests compare against, so the suite runs without it.
+REFERENCE = os.environ.get("FIESTA_REFERENCE", "")
+
+
+def reference_present(reference=REFERENCE):
+    return bool(reference) and os.path.exists(os.path.join(reference, "src", "ESDFMap.cpp"))
+
+
+def build(reference=REFERENCE):
     """Compile the C restatement and, when the reference sources are present, oracle/_ref."""
     subprocess.check_call(["make", "-s", "-C", _HERE, "all", "REFERENCE=" + reference])
 

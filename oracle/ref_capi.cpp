@@ -1,12 +1,12 @@
 // TEST INFRASTRUCTURE ONLY -- never linked into, imported by or called from the product path.
 //
 // C API around the UNMODIFIED reference class fiesta::ESDFMap (compiled in place from
-// /root/reference/src/ESDFMap.cpp + src/raycast.cpp against oracle/shims) so that tests/, bench.py's
+// FIESTA src/ESDFMap.cpp + src/raycast.cpp against oracle/shims) so that tests/, bench.py's
 // cpu_baseline / --impl reference legs and __graft_entry__.smoke() can drive the real reference
 // through ctypes.  Built by oracle/Makefile into oracle/_ref/libfiesta_ref.so (git-ignored).
 //
 // The only logic restated here is Fiesta::RaycastProcess / RaycastMultithread
-// (/root/reference/include/Fiesta.h:194-303): it lives in a header that needs ROS/OpenCV/PCL and
+// (FIESTA include/Fiesta.h:194-303): it lives in a header that needs ROS/OpenCV/PCL and
 // cannot be compiled in this image.  The restatement follows that text in serial mode
 // (ray_cast_num_thread == 0, the only deterministic mode; launch/*.launch:23) and calls the
 // compiled reference Raycast() and ESDFMap::SetOccupancy().

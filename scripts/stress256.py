@@ -1,8 +1,8 @@
 """Dynamic-obstacle stress (BASELINE.json configs[4], SURVEY.md 8(d)-5): 256^3 grid, every voxel observed, then every frame a
 uniformly random 20 % of the voxels is toggled occupied <-> free (toggle probabilities: one observation flips a voxel).
 
-  python tests/golden/make_stress_nref.py 6      # dev box: CPU oracle -> tests/golden/stress_nref.json
-  python scripts/stress256.py --frames 6         # B200: FAST mode, events resident in HBM; prints one JSON line
+  python tests/golden/make_stress_nref.py 6      # CPU oracle -> tests/golden/stress_nref.json
+  python scripts/stress256.py --frames 6         # GPU: FAST mode, events resident in HBM; prints one JSON line
 """
 import argparse
 import json

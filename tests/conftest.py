@@ -9,13 +9,13 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with -m gpu")
 
 
 @pytest.fixture(scope="session")
 def oracle_built():
-    """Build the CPU oracles (C restatement always; oracle/_ref only where /root/reference exists)."""
+    """Build the CPU oracles (the C restatement; oracle/_ref too where the reference sources are present)."""
     from oracle import pyoracle
-    if not pyoracle.available("port") or (os.path.exists("/root/reference/src/ESDFMap.cpp") and not pyoracle.available("ref")):
+    if not pyoracle.available("port") or (pyoracle.reference_present() and not pyoracle.available("ref")):
         pyoracle.build()
     return pyoracle

@@ -1,7 +1,7 @@
-"""Generates tests/golden/*.json by running the UNMODIFIED reference (oracle/_ref/libfiesta_ref.so, compiled in place from
-/root/reference by oracle/Makefile).  Run in the dev container (the only place /root/reference exists):
+"""Generates tests/golden/reference_golden.json by running the UNMODIFIED reference (oracle/_ref/libfiesta_ref.so, compiled in
+place from a checkout of upstream FIESTA by oracle/Makefile).  Run where that checkout exists:
 
-    python tests/golden/make_golden.py
+    FIESTA_REFERENCE=<checkout> make -C oracle && python tests/golden/make_golden.py
 
 The JSON files pin the C restatement (oracle/esdf_oracle.c) and the CUDA path on machines without the reference.
 Array-valued results are stored as SHA-256 digests plus a few sampled values.
@@ -120,11 +120,73 @@ def dda_vectors(kind):
     return out
 
 
+def mixed_replay(kind):
+    """Seeded mixed SetOccupancy replay on a 32^3 grid with a local update box in round 3 (seed 5): every exported array
+    after every round, the batch queries and the sentinel returns."""
+    rng = np.random.default_rng(5)
+    m = pyoracle.OracleMap((-1.6, -1.6, -1.6), 0.1, (3.15, 3.15, 3.15), kind)
+    m.SetParameters(*scenes.PARAMS_TOGGLE)
+    out = {"grid_size": list(m.grid_size), "rounds": []}
+    for r in range(5):
+        n = 5000
+        vox = rng.integers(0, m.grid_size[0], (n, 3)).astype(np.int32)
+        occ = (rng.random(n) < 0.1).astype(np.uint8)
+        idx = m.SetOccupancyBatchVox(vox, occ)
+        if r == 3:   # local update box
+            m.SetUpdateRange((-1.0, -1.0, -1.0), (1.0, 0.8, 0.6))
+        changed = m.UpdateOccupancy(r != 3)
+        m.UpdateESDF()
+        c = checkpoint(m)
+        c.update(set_occupancy_returns_sha256=digest(idx), update_occupancy=bool(changed), stats={k: int(v) for k, v in m.stats().items()})
+        out["rounds"].append(c)
+        if r == 3:
+            m.SetOriginalRange()
+    pos = rng.uniform(-1.8, 1.8, (3000, 3))
+    out["distance_batch_sha256"] = digest(m.GetDistanceBatch(pos))
+    d, g = m.GetDistWithGradTrilinearBatch(pos * 0.8)
+    out["trilinear_dist_sha256"], out["trilinear_grad_sha256"] = digest(d), digest(g)
+    out["sentinels"] = [m.SetOccupancy((0.0, 0.0, 0.0), 2), m.SetOccupancy((9.0, 0.0, 0.0), 1), m.GetDistance((9.0, 0.0, 0.0)),
+                        m.GetDistWithGradTrilinear((9.0, 0.0, 0.0))[0]]
+    return out
+
+
+def vis_replay(new_map):
+    """GetPointCloud / GetSliceMarker after 4 depth frames into a 64x64x32 grid (seeds 5/6), over the whole map and over a
+    local box.  `new_map(origin, resolution, size)` makes the map (the reference build or the device map).  Arrays are
+    digested as float64 so that the digests do not depend on the dtype a binding returns."""
+    m = new_map((-3.2, -3.2, -1.6), 0.1, (6.4, 6.4, 3.2))
+    m.SetParameters(*scenes.PARAMS_DEFAULT)
+    sc = scenes.Scene((2.8, 2.8, 1.4), 8, 2, seed=5, edge=(0.3, 0.8))
+    for p, yaw in scenes.pose_walk(4, seed=6, clamp=0.5):
+        pts, T = scenes.depth_frame(sc, p, yaw, width=160, height=120, scale=0.25)
+        m.RaycastFrame(pts, T, 0.3, 4.0)
+        m.UpdateOccupancy(True)
+        m.UpdateESDF()
+        sc.step()
+
+    def cloud(lo, hi):
+        a = np.asarray(m.GetPointCloud(lo, hi), np.float64)
+        return dict(n=len(a), sha256=digest(a))
+
+    def marker(sl, max_dist):
+        x, c = m.GetSliceMarker(sl, max_dist)
+        return dict(n=len(x), xyz_sha256=digest(np.asarray(x, np.float64)), rgba_sha256=digest(np.asarray(c, np.float64)))
+
+    out = {"cloud_0_31": cloud(0, 31), "cloud_10_20": cloud(10, 20)}
+    for sl in (0, 12, 16, 31):
+        out["slice_%d" % sl] = marker(sl, 2.0)
+    m.SetUpdateRange((-1.0, -1.5, -0.5), (2.0, 1.0, 0.7), False)              # local visualisation box (Fiesta.h:150)
+    out["local_cloud_0_31"] = cloud(0, 31)
+    out["local_slice_14"] = marker(14, 1.0)
+    return out
+
+
 if __name__ == "__main__":
-    assert pyoracle.available("ref"), "oracle/_ref is not built: run `make -C oracle ref` where /root/reference exists"
+    assert pyoracle.available("ref"), "oracle/_ref is not built: run `FIESTA_REFERENCE=<checkout> make -C oracle ref`"
     gold = dict(generator="tests/golden/make_golden.py", source="oracle/_ref (unmodified reference ESDFMap.cpp + raycast.cpp)",
                 pillar_replay=pillar_replay("ref"), random_replay=random_replay("ref"), raycast_replay=raycast_replay("ref"),
-                dda=dda_vectors("ref"))
+                dda=dda_vectors("ref"), mixed_replay=mixed_replay("ref"),
+                vis_replay=vis_replay(lambda o, r, s: pyoracle.OracleMap(o, r, s, "ref")))
     with open(os.path.join(HERE, "reference_golden.json"), "w") as f:
         json.dump(gold, f, indent=1, sort_keys=True)
     print("wrote", os.path.join(HERE, "reference_golden.json"))

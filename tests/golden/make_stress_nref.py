@@ -1,4 +1,4 @@
-"""Fixture generator (dev box, CPU): the reference's expansion counts for the dynamic-obstacle stress frames of
+"""Fixture generator (CPU): the reference's expansion counts for the dynamic-obstacle stress frames of
 scripts/stress256.py -> tests/golden/stress_nref.json.      python tests/golden/make_stress_nref.py [frames]"""
 import json
 import os

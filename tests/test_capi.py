@@ -1,4 +1,4 @@
-"""CPU tests of the drop-in boundary: the C-ABI library builds for sm_100a, loads, and exports every symbol that
+"""CPU tests of the drop-in boundary: the C-ABI library builds for sm_90a, loads, and exports every symbol that
 include/fiesta_b200.h declares.  No compute is attempted here (no GPU); creating a map must fail loudly, not fall back."""
 import ctypes as C
 import os
@@ -32,10 +32,10 @@ def test_struct_layouts_match_header():
     assert C.sizeof(fiesta_b200.Stats) == 14 * 8 + 6 * 4
 
 
-def test_sass_is_sm100a_with_tma():
+def test_sass_is_sm90a_with_tma():
     import subprocess
     out = subprocess.run(["cuobjdump", "-sass", fiesta_b200.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     assert "UTMALDG" in out          # the wavefront kernel stages tiles with TMA
     assert "SYNCS" in out            # mbarrier
 

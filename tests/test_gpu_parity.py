@@ -1,6 +1,6 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle on identical inputs.
 
-Oracle = the unmodified reference compiled in place (oracle/_ref) when it was built in the dev container, else the C
+Oracle = the unmodified reference compiled in place (oracle/_ref) when it was built (FIESTA_REFERENCE), else the C
 restatement (oracle/esdf_oracle.c).  Distances are compared bit-exactly (they derive from exact integer obstacle
 coordinates); closest-obstacle differences are only tolerated where both obstacles are exactly equidistant.
 """

@@ -1,38 +1,20 @@
 """GPU test of the device-side visualisation extraction (SURVEY.md 8(f) next #2) against the REFERENCE's own
-GetPointCloud / GetSliceMarker (oracle/_ref; skipped where only the C restatement is available)."""
-import numpy as np
+GetPointCloud / GetSliceMarker (tests/golden/reference_golden.json, section vis_replay, made by the compiled reference)."""
+import json
+import os
+
 import pytest
 
-from tests import scenes
+from tests.golden import make_golden
 
 pytestmark = pytest.mark.gpu
+GOLD = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_golden.json")))
 
 
-def test_point_cloud_and_slice_marker(oracle_built):
-    if not oracle_built.available("ref"):
-        pytest.skip("needs oracle/_ref (the compiled reference)")
+def test_point_cloud_and_slice_marker():
     import fiesta_b200
-    origin, res, size = (-3.2, -3.2, -1.6), 0.1, (6.4, 6.4, 3.2)
-    dev = fiesta_b200.ESDFMap(origin, res, size, mode="exact")
-    ora = oracle_built.OracleMap(origin, res, size, "ref")
-    for m in (dev, ora):
-        m.SetParameters(*scenes.PARAMS_DEFAULT)
-    sc = scenes.Scene((2.8, 2.8, 1.4), 8, 2, seed=5, edge=(0.3, 0.8))
-    for p, yaw in scenes.pose_walk(4, seed=6, clamp=0.5):
-        pts, T = scenes.depth_frame(sc, p, yaw, width=160, height=120, scale=0.25)
-        for m in (dev, ora):
-            m.RaycastFrame(pts, T, 0.3, 4.0)
-            m.UpdateOccupancy(True)
-            m.UpdateESDF()
-        sc.step()
-    a, b = dev.GetPointCloud(0, 31), ora.GetPointCloud(0, 31)
-    assert len(b) > 50 and np.array_equal(a, b)
-    assert np.array_equal(dev.GetPointCloud(10, 20), ora.GetPointCloud(10, 20))
-    for sl in (0, 12, 16, 31):
-        (x1, c1), (x2, c2) = dev.GetSliceMarker(sl, 2.0), ora.GetSliceMarker(sl, 2.0)
-        assert np.array_equal(x1, x2) and np.array_equal(c1, c2), sl
-    for m in (dev, ora):                                       # local visualisation box (Fiesta.h:150)
-        m.SetUpdateRange((-1.0, -1.5, -0.5), (2.0, 1.0, 0.7), False)
-    assert np.array_equal(dev.GetPointCloud(0, 31), ora.GetPointCloud(0, 31))
-    (x1, c1), (x2, c2) = dev.GetSliceMarker(14, 1.0), ora.GetSliceMarker(14, 1.0)
-    assert len(x2) > 0 and np.array_equal(x1, x2) and np.array_equal(c1, c2)
+    got = make_golden.vis_replay(lambda o, r, s: fiesta_b200.ESDFMap(o, r, s, mode="exact"))
+    gold = GOLD["vis_replay"]
+    assert gold["cloud_0_31"]["n"] > 50 and gold["local_slice_14"]["n"] > 0
+    for k in gold:
+        assert got[k] == gold[k], k
