@@ -68,7 +68,11 @@ SYMBOLS = [
     "fiesta_host_mirror_create", "fiesta_host_mirror_destroy", "fiesta_host_mirror_refresh", "fiesta_host_mirror_get_distance_pos",
     "fiesta_host_mirror_get_distance_vox", "fiesta_host_mirror_get_dist_grad_trilinear", "fiesta_host_mirror_get_distance_batch_pos",
     "fiesta_host_mirror_get_dist_grad_trilinear_batch", "fiesta_host_mirror_records", "fiesta_host_mirror_stats",
+    "fiesta_check_segments", "fiesta_check_segments_device", "fiesta_get_distance_batch_device",
+    "fiesta_get_dist_grad_trilinear_batch_device", "fiesta_host_mirror_check_segments",
 ]
+
+SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
 
 _lib = None
 
@@ -113,12 +117,36 @@ def load_library():
         for n in ("fiesta_query_plan_positions", "fiesta_query_plan_distances", "fiesta_query_plan_gradients"):
             getattr(L, n).argtypes = [C.c_void_p]
             getattr(L, n).restype = C.POINTER(C.c_double)
+        seg = [C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_int] + [C.c_void_p] * 4
+        L.fiesta_check_segments.argtypes = seg
+        L.fiesta_host_mirror_check_segments.argtypes = seg
+        L.fiesta_check_segments_device.argtypes = seg + [C.c_void_p]
+        L.fiesta_get_distance_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+        L.fiesta_get_dist_grad_trilinear_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
 
 def _f64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
+
+
+def _is_cuda_tensor(a):
+    return getattr(a, "is_cuda", False) is True
+
+
+def _segment_flags(clearance, unknown_blocks):
+    return C.c_double(float(clearance)), SEGMENT_UNKNOWN_BLOCKS if unknown_blocks else 0
+
+
+def _check_segments_host(fn, h, ab, clearance, unknown_blocks, ck):
+    """fiesta_check_segments / fiesta_host_mirror_check_segments on host arrays: (status, hit_idx, hit_t, min_dist)."""
+    ab = _f64(ab).reshape(-1, 6)
+    n = len(ab)
+    out = (np.empty(n, np.int32), np.empty(n, np.int64), np.empty(n), np.empty(n))
+    r, flags = _segment_flags(clearance, unknown_blocks)
+    ck(fn(h, ab.ctypes, C.c_int64(n), r, flags, *(o.ctypes for o in out)), "CheckSegments")
+    return out
 
 
 class QueryPlan:
@@ -189,6 +217,10 @@ class HostMirror:
         self._m._ck(self._m._L.fiesta_host_mirror_get_dist_grad_trilinear_batch(self._h, pos.ctypes, C.c_int64(len(pos)), d.ctypes, g.ctypes),
                     "mirror trilinear batch")
         return d, g
+
+    def CheckSegments(self, ab, clearance, unknown_blocks=False):
+        """Segment clearance from the pinned records (fiesta_host_mirror_check_segments): ab (n,6) -> (status, hit_idx, hit_t, min_dist)."""
+        return _check_segments_host(self._m._L.fiesta_host_mirror_check_segments, self._h, ab, clearance, unknown_blocks, self._m._ck)
 
     def close(self):
         if self._h:
@@ -310,6 +342,47 @@ class ESDFMap:
         g = np.empty((len(pos), 3))
         self._ck(self._L.fiesta_get_dist_grad_trilinear_batch(self._h, pos.ctypes, C.c_int64(len(pos)), d.ctypes, g.ctypes),
                  "GetDistWithGradTrilinear batch")
+        return d, g
+
+    # --- planner queries: segment clearance, and stream-ordered queries on CUDA tensors (torch is imported on these paths only) ---
+    def _device_tensor(self, t, cols, what):
+        import torch
+        if not (t.is_cuda and t.device.index == self.device and t.dtype == torch.float64 and t.is_contiguous()
+                and t.dim() == 2 and t.shape[1] == cols):
+            raise ValueError("%s: expected a contiguous float64 (n, %d) tensor on cuda:%d, got %s %s on %s"
+                             % (what, cols, self.device, t.dtype, tuple(t.shape), t.device))
+        return torch, torch.cuda.current_stream(t.device).cuda_stream
+
+    def CheckSegments(self, ab, clearance, unknown_blocks=False):
+        """Segment clearance (fiesta_check_segments): ab holds n segments {ax, ay, az, bx, by, bz} -> (status, hit_idx, hit_t,
+        min_dist).  numpy in, numpy out; a CUDA float64 (n, 6) tensor on the map's device runs fiesta_check_segments_device on the
+        current torch stream and returns tensors on that device without synchronising."""
+        if not _is_cuda_tensor(ab):
+            return _check_segments_host(self._L.fiesta_check_segments, self._h, ab, clearance, unknown_blocks, self._ck)
+        torch, stream = self._device_tensor(ab, 6, "CheckSegments")
+        n = ab.shape[0]
+        out = (torch.empty(n, dtype=torch.int32, device=ab.device), torch.empty(n, dtype=torch.int64, device=ab.device),
+               torch.empty(n, dtype=torch.float64, device=ab.device), torch.empty(n, dtype=torch.float64, device=ab.device))
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        self._ck(self._L.fiesta_check_segments_device(self._h, ab.data_ptr(), n, r, flags, *(o.data_ptr() for o in out), stream),
+                 "CheckSegments(device)")
+        return out
+
+    def GetDistanceBatchDevice(self, pos):
+        """GetDistance for a CUDA float64 (n, 3) tensor, on the current torch stream (fiesta_get_distance_batch_device)."""
+        torch, stream = self._device_tensor(pos, 3, "GetDistanceBatchDevice")
+        d = torch.empty(pos.shape[0], dtype=torch.float64, device=pos.device)
+        self._ck(self._L.fiesta_get_distance_batch_device(self._h, pos.data_ptr(), pos.shape[0], d.data_ptr(), stream),
+                 "GetDistanceBatchDevice")
+        return d
+
+    def GetDistWithGradTrilinearBatchDevice(self, pos):
+        """GetDistWithGradTrilinear for a CUDA float64 (n, 3) tensor, on the current torch stream -> (dist (n,), grad (n, 3))."""
+        torch, stream = self._device_tensor(pos, 3, "GetDistWithGradTrilinearBatchDevice")
+        d = torch.empty(pos.shape[0], dtype=torch.float64, device=pos.device)
+        g = torch.empty((pos.shape[0], 3), dtype=torch.float64, device=pos.device)
+        self._ck(self._L.fiesta_get_dist_grad_trilinear_batch_device(self._h, pos.data_ptr(), pos.shape[0], d.data_ptr(), g.data_ptr(), stream),
+                 "GetDistWithGradTrilinearBatchDevice")
         return d, g
 
     # --- Fiesta::RaycastMultithread (Fiesta.h:281-303), serial semantics ---

@@ -202,6 +202,41 @@ int fiesta_host_mirror_get_dist_grad_trilinear_batch(const fiesta_host_mirror *p
 const uint32_t *fiesta_host_mirror_records(const fiesta_host_mirror *p);
 int fiesta_host_mirror_stats(const fiesta_host_mirror *p, int64_t out[4]);
 
+/* ---- segment clearance (planners: RRT/PRM edges, line of sight, trajectory checks between waypoints) ----
+ * Is the straight segment a-b (metres) at least `clearance` away from every obstacle, and if not, where does it first come too
+ * close?  Each endpoint is mapped to voxel units as Pos2Vox does ((p - origin) / resolution, fp64) and truncated to a 2^-20 voxel
+ * lattice; every voxel the lattice segment touches is walked in order, with exact integer arithmetic.  A voxel blocks when
+ * GetDistance(Vector3i) <= clearance or, with FIESTA_SEGMENT_UNKNOWN_BLOCKS, when it was never observed.  In other words: a segment
+ * is clear iff GetDistance(p) > clearance at every point p of it (and, with the flag, no point of it lies in unknown space).
+ * Outputs per segment:
+ *   status   0 = clear, 1 = blocked, 2 = an endpoint is outside the map (PosInMap, ESDFMap.cpp:46-61) or NaN
+ *   hit_idx  linear index x*Gy*Gz + y*Gz + z of the first blocking voxel, else -1
+ *   hit_t    parameter in [0,1] at which the segment enters that voxel (0 for the start voxel), else NaN
+ *   min_dist minimum GetDistance(Vector3i) over the voxels walked up to and including the first blocking one (all of them when
+ *            clear); -10000 when outside
+ * `ab` holds n segments as {ax, ay, az, bx, by, bz}.  FIESTA_ERR_INVALID for a NaN, negative or >= +10000 clearance, unknown flag
+ * bits, or null buffers with n > 0.  All variants return identical arrays for the same records. */
+#define FIESTA_SEGMENT_UNKNOWN_BLOCKS 1
+/* host pointers; synchronous like the other batch queries */
+int fiesta_check_segments(fiesta_map *m, const double *ab, int64_t n, double clearance, int flags, int32_t *status, int64_t *hit_idx,
+                          double *hit_t, double *min_dist);
+/* pure host code on the pinned records, as of the last refresh */
+int fiesta_host_mirror_check_segments(const fiesta_host_mirror *p, const double *ab, int64_t n, double clearance, int flags,
+                                      int32_t *status, int64_t *hit_idx, double *hit_t, double *min_dist);
+
+/* ---- stream-ordered queries on DEVICE buffers (GPU planners whose positions already live in HBM) ----
+ * The same queries on device pointers valid on the map's device, enqueued on `stream` (a cudaStream_t; 0 = the legacy default
+ * stream); they return without synchronising the host.  Ordering: the query sees every map update issued before the call (the
+ * stream first waits for the work enqueued on the map's stream), and every map update issued after the call (ray casting,
+ * UpdateOccupancy, UpdateESDF, ...) waits for the query to finish reading.  The query writes only the caller's buffers.  The point
+ * queries run the kernel of the host batch forms and return the same bits.  CUDA-graph capture is not supported: a capturing
+ * stream is rejected with FIESTA_ERR_INVALID. */
+int fiesta_check_segments_device(fiesta_map *m, const double *d_ab, int64_t n, double clearance, int flags, int32_t *d_status,
+                                 int64_t *d_hit_idx, double *d_hit_t, double *d_min_dist, void *stream);
+int fiesta_get_distance_batch_device(fiesta_map *m, const double *d_pos_xyz, int64_t n, double *d_dist, void *stream);
+int fiesta_get_dist_grad_trilinear_batch_device(fiesta_map *m, const double *d_pos_xyz, int64_t n, double *d_dist, double *d_grad_xyz,
+                                                void *stream);
+
 /* ---- state dumps in the reference's own representation (parity harness; host pointers, grid_total_size entries) ---- */
 int fiesta_export_distance(fiesta_map *m, double *out);             /* distance_buffer_: -10000 unknown, +10000 unreached */
 int fiesta_export_closest_obstacle(fiesta_map *m, int *out_xyz);    /* closest_obstacle_: 3 ints, -10000 = none */

@@ -135,6 +135,27 @@ class ESDFMap {
     return p;
   }
 
+  // Segment clearance for planners (fiesta_check_segments in fiesta_b200.h): n segments {ax, ay, az, bx, by, bz}; per segment
+  // status (0 clear, 1 blocked, 2 outside the map), the first blocking voxel's linear index and entry parameter, and the minimum
+  // distance walked.  flags: FIESTA_SEGMENT_UNKNOWN_BLOCKS.  Host pointers, synchronous.
+  void CheckSegments(const double *ab, long n, double clearance, int flags, int32_t *status, int64_t *hit_idx, double *hit_t,
+                     double *min_dist) {
+    check(fiesta_check_segments(h_, ab, n, clearance, flags, status, hit_idx, hit_t, min_dist), "CheckSegments");
+  }
+  // The same queries on DEVICE buffers, enqueued on `stream` (a cudaStream_t) without synchronising the host; ordered after every
+  // earlier map update and before every later one (fiesta_b200.h).
+  void CheckSegmentsDevice(const double *d_ab, long n, double clearance, int flags, int32_t *d_status, int64_t *d_hit_idx,
+                           double *d_hit_t, double *d_min_dist, void *stream) {
+    check(fiesta_check_segments_device(h_, d_ab, n, clearance, flags, d_status, d_hit_idx, d_hit_t, d_min_dist, stream),
+          "CheckSegmentsDevice");
+  }
+  void GetDistanceBatchDevice(const double *d_pos_xyz, long n, double *d_dist, void *stream) {
+    check(fiesta_get_distance_batch_device(h_, d_pos_xyz, n, d_dist, stream), "GetDistanceBatchDevice");
+  }
+  void GetDistWithGradTrilinearBatchDevice(const double *d_pos_xyz, long n, double *d_dist, double *d_grad_xyz, void *stream) {
+    check(fiesta_get_dist_grad_trilinear_batch_device(h_, d_pos_xyz, n, d_dist, d_grad_xyz, stream), "GetDistWithGradTrilinearBatchDevice");
+  }
+
   // ---- visualisation (ESDFMap.h:144-145): flag pass + ordered stream compaction on the device, only the selected points
   // cross PCIe (fiesta_get_point_cloud / fiesta_get_slice_marker) ----
   void GetPointCloud(sensor_msgs::PointCloud &m, int vis_lower_bound, int vis_upper_bound) {
