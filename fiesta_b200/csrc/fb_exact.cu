@@ -21,6 +21,7 @@
 #include <cub/cub.cuh>
 #include <stdio.h>
 #include <stdlib.h>
+#include <algorithm>
 #include <chrono>
 #include "fb_common.cuh"
 #include "fb_exact.h"
@@ -111,141 +112,100 @@ __global__ void k_x_fill64(unsigned long long *a, size_t n, unsigned long long v
 }
 
 // ================================================================== host side
-#define XCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { snprintf(X->err, sizeof(X->err), "%s: %s", #call, cudaGetErrorString(e__)); return e__; } } while (0)
 static inline unsigned nblk(size_t n, unsigned t = 256) { return (unsigned)((n + t - 1) / t); }
 
-template <typename T>
-static cudaError_t x_ensure(FbExact *X, T **p, size_t *cap, size_t need) {
-  if (need <= *cap) return cudaSuccess;
-  size_t nc = need + need / 2 + 4096;
-  T *np = nullptr;
-  XCK(cudaMalloc((void **)&np, nc * sizeof(T)));
-  if (*p) cudaFree(*p);
-  *p = np; *cap = nc;
-  return cudaSuccess;
-}
-static cudaError_t x_tmp(FbExact *X, size_t bytes) {
-  if (bytes <= X->cub_bytes) return cudaSuccess;
-  if (X->cub_tmp) cudaFree(X->cub_tmp);
-  X->cub_bytes = bytes + bytes / 2 + (1u << 20);
-  XCK(cudaMalloc(&X->cub_tmp, X->cub_bytes));
-  return cudaSuccess;
-}
 // ordered compaction: out[0..count) = in[i] for flags[i] != 0, order kept
-static cudaError_t x_select(FbExact *X, const uint32_t *in, const uint8_t *flags, uint32_t *out, unsigned n, unsigned *count, cudaStream_t s) {
+static int x_select(FbExact *X, const uint32_t *in, const uint8_t *flags, uint32_t *out, unsigned n, unsigned *count, cudaStream_t s) {
   *count = 0;
-  if (n == 0) return cudaSuccess;
+  if (n == 0) return FIESTA_OK;
   size_t bytes = 0;
-  XCK(cub::DeviceSelect::Flagged(nullptr, bytes, in, flags, out, X->d_count, (int)n, s));
-  cudaError_t e = x_tmp(X, bytes); if (e) return e;
-  XCK(cub::DeviceSelect::Flagged(X->cub_tmp, bytes, in, flags, out, X->d_count, (int)n, s));
-  XCK(cudaMemcpyAsync(X->h_count, X->d_count, 4, cudaMemcpyDeviceToHost, s));
-  XCK(cudaStreamSynchronize(s));
+  CK(cub::DeviceSelect::Flagged(nullptr, bytes, in, flags, out, X->d_count.p, (int)n, s));
+  CK(X->cub_tmp.grow(bytes, s));
+  CK(cub::DeviceSelect::Flagged(X->cub_tmp.p, bytes, in, flags, out, X->d_count.p, (int)n, s));
+  CK(cudaMemcpyAsync(X->h_count, X->d_count, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
   *count = *X->h_count;
-  return cudaSuccess;
+  return FIESTA_OK;
 }
-static cudaError_t x_sort_pairs(FbExact *X, const unsigned long long *kin, unsigned long long *kout, const uint32_t *vin, uint32_t *vout, unsigned n, cudaStream_t s,
-                                int key_bits = 64) {
+static int x_sort_pairs(FbExact *X, const unsigned long long *kin, unsigned long long *kout, const uint32_t *vin, uint32_t *vout, unsigned n, cudaStream_t s,
+                        int key_bits = 64) {
   size_t bytes = 0;
-  XCK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, kin, kout, vin, vout, (int)n, 0, key_bits, s));
-  cudaError_t e = x_tmp(X, bytes); if (e) return e;
-  XCK(cub::DeviceRadixSort::SortPairs(X->cub_tmp, bytes, kin, kout, vin, vout, (int)n, 0, key_bits, s));
-  return cudaSuccess;
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, kin, kout, vin, vout, (int)n, 0, key_bits, s));
+  CK(X->cub_tmp.grow(bytes, s));
+  CK(cub::DeviceRadixSort::SortPairs(X->cub_tmp.p, bytes, kin, kout, vin, vout, (int)n, 0, key_bits, s));
+  return FIESTA_OK;
 }
-cudaError_t fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t s) {
-  memset(X, 0, sizeof(*X));
+int fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t s) {
   const size_t P = (size_t)g.ptotal;
-  XCK(fb_xrelax_init());
+  CK(fb_xrelax_init());
   X->relax_blocks = fb_xrelax_blocks(device);
-  if (X->relax_blocks <= 0 || X->relax_blocks > FB_X_MAX_BLOCKS) { snprintf(X->err, sizeof(X->err), "k_x_relax does not fit on this device"); return cudaErrorInvalidConfiguration; }
-  XCK(cudaMalloc((void **)&X->MB, P * 8)); XCK(cudaMalloc((void **)&X->LS, P * 8)); XCK(cudaMalloc((void **)&X->tkey, P * 8));
-  XCK(cudaMalloc((void **)&X->touched, P * 4));
-  XCK(cudaMalloc((void **)&X->SUM, P * 16)); XCK(cudaMalloc((void **)&X->SUMg, P * 4)); XCK(cudaMemsetAsync(X->SUMg, 0, P * 4, s));
-  XCK(cudaMalloc((void **)&X->emask, P * 4));
-  XCK(cudaMalloc((void **)&X->wstamp, P * 4)); XCK(cudaMemsetAsync(X->wstamp, 0, P * 4, s));
-  for (int k = 0; k < 3; ++k) { XCK(cudaMalloc((void **)&X->W[k], P * 4)); XCK(cudaMalloc((void **)&X->F[k], P * 4)); }
-  for (int k = 0; k < 2; ++k) { XCK(cudaMalloc((void **)&X->E[k], P * 4)); X->cap_E[k] = P; }
+  if (X->relax_blocks <= 0 || X->relax_blocks > FB_X_MAX_BLOCKS) { fb_set_error("exact mode init: k_x_relax does not fit on this device"); return FIESTA_ERR_CUDA; }
+  CK(X->MB.alloc(P)); CK(X->LS.alloc(P)); CK(X->tkey.alloc(P));
+  CK(X->touched.alloc(P));
+  CK(X->SUM.alloc(P)); CK(X->SUMg.alloc(P)); CK(cudaMemsetAsync(X->SUMg, 0, P * 4, s));
+  CK(X->emask.alloc(P));
+  CK(X->wstamp.alloc(P)); CK(cudaMemsetAsync(X->wstamp, 0, P * 4, s));
+  for (int k = 0; k < 3; ++k) { CK(X->W[k].alloc(P)); CK(X->F[k].alloc(P)); }
+  for (int k = 0; k < 2; ++k) CK(X->E[k].alloc(P));
   X->dense_min = 16384u;
   if (const char *e = getenv("FIESTA_X_DENSE")) { long v = atol(e); if (v >= 0 && v <= (1 << 24)) X->dense_min = (unsigned)v; }
   X->small_max = FB_X_SMALL_DEFAULT;
   if (const char *e = getenv("FIESTA_X_SMALL")) { long v = atol(e); if (v >= 0 && v <= 65536) X->small_max = (unsigned)v; }
-  XCK(cudaMalloc((void **)&X->slotc, ((size_t)X->small_max + 1) * 32 * 4));
+  CK(X->slotc.alloc(((size_t)X->small_max + 1) * 32));
   // Per-frame work arrays (touched voxels, dependants of deleted obstacles, sort scratch) are sized up front for 1/8 of the
   // grid: growing them on demand puts cudaMalloc / cudaFree (device-wide synchronisations, milliseconds) inside UpdateESDF.
-  {
-    const size_t c0 = P / 8 > (1u << 20) ? P / 8 : (1u << 20);
-    cudaError_t e;
-    if ((e = x_ensure(X, &X->k1, &X->cap_k1, c0)) || (e = x_ensure(X, &X->k2, &X->cap_k2, c0)) || (e = x_ensure(X, &X->k1b, &X->cap_k1b, c0)) ||
-        (e = x_ensure(X, &X->k2b, &X->cap_k2b, c0)) || (e = x_ensure(X, &X->dv, &X->cap_dv, c0)) || (e = x_ensure(X, &X->idx[0], &X->cap_idx[0], c0)) ||
-        (e = x_ensure(X, &X->idx[1], &X->cap_idx[1], c0)) || (e = x_ensure(X, &X->deps, &X->cap_deps, c0)) || (e = x_ensure(X, &X->nc[0], &X->cap_nc[0], c0)) ||
-        (e = x_ensure(X, &X->nc[1], &X->cap_nc[1], c0)) || (e = x_ensure(X, &X->flags, &X->cap_flags, c0)) || (e = x_ensure(X, &X->flags2, &X->cap_flags2, c0)) ||
-        (e = x_ensure(X, &X->sel, &X->cap_sel, c0)) || (e = x_tmp(X, c0 * 16 + (64u << 20)))) return e;
-  }
-  XCK(cudaMalloc((void **)&X->d_ctl, sizeof(FbXCtl))); XCK(cudaMemsetAsync(X->d_ctl, 0, sizeof(FbXCtl), s));
-  XCK(cudaMallocHost((void **)&X->h_ctl, sizeof(FbXCtl)));
-  XCK(cudaMalloc((void **)&X->d_count, 16)); XCK(cudaMalloc((void **)&X->d_flag, 16));
-  XCK(cudaMallocHost((void **)&X->h_count, 16));
-  XCK(cudaMemsetAsync(X->d_count, 0, 16, s)); XCK(cudaMemsetAsync(X->d_flag, 0, 16, s));
+  const size_t c0 = P / 8 > (1u << 20) ? P / 8 : (1u << 20);
+  for (FbDevBuf<unsigned long long> *b : {&X->k1, &X->k2, &X->k1b, &X->k2b}) CK(b->grow(c0, s));
+  for (FbDevBuf<uint32_t> *b : {&X->dv, &X->idx[0], &X->idx[1], &X->deps, &X->nc[0], &X->nc[1], &X->sel}) CK(b->grow(c0, s));
+  CK(X->flags.grow(c0, s)); CK(X->flags2.grow(c0, s));
+  CK(X->cub_tmp.grow(c0 * 16 + (64u << 20), s));
+  CK(X->d_ctl.alloc(1)); CK(cudaMemsetAsync(X->d_ctl, 0, sizeof(FbXCtl), s));
+  CK(X->h_ctl.alloc(1));
+  CK(X->d_count.alloc(4)); CK(X->d_flag.alloc(4));
+  CK(X->h_count.alloc(4));
+  CK(cudaMemsetAsync(X->d_count, 0, 16, s)); CK(cudaMemsetAsync(X->d_flag, 0, 16, s));
   k_x_fill64<<<FB_SMS * 8, 256, 0, s>>>(X->MB, P, XMB_NONE);
-  XCK(cudaMemsetAsync(X->tkey, 0, P * 8, s));
-  XCK(cudaMemsetAsync(X->LS, 0, P * 8, s));
+  CK(cudaMemsetAsync(X->tkey, 0, P * 8, s));
+  CK(cudaMemsetAsync(X->LS, 0, P * 8, s));
   X->tclock = 1; X->key_base = 0; X->key_epoch = 1; X->key_hi = 1ull << FB_KEY_BITS; X->gen_id = 0; X->wclock = 0; X->sclock = 0;
-  return cudaGetLastError();
-}
-void fb_exact_free(FbExact *X) {
-  void *p[] = {X->MB, X->LS, X->tkey, X->touched, X->SUM, X->SUMg, X->emask, X->wstamp, X->W[0], X->W[1], X->W[2], X->F[0], X->F[1], X->F[2], X->slotc,
-               X->d_ctl, X->d_dbg, X->d_count, X->d_flag, X->E[0], X->E[1], X->sel,
-               X->k1, X->k2, X->k1b, X->k2b, X->dv, X->idx[0], X->idx[1], X->deps, X->nc[0], X->nc[1], X->flags, X->flags2, X->cub_tmp};
-  for (void *q : p) if (q) cudaFree(q);
-  if (X->h_count) cudaFreeHost(X->h_count);
-  if (X->h_ctl) cudaFreeHost(X->h_ctl);
-  memset(X, 0, sizeof(*X));
+  CK(cudaGetLastError());
+  return FIESTA_OK;
 }
 
 // Second half of UpdateOccupancy (ESDFMap.cpp:263-267): k_integrate<true> (fb_map.cu) staged the voxels that crossed the
 // occupancy threshold with the serial time of their first observation; sorted by that time they are appended to
 // insert_queue_ / delete_queue_ in the order the reference's walk over occupancy_queue_ pushes them.
-cudaError_t fb_exact_queue_crossings(FbExact *X, const unsigned long long *ins_key, const uint32_t *ins_vox, const unsigned long long *del_key,
-                                     const uint32_t *del_vox, uint32_t **ins, size_t *cap_ins, unsigned *n_ins, uint32_t **del, size_t *cap_del,
-                                     unsigned *n_del, cudaStream_t s, int *launches) {
-  cudaError_t e;
-  XCK(cudaMemcpyAsync(X->h_count, X->d_count, 8, cudaMemcpyDeviceToHost, s));
-  XCK(cudaStreamSynchronize(s));
+int fb_exact_queue_crossings(FbExact *X, const unsigned long long *ins_key, const uint32_t *ins_vox, const unsigned long long *del_key,
+                             const uint32_t *del_vox, FbDevBuf<uint32_t> &ins, unsigned *n_ins, FbDevBuf<uint32_t> &del, unsigned *n_del,
+                             cudaStream_t s, int *launches) {
+  int r;
+  CK(cudaMemcpyAsync(X->h_count, X->d_count, 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
   const unsigned ni = X->h_count[0], nd = X->h_count[1];
-  for (int q = 0; q < 2; ++q) {                                 // grow the queues if needed (contents kept)
-    uint32_t **lst = q ? del : ins; size_t *cap = q ? cap_del : cap_ins; const unsigned have = q ? *n_del : *n_ins, add = q ? nd : ni;
-    if ((size_t)have + add > *cap) {
-      size_t nc = (size_t)have + add + ((size_t)have + add) / 2 + 4096;
-      uint32_t *np = nullptr;
-      XCK(cudaMalloc((void **)&np, nc * 4));
-      if (*lst && have) XCK(cudaMemcpyAsync(np, *lst, (size_t)have * 4, cudaMemcpyDeviceToDevice, s));
-      XCK(cudaStreamSynchronize(s));
-      if (*lst) cudaFree(*lst);
-      *lst = np; *cap = nc;
-    }
-  }
-  if ((e = x_ensure(X, &X->k1b, &X->cap_k1b, ni > nd ? ni : nd))) return e;
-  if (ni) { if ((e = x_sort_pairs(X, ins_key, X->k1b, ins_vox, *ins + *n_ins, ni, s, FB_KEY_BITS))) return e; *n_ins += ni; *launches += 1; }
-  if (nd) { if ((e = x_sort_pairs(X, del_key, X->k1b, del_vox, *del + *n_del, nd, s, FB_KEY_BITS))) return e; *n_del += nd; *launches += 1; }
-  return cudaSuccess;
+  CK(ins.grow((size_t)*n_ins + ni, s, *n_ins));                // the queued entries are kept
+  CK(del.grow((size_t)*n_del + nd, s, *n_del));
+  CK(X->k1b.grow(ni > nd ? ni : nd, s));
+  if (ni) { if ((r = x_sort_pairs(X, ins_key, X->k1b, ins_vox, ins + *n_ins, ni, s, FB_KEY_BITS))) return r; *n_ins += ni; *launches += 1; }
+  if (nd) { if ((r = x_sort_pairs(X, del_key, X->k1b, del_vox, del + *n_del, nd, s, FB_KEY_BITS))) return r; *n_del += nd; *launches += 1; }
+  return FIESTA_OK;
 }
 // A new integration epoch: later observations beat everything recorded so far in tkey (fb_touch), so nothing is reset.
-cudaError_t fb_exact_next_epoch(FbExact *X, const FbGeom &g, cudaStream_t s) {
+int fb_exact_next_epoch(FbExact *X, const FbGeom &g, cudaStream_t s) {
   X->key_base = 0;
   if (++X->key_epoch >= (1u << (64 - FB_KEY_BITS))) {          // epoch field exhausted (2^20 integrations): start over on a zeroed array
-    XCK(cudaMemsetAsync(X->tkey, 0, (size_t)g.ptotal * 8, s));
+    CK(cudaMemsetAsync(X->tkey, 0, (size_t)g.ptotal * 8, s));
     X->key_epoch = 1;
   }
   X->key_hi = (unsigned long long)X->key_epoch << FB_KEY_BITS;
-  return cudaSuccess;
+  return FIESTA_OK;
 }
 
-cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *scratch, const double *occ, const uint32_t *occbits, double l_occ,
-                                 const uint32_t *ins, unsigned n_ins, const uint32_t *del, unsigned n_del, cudaStream_t s, FbExactStats *st, int *launches) {
-  cudaError_t e;
+int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *scratch, const double *occ, const uint32_t *occbits, double l_occ,
+                         const uint32_t *ins, unsigned n_ins, const uint32_t *del, unsigned n_del, cudaStream_t s, FbExactStats *st, int *launches) {
+  int r;
   const size_t P = (size_t)g.ptotal;
   memset(st, 0, sizeof(*st));
-  if ((e = x_ensure(X, &X->flags, &X->cap_flags, (size_t)(n_ins > n_del ? n_ins : n_del) + 16))) return e;
+  CK(X->flags.grow((size_t)(n_ins > n_del ? n_ins : n_del) + 16, s));
   static const bool xdbg = getenv("FIESTA_DEBUG_X") != nullptr;
   auto now = [] { return std::chrono::steady_clock::now(); };
   auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
@@ -256,14 +216,14 @@ cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, ui
   bool scratch_ok = X->scratch_clean;
   if (n_ins) {
     k_x_flag_exist<<<nblk(n_ins), 256, 0, s>>>(ins, n_ins, occ, l_occ, X->flags, 1);
-    if ((e = x_select(X, ins, X->flags, X->E[0], n_ins, &nE, s))) return e;
+    if ((r = x_select(X, ins, X->flags, X->E[0], n_ins, &nE, s))) return r;
     if (nE) k_x_apply_seed<<<nblk(nE), 256, 0, s>>>(g, X->E[0], nE, cobs, X->LS, X->tclock);
     X->tclock += nE;
     *launches += 2;
   }
   // ---- E2: deletes (:292-337)
   if (n_del) {
-    if ((e = x_ensure(X, &X->sel, &X->cap_sel, (size_t)n_del + 16))) return e;
+    CK(X->sel.grow((size_t)n_del + 16, s));
     // `scratch` (one word per voxel) is all-XNONE between uses: every sparse use below undoes its own writes instead of
     // refilling 4 bytes per voxel of the grid three times per call
     if (!X->scratch_clean) { k_x_fill32<<<FB_SMS * 8, 256, 0, s>>>(scratch, P, XNONE); *launches += 1; }
@@ -272,7 +232,7 @@ cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, ui
     k_x_del_minpos<<<nblk(n_del), 256, 0, s>>>(del, n_del, occ, l_occ, scratch);
     k_x_del_flag<<<nblk(n_del), 256, 0, s>>>(del, n_del, occ, l_occ, scratch, X->flags);
     unsigned nd = 0;
-    if ((e = x_select(X, del, X->flags, X->sel, n_del, &nd, s))) return e;
+    if ((r = x_select(X, del, X->flags, X->sel, n_del, &nd, s))) return r;
     k_x_unset<<<nblk(n_del), 256, 0, s>>>(del, n_del, scratch);
     *launches += 3;
     if (nd) {
@@ -286,41 +246,41 @@ cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, ui
       // dependants: the list is sized by a first counting attempt, then (rarely) re-run with more room
       unsigned ndep = 0;
       for (int attempt = 0; attempt < 2; ++attempt) {
-        size_t cap = X->cap_dv;
-        XCK(cudaMemsetAsync(X->d_count, 0, 4, s));
-        k_x_scan_deps<<<FB_SMS * 16, 256, 0, s>>>(g, cobs, occbits, scratch, X->LS, X->k1, X->k2, X->dv, X->d_count, (unsigned)((cap < X->cap_k1 ? cap : X->cap_k1) < X->cap_k2 ? (cap < X->cap_k1 ? cap : X->cap_k1) : X->cap_k2), shift);
-        XCK(cudaMemcpyAsync(X->h_count, X->d_count, 4, cudaMemcpyDeviceToHost, s));
-        XCK(cudaStreamSynchronize(s));
+        const size_t cap = std::min({X->dv.cap, X->k1.cap, X->k2.cap});
+        CK(cudaMemsetAsync(X->d_count, 0, 4, s));
+        k_x_scan_deps<<<FB_SMS * 16, 256, 0, s>>>(g, cobs, occbits, scratch, X->LS, X->k1, X->k2, X->dv, X->d_count, (unsigned)cap, shift);
+        CK(cudaMemcpyAsync(X->h_count, X->d_count, 4, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
         ndep = *X->h_count;
         *launches += 1;
-        if (ndep <= cap && ndep <= X->cap_k1 && ndep <= X->cap_k2) break;
-        if ((e = x_ensure(X, &X->dv, &X->cap_dv, ndep))) return e;
-        if ((e = x_ensure(X, &X->k1, &X->cap_k1, ndep))) return e;
-        if ((e = x_ensure(X, &X->k2, &X->cap_k2, ndep))) return e;
+        if (ndep <= cap) break;
+        CK(X->dv.grow(ndep, s));
+        CK(X->k1.grow(ndep, s));
+        CK(X->k2.grow(ndep, s));
       }
       st->dependants = ndep;
       k_x_unset<<<nblk(nd), 256, 0, s>>>(X->sel, nd, scratch);
       if (ndep) {
-        if ((e = x_ensure(X, &X->k1b, &X->cap_k1b, ndep))) return e;
-        if ((e = x_ensure(X, &X->k2b, &X->cap_k2b, ndep))) return e;
-        if ((e = x_ensure(X, &X->idx[0], &X->cap_idx[0], ndep))) return e;
-        if ((e = x_ensure(X, &X->idx[1], &X->cap_idx[1], ndep))) return e;
-        if ((e = x_ensure(X, &X->deps, &X->cap_deps, ndep))) return e;
-        if ((e = x_ensure(X, &X->nc[0], &X->cap_nc[0], ndep))) return e;
-        if ((e = x_ensure(X, &X->nc[1], &X->cap_nc[1], ndep))) return e;
-        if ((e = x_ensure(X, &X->flags, &X->cap_flags, ndep))) return e;
+        CK(X->k1b.grow(ndep, s));
+        CK(X->k2b.grow(ndep, s));
+        CK(X->idx[0].grow(ndep, s));
+        CK(X->idx[1].grow(ndep, s));
+        CK(X->deps.grow(ndep, s));
+        CK(X->nc[0].grow(ndep, s));
+        CK(X->nc[1].grow(ndep, s));
+        CK(X->flags.grow(ndep, s));
         if (shift) {
-          if ((e = x_sort_pairs(X, X->k1, X->k1b, X->dv, X->deps, ndep, s))) return e;
+          if ((r = x_sort_pairs(X, X->k1, X->k1b, X->dv, X->deps, ndep, s))) return r;
           *launches += 1;
         } else {
           k_x_iota<<<nblk(ndep), 256, 0, s>>>(X->idx[0], ndep);
-          if ((e = x_sort_pairs(X, X->k2, X->k2b, X->idx[0], X->idx[1], ndep, s))) return e;
+          if ((r = x_sort_pairs(X, X->k2, X->k2b, X->idx[0], X->idx[1], ndep, s))) return r;
           k_x_gather64<<<nblk(ndep), 256, 0, s>>>(X->k1, X->idx[1], ndep, X->k1b);
-          if ((e = x_sort_pairs(X, X->k1b, X->k2b, X->idx[1], X->idx[0], ndep, s))) return e;
+          if ((r = x_sort_pairs(X, X->k1b, X->k2b, X->idx[1], X->idx[0], ndep, s))) return r;
           k_x_gather32<<<nblk(ndep), 256, 0, s>>>(X->dv, X->idx[0], ndep, X->deps);
           *launches += 5;
         }
-        if ((e = x_ensure(X, &X->flags2, &X->cap_flags2, ndep))) return e;
+        CK(X->flags2.grow(ndep, s));
         k_x_set_ord<<<nblk(ndep), 256, 0, s>>>(X->deps, ndep, scratch, X->nc[0], X->flags2);
         *launches += 1;
         ndep_run = ndep; ls_deps = X->tclock;                // the fixpoint and the hand-over to E[0] run inside k_x_relax
@@ -332,27 +292,27 @@ cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, ui
   st->generations = 0;
   if (xdbg) { cudaStreamSynchronize(s); fprintf(stderr, "[x] seeds+deletes %.2f ms (reseed rounds %u, dependants %u)\n", ms(t_begin, now()), st->reseed_rounds, st->dependants); }
   if (nE || ndep_run) {
-    if (xdbg && !X->d_dbg) XCK(cudaMalloc((void **)&X->d_dbg, FB_X_DBG_WORDS * 8));
-    if (xdbg) XCK(cudaMemsetAsync(X->d_dbg, 0, FB_X_DBG_WORDS * 8, s));
-    if (X->sclock > 0xf0000000u) { XCK(cudaMemsetAsync(X->SUMg, 0, P * 4, s)); X->sclock = 0; }       // stamp wrap-around
+    if (xdbg && !X->d_dbg) CK(X->d_dbg.alloc(FB_X_DBG_WORDS));
+    if (xdbg) CK(cudaMemsetAsync(X->d_dbg, 0, FB_X_DBG_WORDS * 8, s));
+    if (X->sclock > 0xf0000000u) { CK(cudaMemsetAsync(X->SUMg, 0, P * 4, s)); X->sclock = 0; }       // stamp wrap-around
     if (X->gen_id > 0xf0000000u) X->gen_id = 0;
-    if (X->wclock > 0xf0000000u) { XCK(cudaMemsetAsync(X->wstamp, 0, P * 4, s)); X->wclock = 0; }
+    if (X->wclock > 0xf0000000u) { CK(cudaMemsetAsync(X->wstamp, 0, P * 4, s)); X->wclock = 0; }
     FbXCtl *h = X->h_ctl;
     memset(h, 0, sizeof(*h));
     h->gen_id = X->gen_id; h->wclock = X->wclock; h->tclock = X->tclock; h->sclock = X->sclock;
-    XCK(cudaMemcpyAsync(X->d_ctl, h, sizeof(FbXCtl), cudaMemcpyHostToDevice, s));
-    XCK(fb_xrelax_launch(X, g, cobs, nE, X->deps, ndep_run, scratch, X->nc[0], X->flags2, occbits, ls_deps, xdbg ? X->d_dbg : nullptr, s));
+    CK(cudaMemcpyAsync(X->d_ctl, h, sizeof(FbXCtl), cudaMemcpyHostToDevice, s));
+    CK(fb_xrelax_launch(X, g, cobs, nE, X->deps, ndep_run, scratch, X->nc[0], X->flags2, occbits, ls_deps, xdbg ? X->d_dbg.p : nullptr, s));
     if (ndep_run) k_x_unset<<<nblk(ndep_run), 256, 0, s>>>(X->deps, ndep_run, scratch);
-    XCK(cudaMemcpyAsync(h, X->d_ctl, sizeof(FbXCtl), cudaMemcpyDeviceToHost, s));
-    XCK(cudaStreamSynchronize(s));
+    CK(cudaMemcpyAsync(h, X->d_ctl, sizeof(FbXCtl), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
     *launches += 1;
-    if (h->err) { snprintf(X->err, sizeof(X->err), h->err == 1u ? "exact mode: generation with more than 2^27 entries" : "exact mode: behaviour fixpoint did not converge"); return cudaErrorInvalidValue; }
+    if (h->err) { fb_set_error(h->err == 1u ? "exact mode: generation with more than 2^27 entries" : "exact mode: behaviour fixpoint did not converge"); return FIESTA_ERR_CUDA; }
     X->gen_id = h->gen_id; X->wclock = h->wclock; X->tclock = h->tclock; X->sclock = h->sclock;
     st->generations = h->generations; st->reseed_rounds = h->reseed_rounds; st->eval_rounds = h->rounds; st->dense_rounds = h->dense_rounds;
     st->voxels_changed = h->voxels_changed; st->expansions = h->expansions;
     if (xdbg) {
       static unsigned long long hd[FB_X_DBG_WORDS];
-      XCK(cudaMemcpy(hd, X->d_dbg, sizeof(hd), cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(hd, X->d_dbg, sizeof(hd), cudaMemcpyDeviceToHost));
       static const char *cat[14] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top", "empty-barrier", "reseed.rounds", "reseed.assemble"};
       fprintf(stderr, "[x] reseed rounds %u; phases (us, count):", st->reseed_rounds);
       for (int c = 0; c < 14; ++c) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[3 * 1024 + 2 * c] / 1965.0, hd[3 * 1024 + 2 * c + 1]);
@@ -365,5 +325,5 @@ cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, ui
     }
   }
   X->scratch_clean = scratch_ok;                             // every sparse write above has its undo queued behind it
-  return cudaSuccess;
+  return FIESTA_OK;
 }

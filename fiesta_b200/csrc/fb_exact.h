@@ -24,46 +24,47 @@ struct FbXCtl {
   unsigned partial[FB_X_MAX_BLOCKS];  // winners per CTA range (ordered hand-over)
 };
 
+// Order-exact state of one map.  Zero until fb_exact_init; freed with the map.
 struct FbExact {
-  unsigned long long *MB;      // per voxel: {parity | queue position | behaviour | code} of its live entry in the current generation
-  unsigned long long *LS;      // per voxel: time of the last relink into a dependant list
-  unsigned long long *tkey;    // per voxel: epoch-coded serial time of the first pending observation (fb_touch, fb_common.cuh)
-  uint32_t *touched;           // [ptotal] staging of the voxels whose occupancy crossed the threshold (inserts; deletes use emask)
-  unsigned long long tclock;   // relink clock
-  unsigned long long key_base; // observation clock within the current integration epoch
-  unsigned long long key_hi;   // key_epoch << FB_KEY_BITS
-  unsigned key_epoch;          // integration epoch (one per UpdateOccupancy)
-  unsigned *d_count, *d_flag, *h_count;
-  bool scratch_clean;           // the per-voxel scratch word array of UpdateESDF is all-XNONE
-  uint4 *SUM;                  // per voxel offer summary of the current generation: {first ts, best ts, best code, snapshot code}
-  uint32_t *SUMg;              // per voxel: summary pass for which SUM was computed (each target is claimed once per pass)
-  unsigned gen_id, wclock, sclock;
-  uint32_t *emask;             // per entry: slots it owns in the next generation
-  uint32_t *W[3], *F[3];       // work lists / flip lists, rotating per round
-  uint32_t *wstamp;            // per entry: round for which it is already in a work list
-  uint32_t *slotc;             // SMALL generations: codes of the owned slots
-  unsigned dense_min;          // work lists longer than this are evaluated through refreshed summaries (one wave of warps)
-  unsigned small_max;          // generations up to this many entries run without summaries
-  FbXCtl *d_ctl, *h_ctl;
-  unsigned long long *d_dbg;
-  int relax_blocks;
-  uint32_t *E[2]; size_t cap_E[2];
-  uint32_t *sel; size_t cap_sel;
-  unsigned long long *k1, *k2, *k1b, *k2b; size_t cap_k1, cap_k2, cap_k1b, cap_k2b;
-  uint32_t *dv, *idx[2], *deps, *nc[2]; size_t cap_dv, cap_idx[2], cap_deps, cap_nc[2];
-  uint8_t *flags, *flags2; size_t cap_flags, cap_flags2;
-  void *cub_tmp; size_t cub_bytes;
-  char err[256];
+  FbDevBuf<unsigned long long> MB;    // per voxel: {parity | queue position | behaviour | code} of its live entry in the current generation
+  FbDevBuf<unsigned long long> LS;    // per voxel: time of the last relink into a dependant list
+  FbDevBuf<unsigned long long> tkey;  // per voxel: epoch-coded serial time of the first pending observation (fb_touch, fb_common.cuh)
+  FbDevBuf<uint32_t> touched;         // [ptotal] staging of the voxels whose occupancy crossed the threshold (inserts; deletes use emask)
+  unsigned long long tclock = 0;      // relink clock
+  unsigned long long key_base = 0;    // observation clock within the current integration epoch
+  unsigned long long key_hi = 0;      // key_epoch << FB_KEY_BITS
+  unsigned key_epoch = 0;             // integration epoch (one per UpdateOccupancy)
+  FbDevBuf<unsigned> d_count, d_flag;
+  FbHostBuf<unsigned> h_count;
+  bool scratch_clean = false;         // the per-voxel scratch word array of UpdateESDF is all-XNONE
+  FbDevBuf<uint4> SUM;                // per voxel offer summary of the current generation: {first ts, best ts, best code, snapshot code}
+  FbDevBuf<uint32_t> SUMg;            // per voxel: summary pass for which SUM was computed (each target is claimed once per pass)
+  unsigned gen_id = 0, wclock = 0, sclock = 0;
+  FbDevBuf<uint32_t> emask;           // per entry: slots it owns in the next generation
+  FbDevBuf<uint32_t> W[3], F[3];      // work lists / flip lists, rotating per round
+  FbDevBuf<uint32_t> wstamp;          // per entry: round for which it is already in a work list
+  FbDevBuf<uint32_t> slotc;           // SMALL generations: codes of the owned slots
+  unsigned dense_min = 0;             // work lists longer than this are evaluated through refreshed summaries (one wave of warps)
+  unsigned small_max = 0;             // generations up to this many entries run without summaries
+  FbDevBuf<FbXCtl> d_ctl;
+  FbHostBuf<FbXCtl> h_ctl;
+  FbDevBuf<unsigned long long> d_dbg;
+  int relax_blocks = 0;
+  FbDevBuf<uint32_t> E[2], sel;
+  FbDevBuf<unsigned long long> k1, k2, k1b, k2b;
+  FbDevBuf<uint32_t> dv, idx[2], deps, nc[2];
+  FbDevBuf<uint8_t> flags, flags2;
+  FbDevBuf<char> cub_tmp;
 };
 
-cudaError_t fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t s);
-void fb_exact_free(FbExact *X);
-cudaError_t fb_exact_queue_crossings(FbExact *X, const unsigned long long *ins_key, const uint32_t *ins_vox, const unsigned long long *del_key,
-                                     const uint32_t *del_vox, uint32_t **ins, size_t *cap_ins, unsigned *n_ins, uint32_t **del, size_t *cap_del,
-                                     unsigned *n_del, cudaStream_t s, int *launches);
-cudaError_t fb_exact_next_epoch(FbExact *X, const FbGeom &g, cudaStream_t s);
-cudaError_t fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *scratch, const double *occ, const uint32_t *occbits, double l_occ,
-                                 const uint32_t *ins, unsigned n_ins, const uint32_t *del, unsigned n_del, cudaStream_t s, FbExactStats *st, int *launches);
+// Host functions return FIESTA_OK or a FIESTA_ERR_* code and set fiesta_last_error().
+int fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t s);
+int fb_exact_queue_crossings(FbExact *X, const unsigned long long *ins_key, const uint32_t *ins_vox, const unsigned long long *del_key,
+                             const uint32_t *del_vox, FbDevBuf<uint32_t> &ins, unsigned *n_ins, FbDevBuf<uint32_t> &del, unsigned *n_del,
+                             cudaStream_t s, int *launches);
+int fb_exact_next_epoch(FbExact *X, const FbGeom &g, cudaStream_t s);
+int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *scratch, const double *occ, const uint32_t *occbits, double l_occ,
+                         const uint32_t *ins, unsigned n_ins, const uint32_t *del, unsigned n_del, cudaStream_t s, FbExactStats *st, int *launches);
 // fb_xrelax.cu
 cudaError_t fb_xrelax_init();
 int fb_xrelax_blocks(int device);

@@ -79,4 +79,8 @@ FB_HD bool fb_pos_in_map(const FbGeom &g, const double *p) {
   if (p[0] > g.max_range[0] || p[1] > g.max_range[1] || p[2] > g.max_range[2]) return false;
   return true;
 }
+// ESDFMap::Pos2Vox (ESDFMap.cpp:74-77)
+FB_HD void fb_pos2vox(const FbGeom &g, const double *p, int *v) {
+  for (int k = 0; k < 3; ++k) v[k] = (int)floor((p[k] - g.origin[k]) / g.res);
+}
 #endif

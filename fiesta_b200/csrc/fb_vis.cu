@@ -23,12 +23,7 @@ __global__ void k_vis_occ_points(FbGeom g, const uint32_t *sel, unsigned n, floa
   for (int k = 0; k < 3; ++k) out[3 * i + k] = (float)((v[k] + 0.5) * g.res + g.origin[k]);   // Vox2Pos (:79-82), Point32 is float
 }
 __device__ __forceinline__ double fb_slice_dist(const FbGeom &g, const uint32_t *cobs, int x, int y, int z) {
-  const uint32_t raw = cobs[fb_ii(g, x, y, z)], c = raw & FB_CODE_MASK;
-  if (c == FB_UNKNOWN) return -10000.0;
-  if (c == FB_INF || (raw & FB_DINF)) return 10000.0;
-  int ox, oy, oz; fb_unpack(c, ox, oy, oz);
-  const double dx = (double)(ox - x), dy = (double)(oy - y), dz = (double)(oz - z);
-  return sqrt((dx * dx + dy * dy) + dz * dz) * g.res;
+  return fb_record_distance(cobs[fb_ii(g, x, y, z)], x, y, z, g.res);
 }
 __global__ void k_vis_slice_flags(FbGeom g, const uint32_t *cobs, int slice, uint8_t *flags) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -67,59 +62,66 @@ __global__ void k_vis_slice_points(FbGeom g, const uint32_t *cobs, const uint32_
   rgba[4 * i] = (float)r; rgba[4 * i + 1] = (float)gg; rgba[4 * i + 2] = (float)b; rgba[4 * i + 3] = 1.0f;
 }
 
-static cudaError_t vis_select(const uint8_t *flags, size_t n, uint32_t *sel, unsigned *count, cudaStream_t s) {
-  unsigned *d_cnt = nullptr; void *tmp = nullptr; size_t bytes = 0;
-  cudaError_t e = cudaMalloc((void **)&d_cnt, 4);
-  if (e) return e;
+static int vis_select(const uint8_t *flags, size_t n, uint32_t *sel, unsigned *count, cudaStream_t s) {
+  FbDevBuf<unsigned> d_cnt;
+  FbDevBuf<char> tmp;
+  size_t bytes = 0;
   thrust::counting_iterator<uint32_t> it(0);
-  e = cub::DeviceSelect::Flagged(nullptr, bytes, it, flags, sel, d_cnt, (int)n, s);
-  if (!e) e = cudaMalloc(&tmp, bytes ? bytes : 16);
-  if (!e) e = cub::DeviceSelect::Flagged(tmp, bytes, it, flags, sel, d_cnt, (int)n, s);
-  if (!e) e = cudaMemcpyAsync(count, d_cnt, 4, cudaMemcpyDeviceToHost, s);
-  if (!e) e = cudaStreamSynchronize(s);
-  cudaFree(tmp); cudaFree(d_cnt);
-  return e;
+  CK(d_cnt.alloc(1));
+  CK(cub::DeviceSelect::Flagged(nullptr, bytes, it, flags, sel, d_cnt.p, (int)n, s));
+  CK(tmp.alloc(bytes ? bytes : 16));
+  CK(cub::DeviceSelect::Flagged(tmp.p, bytes, it, flags, sel, d_cnt.p, (int)n, s));
+  CK(cudaMemcpyAsync(count, d_cnt, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return FIESTA_OK;
 }
 
-cudaError_t fb_vis_point_cloud(const FbGeom &g, const double *occ, double l_occ, int zlo, int zhi, float *h_out, long long cap, long long *count, cudaStream_t s) {
+int fb_vis_point_cloud(const FbGeom &g, const double *occ, double l_occ, int zlo, int zhi, float *h_out, long long cap, long long *count, cudaStream_t s) {
   const size_t G = (size_t)g.total;
-  uint8_t *flags = nullptr; uint32_t *sel = nullptr; float *pts = nullptr;
-  cudaError_t e = cudaMalloc((void **)&flags, G);
-  if (!e) e = cudaMalloc((void **)&sel, G * 4);
+  FbDevBuf<uint8_t> flags;
+  FbDevBuf<uint32_t> sel;
+  FbDevBuf<float> pts;
   unsigned n = 0;
-  if (!e) { k_vis_occ_flags<<<(unsigned)((G + 255) / 256), 256, 0, s>>>(g, occ, l_occ, zlo, zhi, flags); e = vis_select(flags, G, sel, &n, s); }
+  int r;
+  *count = 0;
+  CK(flags.alloc(G));
+  CK(sel.alloc(G));
+  k_vis_occ_flags<<<(unsigned)((G + 255) / 256), 256, 0, s>>>(g, occ, l_occ, zlo, zhi, flags);
+  if ((r = vis_select(flags, G, sel, &n, s))) return r;
   *count = n;
   const unsigned m = (long long)n < cap ? n : (unsigned)(cap < 0 ? 0 : cap);
-  if (!e && m) {
-    e = cudaMalloc((void **)&pts, (size_t)m * 12);
-    if (!e) { k_vis_occ_points<<<(m + 255) / 256, 256, 0, s>>>(g, sel, m, pts); e = cudaMemcpyAsync(h_out, pts, (size_t)m * 12, cudaMemcpyDeviceToHost, s); }
-    if (!e) e = cudaStreamSynchronize(s);
+  if (m) {
+    CK(pts.alloc((size_t)m * 3));
+    k_vis_occ_points<<<(m + 255) / 256, 256, 0, s>>>(g, sel, m, pts);
+    CK(cudaMemcpyAsync(h_out, pts, (size_t)m * 12, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
   }
-  cudaFree(flags); cudaFree(sel); cudaFree(pts);
-  return e;
+  return FIESTA_OK;
 }
 
-cudaError_t fb_vis_slice(const FbGeom &g, const uint32_t *cobs, int slice, double max_dist, double *h_xyz, float *h_rgba, long long cap, long long *count, cudaStream_t s) {
+int fb_vis_slice(const FbGeom &g, const uint32_t *cobs, int slice, double max_dist, double *h_xyz, float *h_rgba, long long cap, long long *count, cudaStream_t s) {
   *count = 0;
-  if (slice < 0 || slice >= g.gz) return cudaSuccess;
+  if (slice < 0 || slice >= g.gz) return FIESTA_OK;
   const size_t G = (size_t)g.gx * g.gy;
-  uint8_t *flags = nullptr; uint32_t *sel = nullptr; double *xyz = nullptr; float *rgba = nullptr;
-  cudaError_t e = cudaMalloc((void **)&flags, G);
-  if (!e) e = cudaMalloc((void **)&sel, G * 4);
+  FbDevBuf<uint8_t> flags;
+  FbDevBuf<uint32_t> sel;
+  FbDevBuf<double> xyz;
+  FbDevBuf<float> rgba;
   unsigned n = 0;
-  if (!e) { k_vis_slice_flags<<<(unsigned)((G + 255) / 256), 256, 0, s>>>(g, cobs, slice, flags); e = vis_select(flags, G, sel, &n, s); }
+  int r;
+  CK(flags.alloc(G));
+  CK(sel.alloc(G));
+  k_vis_slice_flags<<<(unsigned)((G + 255) / 256), 256, 0, s>>>(g, cobs, slice, flags);
+  if ((r = vis_select(flags, G, sel, &n, s))) return r;
   *count = n;
   const unsigned m = (long long)n < cap ? n : (unsigned)(cap < 0 ? 0 : cap);
-  if (!e && m) {
-    e = cudaMalloc((void **)&xyz, (size_t)m * 24);
-    if (!e) e = cudaMalloc((void **)&rgba, (size_t)m * 16);
-    if (!e) {
-      k_vis_slice_points<<<(m + 255) / 256, 256, 0, s>>>(g, cobs, sel, m, slice, max_dist, xyz, rgba);
-      e = cudaMemcpyAsync(h_xyz, xyz, (size_t)m * 24, cudaMemcpyDeviceToHost, s);
-      if (!e) e = cudaMemcpyAsync(h_rgba, rgba, (size_t)m * 16, cudaMemcpyDeviceToHost, s);
-    }
-    if (!e) e = cudaStreamSynchronize(s);
+  if (m) {
+    CK(xyz.alloc((size_t)m * 3));
+    CK(rgba.alloc((size_t)m * 4));
+    k_vis_slice_points<<<(m + 255) / 256, 256, 0, s>>>(g, cobs, sel, m, slice, max_dist, xyz, rgba);
+    CK(cudaMemcpyAsync(h_xyz, xyz, (size_t)m * 24, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(h_rgba, rgba, (size_t)m * 16, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
   }
-  cudaFree(flags); cudaFree(sel); cudaFree(xyz); cudaFree(rgba);
-  return e;
+  return FIESTA_OK;
 }
