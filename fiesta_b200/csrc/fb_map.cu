@@ -546,7 +546,9 @@ int fiesta_raycast_frame_device(fiesta_map *m, const float *d_xyz, int64_t n, co
   // Lattice fast path: the DDA walks floor(world/res) voxels while the map uses floor((world-origin)/res) (ESDFMap.cpp:74-77).
   // If, for every DDA coordinate c inside the box and every axis, the voxel centre (c+0.5)*res lies in the map and maps to
   // c - off (checked here with the reference's own fp64 expressions), the per-voxel divisions can be skipped exactly.
-  a.lattice_ok = 1;
+  // FIESTA_RAY_LATTICE=0 (read on every call, tests: run any scene through the general per-voxel path) turns it off.
+  const char *lat_env = getenv("FIESTA_RAY_LATTICE");
+  a.lattice_ok = (lat_env && strcmp(lat_env, "0") == 0) ? 0 : 1;
   for (int k = 0; k < 3 && a.lattice_ok; ++k) {
     const int G = k == 0 ? g.gx : (k == 1 ? g.gy : g.gz);
     const long long clo = (long long)ceil(a.bmin[k]), chi = (long long)ceil(a.bmax[k]);   // integers c with bmin <= c < bmax

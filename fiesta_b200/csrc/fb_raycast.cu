@@ -227,10 +227,14 @@ __global__ void k_ray_trace(FbGeom g, FbRayArgs a) {
 // stopped at a voxel stamped by an earlier ray (that voxel is still counted, Fiesta.h:248-268).
 #define FB_REACH_BLOCKED 0x40000000
 
-// Is the voxel whose claim word is `seen` validly claimed by a ray with a lower index than `i`?
-__device__ __forceinline__ bool fb_claim_blocks(const FbRayArgs &a, unsigned seen, unsigned i) {
+// Does the voxel whose claim word is `seen` stop ray `i` at walk position `t`?  It does when a ray with a lower index than
+// `i` validly claims it, or when ray `i` itself claimed it at an earlier position of its walk: off the lattice fast path two
+// DDA voxels of one ray can have the same map voxel (their centres lie on a map voxel face and Pos2Vox sends both to one
+// side), and the reference's walk stops at the second one because it stamped set_free_ there itself (Fiesta.h:265-273).
+__device__ __forceinline__ bool fb_claim_blocks(const FbRayArgs &a, unsigned seen, unsigned i, int t) {
   if ((seen >> FB_CLAIM_FRAME_SHIFT) != a.frame_tag) return false;                       // claim of an older frame
   const unsigned j = (seen >> FB_POS_BITS) & FB_RAY_MASK, tj = seen & FB_POS_MASK;
+  if (j == i) return (int)tj < t;                                                        // stamped by this ray, earlier
   return j < i && (int)tj < (__ldcg(&a.ray_reach[j]) & ~FB_REACH_BLOCKED);               // set_free_[idx] == tt by an EARLIER ray
 }
 
@@ -259,7 +263,11 @@ __device__ __forceinline__ int fb_walk_ray(const FbRayArgs &a, unsigned i, unsig
     const bool normal = cls == FB_CLS_COUNT || cls == FB_CLS_STAMP;
     const unsigned mine = fr | (i << FB_POS_BITS) | (unsigned)t;
     int st = 0;                           // 0 = passable & already mine, 1 = passable & must be claimed, 2 = blocked
-    if (normal && seen != mine) st = fb_claim_blocks(a, seen, i) ? 2 : 1;
+    if (normal && seen != mine) st = fb_claim_blocks(a, seen, i, t) ? 2 : 1;
+    if (!a.lattice_ok) {                  // the same map voxel at a lower position of this chunk stamps it first: blocked
+      const unsigned same = __match_any_sync(0xffffffffu, normal ? ii : (0x80000000u | lane));
+      if (normal && (same & ((1u << lane) - 1u))) st = 2;
+    }
     const unsigned m = __ballot_sync(0xffffffffu, st == 2 || cls == FB_CLS_STOP);
     const int first = m ? (__ffs(m) - 1) : 32;
     while (st == 1 && (int)lane < first) {                    // claim; a failed CAS means someone else wrote: look again
@@ -274,7 +282,7 @@ __device__ __forceinline__ int fb_walk_ray(const FbRayArgs &a, unsigned i, unsig
       }
       seen = old;
       if (seen == mine) { st = 0; break; }
-      if (fb_claim_blocks(a, seen, i)) { st = 2; break; }
+      if (fb_claim_blocks(a, seen, i, t)) { st = 2; break; }
     }
     const unsigned m2 = __ballot_sync(0xffffffffu, st == 2 || cls == FB_CLS_STOP);
     if (m2) {
@@ -338,7 +346,7 @@ __global__ void __launch_bounds__(RR_THREADS, 1) k_ray_resolve(FbGeom g, FbRayAr
             if (dp < (unsigned)rpos) { need = true; start = (int)dp; }   // (a displaced claim beyond the reach was stale anyway)
             else if (rr & FB_REACH_BLOCKED) {
               const unsigned e = __ldcg(&a.ray_list[i * a.cap + (L - 1 - rpos)]);
-              need = !fb_claim_blocks(a, __ldcg(&claims[e & FB_LIST_IDX_MASK]), (unsigned)i);
+              need = !fb_claim_blocks(a, __ldcg(&claims[e & FB_LIST_IDX_MASK]), (unsigned)i, rpos);
               start = rpos;
             }
           }

@@ -119,7 +119,10 @@ int fiesta_set_occupancy_batch_vox_device(fiesta_map *m, const int *d_vox_xyz, c
  * the frame's counters are complete (the call reads back the frame statistics).
  * Limits (FIESTA_ERR_LIMIT, nothing is truncated): n <= 524286 points per call (split larger clouds into ordered sub-frames);
  * 1500 voxels per ray as in the reference (raycast.cpp:127-130); EXACT mode: at most 16383 frames between two
- * fiesta_update_occupancy calls (observation time stamps are 44 bits per integration epoch). */
+ * fiesta_update_occupancy calls (observation time stamps are 44 bits per integration epoch).
+ * The environment variable FIESTA_RAY_LATTICE=0, read on every call, turns off the lattice fast path (per-voxel Pos2Vox
+ * skipped when the map's voxels line up with the DDA's, DESIGN.md 3.1) so that tests can run any map through the general
+ * per-voxel path; the results are the same either way. */
 int fiesta_raycast_frame(fiesta_map *m, const float *xyz, int64_t n, const double T[16], const fiesta_raycast_params *p);
 int fiesta_raycast_frame_device(fiesta_map *m, const float *d_xyz, int64_t n, const double T[16],
                                 const fiesta_raycast_params *p);
