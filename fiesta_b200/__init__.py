@@ -42,6 +42,11 @@ class ShardInfo(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("rank", "world", "x_begin", "x_end", "has_lo", "has_hi")] + [("layer_words", C.c_int64)]
 
 
+class NavStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("box_voxels", "blocked", "reached", "goals_placed", "generations", "tile_visits")] + [
+        ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
+
+
 class Stats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
         "occupancy_updates", "inserts", "deletes", "voxels_changed", "expansions", "voxels_reset", "tile_visits", "generations",
@@ -70,6 +75,7 @@ SYMBOLS = [
     "fiesta_host_mirror_get_dist_grad_trilinear_batch", "fiesta_host_mirror_records", "fiesta_host_mirror_stats",
     "fiesta_check_segments", "fiesta_check_segments_device", "fiesta_get_distance_batch_device",
     "fiesta_get_dist_grad_trilinear_batch_device", "fiesta_host_mirror_check_segments",
+    "fiesta_nav_create", "fiesta_nav_destroy", "fiesta_nav_compute", "fiesta_nav_export", "fiesta_nav_paths",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -121,6 +127,12 @@ def load_library():
         L.fiesta_check_segments.argtypes = seg
         L.fiesta_host_mirror_check_segments.argtypes = seg
         L.fiesta_check_segments_device.argtypes = seg + [C.c_void_p]
+        L.fiesta_nav_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+        L.fiesta_nav_destroy.argtypes = [C.c_void_p]
+        L.fiesta_nav_destroy.restype = None
+        L.fiesta_nav_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_int, C.c_void_p]
+        L.fiesta_nav_export.argtypes = [C.c_void_p, C.c_void_p]
+        L.fiesta_nav_paths.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 4
         L.fiesta_get_distance_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
         L.fiesta_get_dist_grad_trilinear_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
@@ -225,6 +237,54 @@ class HostMirror:
     def close(self):
         if self._h:
             self._m._L.fiesta_host_mirror_destroy(self._h)
+            self._h = None
+
+
+class NavField:
+    """fiesta_nav_field: cost-to-go field of a voxel box -- geodesic distance to a goal set through free space at a clearance --
+    and path extraction down it.  The buffers grow to the largest box computed; close() it before the map."""
+
+    def __init__(self, m):
+        self._m = m
+        h = C.c_void_p()
+        m._ck(m._L.fiesta_nav_create(m._h, C.byref(h)), "fiesta_nav_create")
+        self._h = h
+        self.shape = None
+
+    def compute(self, box_lo, box_hi, goals, clearance, unknown_blocks=False):
+        """Field over the inclusive voxel box [box_lo, box_hi] for goals (n, 3) in metres -> stats dict."""
+        lo, hi = np.ascontiguousarray(box_lo, dtype=np.int32), np.ascontiguousarray(box_hi, dtype=np.int32)
+        if lo.shape != (3,) or hi.shape != (3,):
+            raise ValueError("NavField.compute: box_lo and box_hi must be 3 voxel coordinates each")
+        goals = _f64(goals).reshape(-1, 3)
+        st = NavStats()
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        self._m._ck(self._m._L.fiesta_nav_compute(self._h, lo.ctypes, hi.ctypes, goals.ctypes, C.c_int64(len(goals)), r, flags, C.byref(st)),
+                    "NavField.compute")
+        self.shape = tuple(int(b - a + 1) for a, b in zip(lo, hi))
+        return {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved_f"}
+
+    def export(self):
+        """The last computed field as a (Bx, By, Bz) float64 array: -1 blocked, +inf unreachable."""
+        if self.shape is None:
+            raise FiestaError("NavField.export: no field has been computed")
+        out = np.empty(self.shape)
+        self._m._ck(self._m._L.fiesta_nav_export(self._h, out.ctypes), "NavField.export")
+        return out
+
+    def paths(self, starts, max_len):
+        """Paths from starts (n, 3) in metres -> (status (n,), len (n,), cost (n,), vox (n, max_len, 3) grid voxels, -1 past len)."""
+        starts = _f64(starts).reshape(-1, 3)
+        n = len(starts)
+        st, ln, cost = np.empty(n, np.int32), np.empty(n, np.int32), np.empty(n)
+        vox = np.empty((n, int(max_len), 3), np.int32)
+        self._m._ck(self._m._L.fiesta_nav_paths(self._h, starts.ctypes, C.c_int64(n), C.c_int32(int(max_len)), st.ctypes, ln.ctypes,
+                                                cost.ctypes, vox.ctypes), "NavField.paths")
+        return st, ln, cost, vox
+
+    def close(self):
+        if self._h:
+            self._m._L.fiesta_nav_destroy(self._h)
             self._h = None
 
 
@@ -393,6 +453,10 @@ class ESDFMap:
     def HostMirror(self):
         """Pinned host copy of the distance records, patched by refresh() with the records UpdateESDF changed (fiesta_host_mirror_*)."""
         return HostMirror(self)
+
+    def NavField(self):
+        """Cost-to-go field of a voxel box through free space at a clearance, with path extraction (fiesta_nav_*)."""
+        return NavField(self)
 
     def RaycastFrame(self, xyz, T, min_ray_length, max_ray_length):
         """xyz: (n,3) float32 host array, or an integer device pointer paired with `n` as a tuple (ptr, n)."""

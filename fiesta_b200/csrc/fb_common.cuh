@@ -21,6 +21,7 @@
 #include <stdint.h>
 #include "fb_host.h"     // FbDevBuf, CK
 #include "fb_record.h"   // FB_UNKNOWN / FB_INF / FB_DINF / FB_CODE_MASK, FbGeom, fb_pack / fb_unpack, fb_ii, the distance read
+#include "fb_nav.h"      // FbNavBox (cost-to-go field)
 
 // SMs of an H100 SXM: fixed-size grid-stride launches are sized to a multiple of it.
 #define FB_SMS 132
@@ -178,6 +179,27 @@ int fb_vis_point_cloud(const FbGeom &g, const double *occ, double l_occ, int zlo
 cudaError_t fb_segment_clearance(const FbGeom &g, const uint32_t *cobs, const double *ab, long long n, double r, int unknown_blocks,
                                  int32_t *status, int64_t *hit_idx, double *hit_t, double *min_dist, cudaStream_t s);
 int fb_vis_slice(const FbGeom &g, const uint32_t *cobs, int slice, double max_dist, double *h_xyz, float *h_rgba, long long cap, long long *count, cudaStream_t s);
+// cost-to-go field (fb_nav.cu)
+struct FbNavCtr {
+  unsigned n[3];               // tile work-list lengths, rotating by generation (k_nav_relax)
+  unsigned next[3];            // dynamic tile fetch counters, rotating the same way
+  unsigned generations, pad;
+  unsigned long long goals_placed, blocked, reached, tile_visits;
+};
+struct FbNavArgs {
+  double *D;                   // the field, box layout (fb_nav.h)
+  FbNavBox b;
+  int tn[3];                   // 8^3 tiles per box axis
+  double w[3];                 // res * sqrt(1), res * sqrt(2), res * sqrt(3)
+  uint32_t *stamp;             // per tile: stamp of the generation it is queued for (generation g has stamp g + 1)
+  uint32_t *list[2];           // tile work lists by generation parity
+  FbNavCtr *ctr;
+};
+cudaError_t fb_nav_compute(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, const double *goals, long long n_goals, double r,
+                           int unknown_blocks, int nblocks, cudaStream_t s);
+int fb_nav_relax_blocks(int device);
+cudaError_t fb_nav_paths(const FbGeom &g, const FbNavBox &b, const double *D, const double *w, const double *starts, long long n, int max_len,
+                         int32_t *status, int32_t *len, double *cost, int32_t *vox, cudaStream_t s);
 struct FbDepthRel { double m[16]; };
 struct fiesta_depth_params;
 cudaError_t fb_depth_to_cloud(const uint16_t *d_img, const uint16_t *d_last, int rows, int cols, const fiesta_depth_params &p, int filter_on,

@@ -939,6 +939,142 @@ int fiesta_check_segments_device(fiesta_map *m, const double *d_ab, int64_t n, d
   return device_query_end(m, s);
 }
 
+// ---- cost-to-go field (fb_nav.h, fb_nav.cu): a box's geodesic distance to a goal set through free space at a clearance
+struct fiesta_nav_field {
+  fiesta_map *m = nullptr;
+  int blocks = 0;                   // co-resident CTAs of k_nav_relax (cooperative launch)
+  FbDevBuf<double> D, d_goals;
+  FbDevBuf<uint32_t> stamp, list[2];
+  FbDevBuf<FbNavCtr> ctr;
+  FbHostBuf<FbNavCtr> h_ctr;
+  FbDevBuf<double> d_pd;            // fiesta_nav_paths: [starts 3n][cost n]
+  FbDevBuf<int32_t> d_pi;           //                   [status n][len n][vox 3 n max_len]
+  cudaEvent_t ev[2] = {};
+  FbNavBox box{};
+  double w[3]{};
+  bool valid = false;               // D holds a field computed for `box`
+};
+void fiesta_nav_destroy(fiesta_nav_field *f) {
+  if (!f) return;
+  cudaSetDevice(f->m->device);
+  cudaStreamSynchronize(f->m->stream);
+  for (cudaEvent_t e : f->ev) if (e) cudaEventDestroy(e);
+  delete f;
+}
+int fiesta_nav_create(fiesta_map *m, fiesta_nav_field **out) {
+  if (!m || !out) { fb_set_error("fiesta_nav_create: null argument"); return FIESTA_ERR_INVALID; }
+  *out = nullptr;
+  CK(cudaSetDevice(m->device));
+  std::unique_ptr<fiesta_nav_field, void (*)(fiesta_nav_field *)> f(new (std::nothrow) fiesta_nav_field(), fiesta_nav_destroy);
+  if (!f) { fb_set_error("out of host memory"); return FIESTA_ERR_INVALID; }
+  f->m = m;
+  f->blocks = fb_nav_relax_blocks(m->device);
+  if (f->blocks <= 0) { fb_set_error("fiesta_nav_create: the relaxation kernel does not fit on this device"); return FIESTA_ERR_CUDA; }
+  for (cudaEvent_t &e : f->ev) CK(cudaEventCreate(&e));
+  CK(f->ctr.alloc(1));
+  CK(f->h_ctr.alloc(1));
+  for (int k = 0; k < 3; ++k) f->w[k] = m->g.res * sqrt((double)(k + 1));
+  *out = f.release();
+  return FIESTA_OK;
+}
+int fiesta_nav_compute(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *goals_xyz, int64_t n_goals,
+                       double clearance, int flags, fiesta_nav_stats *stats) {
+  const char *fn = "fiesta_nav_compute";
+  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (!segment_args_ok(fn, n_goals, clearance, flags, goals_xyz != nullptr)) return FIESTA_ERR_INVALID;
+  fiesta_map *m = f->m;
+  const FbGeom &g = m->g;
+  const int gs[3] = {g.gx, g.gy, g.gz};
+  FbNavArgs a{};
+  for (int k = 0; k < 3; ++k) {
+    if (!(box_lo[k] >= 0 && box_lo[k] <= box_hi[k] && box_hi[k] < gs[k])) {
+      fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
+      return FIESTA_ERR_INVALID;
+    }
+    a.b.lo[k] = box_lo[k];
+    a.b.n[k] = box_hi[k] - box_lo[k] + 1;
+    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
+    a.w[k] = f->w[k];
+  }
+  const size_t nv = (size_t)a.b.n[0] * a.b.n[1] * a.b.n[2], nt = (size_t)a.tn[0] * a.tn[1] * a.tn[2];
+  CK(cudaSetDevice(m->device));
+  f->valid = false;
+  cudaError_t e = f->D.grow(nv, m->stream);
+  for (FbDevBuf<uint32_t> *b : {&f->stamp, &f->list[0], &f->list[1]})
+    if (e == cudaSuccess) e = b->grow(nt, m->stream);
+  if (e == cudaSuccess && n_goals > 0) e = f->d_goals.grow((size_t)n_goals * 3, m->stream);
+  if (e != cudaSuccess) {
+    cudaGetLastError();                                                   // not sticky: later calls must not see it
+    fb_set_error("%s: cannot allocate the field of %zu voxels: %s", fn, nv, cudaGetErrorString(e));
+    return FIESTA_ERR_CUDA;
+  }
+  a.D = f->D; a.stamp = f->stamp; a.list[0] = f->list[0]; a.list[1] = f->list[1]; a.ctr = f->ctr;
+  if (n_goals > 0) CK(cudaMemcpyAsync(f->d_goals, goals_xyz, (size_t)n_goals * 24, cudaMemcpyHostToDevice, m->stream));
+  CK(cudaMemsetAsync(f->stamp, 0, nt * 4, m->stream));
+  CK(cudaMemsetAsync(f->ctr, 0, sizeof(FbNavCtr), m->stream));
+  CK(cudaEventRecord(f->ev[0], m->stream));
+  CK(fb_nav_compute(g, m->cobs, a, f->d_goals, n_goals, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, f->blocks, m->stream));
+  m->st.kernel_launches += n_goals > 0 ? 4 : 3;
+  CK(cudaEventRecord(f->ev[1], m->stream));
+  CK(cudaMemcpyAsync(f->h_ctr, f->ctr, sizeof(FbNavCtr), cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  f->box = a.b;
+  f->valid = true;
+  if (stats) {
+    const FbNavCtr &c = *f->h_ctr;
+    *stats = fiesta_nav_stats{};
+    stats->box_voxels = (int64_t)nv;
+    stats->blocked = (int64_t)c.blocked;
+    stats->reached = (int64_t)c.reached;
+    stats->goals_placed = (int64_t)c.goals_placed;
+    stats->generations = (int64_t)c.generations;
+    stats->tile_visits = (int64_t)c.tile_visits;
+    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
+  }
+  return FIESTA_OK;
+}
+int fiesta_nav_export(const fiesta_nav_field *f, double *out) {
+  if (!f || !out) { fb_set_error("fiesta_nav_export: null argument"); return FIESTA_ERR_INVALID; }
+  if (!f->valid) { fb_set_error("fiesta_nav_export: no field has been computed"); return FIESTA_ERR_INVALID; }
+  const fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  CK(cudaMemcpyAsync(out, f->D, (size_t)f->box.n[0] * f->box.n[1] * f->box.n[2] * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, int32_t max_len, int32_t *status, int32_t *len, double *cost,
+                     int32_t *vox_xyz) {
+  const char *fn = "fiesta_nav_paths";
+  if (!f || n < 0 || max_len < 1 || (n > 0 && !(starts_xyz && status && len && cost && vox_xyz))) {
+    fb_set_error("%s: null buffer, negative count or max_len < 1", fn);
+    return FIESTA_ERR_INVALID;
+  }
+  if (!f->valid) { fb_set_error("%s: no field has been computed", fn); return FIESTA_ERR_INVALID; }
+  if (n == 0) return FIESTA_OK;
+  fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  const size_t nv = (size_t)n * max_len * 3;
+  cudaError_t e = f->d_pd.grow((size_t)n * 4, m->stream);
+  if (e == cudaSuccess) e = f->d_pi.grow((size_t)n * 2 + nv, m->stream);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    fb_set_error("%s: cannot allocate %lld paths of %d voxels: %s", fn, (long long)n, (int)max_len, cudaGetErrorString(e));
+    return FIESTA_ERR_CUDA;
+  }
+  double *d_starts = f->d_pd, *d_cost = d_starts + 3 * n;
+  int32_t *d_st = f->d_pi, *d_len = d_st + n, *d_vox = d_len + n;
+  CK(cudaMemcpyAsync(d_starts, starts_xyz, (size_t)n * 24, cudaMemcpyHostToDevice, m->stream));
+  CK(cudaMemsetAsync(d_vox, 0xff, nv * 4, m->stream));                    // -1 past each path's end
+  CK(fb_nav_paths(m->g, f->box, f->D, f->w, d_starts, n, max_len, d_st, d_len, d_cost, d_vox, m->stream));
+  m->st.kernel_launches++;
+  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(len, d_len, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(cost, d_cost, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(vox_xyz, d_vox, nv * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+
 // ---- planner query plan: fixed batch size, pinned host buffers, the copy-in / kernel / copy-out sequence captured once as a
 // CUDA graph; a run is one graph launch + one stream synchronisation (SURVEY.md 8(f) #3).
 struct fiesta_query_plan {

@@ -227,6 +227,47 @@ int fiesta_check_segments(fiesta_map *m, const double *ab, int64_t n, double cle
 int fiesta_host_mirror_check_segments(const fiesta_host_mirror *p, const double *ab, int64_t n, double clearance, int flags,
                                       int32_t *status, int64_t *hit_idx, double *hit_t, double *min_dist);
 
+/* ---- cost-to-go field (planners: A* / hybrid-A* heuristics, guide paths for trajectory optimisers, cost to frontier goals) ----
+ * How far is the nearest goal through free space, keeping a clearance, and which way leads there?  The field covers an inclusive
+ * voxel box [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis) and is a snapshot of the records at the time of the call.
+ *   traversable  a voxel of the box that does not block in the sense of segment clearance: GetDistance(Vector3i) > clearance,
+ *                and, with FIESTA_SEGMENT_UNKNOWN_BLOCKS, observed.  Voxels outside the box count as blocked.
+ *   moves        u -> u+d for the 26 offsets d in {-1,0,1}^3 \ {0}, allowed iff every voxel of the axis-aligned box spanned by u
+ *                and u+d (2, 4 or 8 voxels) is traversable: no corner cutting between diagonal obstacles.  Weight
+ *                resolution * sqrt(k), k = the number of non-zero components of d.
+ *   goals        positions (metres), mapped to voxels as Pos2Vox does; goals outside the box or on a blocked voxel are ignored
+ *                (stats.goals_placed counts the others).  Duplicates are allowed.
+ *   field        D = 0 on goals, else the least fixpoint of D(v) = min over allowed moves u -> v of fl(D(u) + w) in fp64 (the bits
+ *                of a sequential Dijkstra, whatever order the device relaxes in); +inf where no goal is reachable; -1 on blocked
+ *                voxels.  fiesta_nav_export writes it for the box, index ((x-lo.x)*By + (y-lo.y))*Bz + (z-lo.z), z fastest.
+ *   paths        from each start position: the start voxel, then repeatedly the first allowed neighbour u, in (dx, dy, dz) order
+ *                with dx slowest and -1 first, with fl(D(u) + w) == D(v), until D == 0.  vox_xyz receives max_len grid voxels
+ *                (x, y, z) per start, -1 past len[i]; cost[i] = D(start).  Folding the weights from the goal back along the path
+ *                reproduces D(start) bit for bit.  status 0 = reached, 1 = unreachable (cost +inf, len 0), 2 = start blocked,
+ *                outside the box or the map (PosInMap) or NaN (cost NaN, len 0), 3 = truncated after max_len voxels.
+ * The field object owns its device buffers, which grow to the largest box used: 8 bytes per box voxel plus 12 bytes per 8^3 tile,
+ * with the library's 50 % growth headroom (about 1.6 GB for a 512^3 box; 6.5 GB for a 1024 x 1024 x 512 box, which next to an
+ * EXACT map of that grid -- 68.1 GiB on a 79.2 GiB card -- is tight).  It runs on the map's stream; the calls are synchronous.
+ * Destroy it before the map.  Errors:
+ * FIESTA_ERR_INVALID for a box outside the grid or inverted, a clearance or flags that fiesta_check_segments rejects, null
+ * buffers, max_len < 1, or export / paths before a compute; nothing changes then.  FIESTA_ERR_CUDA when the buffers cannot be
+ * allocated; the map is untouched and the field must be computed again. */
+typedef struct fiesta_nav_field fiesta_nav_field;
+typedef struct fiesta_nav_stats {
+  int64_t box_voxels, blocked, reached;   /* reached: voxels with a finite D, goals included */
+  int64_t goals_placed;                   /* goals inside the box on a traversable voxel (duplicates counted) */
+  int64_t generations, tile_visits;       /* grid-wide relaxation rounds and 8^3 tile relaxations of the device solver */
+  float ms_compute;                       /* device time of the compute */
+  float reserved_f[1];
+} fiesta_nav_stats;
+int fiesta_nav_create(fiesta_map *m, fiesta_nav_field **out);
+void fiesta_nav_destroy(fiesta_nav_field *f);
+int fiesta_nav_compute(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *goals_xyz, int64_t n_goals,
+                       double clearance, int flags, fiesta_nav_stats *stats /* nullable */);
+int fiesta_nav_export(const fiesta_nav_field *f, double *out);   /* box_voxels doubles */
+int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, int32_t max_len, int32_t *status, int32_t *len,
+                     double *cost, int32_t *vox_xyz /* n * max_len * 3 */);
+
 /* ---- stream-ordered queries on DEVICE buffers (GPU planners whose positions already live in HBM) ----
  * The same queries on device pointers valid on the map's device, enqueued on `stream` (a cudaStream_t; 0 = the legacy default
  * stream); they return without synchronising the host.  Ordering: the query sees every map update issued before the call (the

@@ -149,6 +149,24 @@ class ESDFMap {
     check(fiesta_check_segments_device(h_, d_ab, n, clearance, flags, d_status, d_hit_idx, d_hit_t, d_min_dist, stream),
           "CheckSegmentsDevice");
   }
+  // Cost-to-go field for planners (fiesta_nav_* in fiesta_b200.h): geodesic distance from every voxel of a box to the nearest
+  // goal through free space at a clearance, and paths down it.  Destroy the field with fiesta_nav_destroy before the map.
+  fiesta_nav_field *MakeNavField() {
+    fiesta_nav_field *f = nullptr;
+    check(fiesta_nav_create(h_, &f), "MakeNavField");
+    return f;
+  }
+  fiesta_nav_stats ComputeNavField(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *goals_xyz, long n_goals,
+                                   double clearance, int flags) {
+    fiesta_nav_stats st = {};
+    check(fiesta_nav_compute(f, box_lo, box_hi, goals_xyz, n_goals, clearance, flags, &st), "ComputeNavField");
+    return st;
+  }
+  void ExportNavField(const fiesta_nav_field *f, double *out) { check(fiesta_nav_export(f, out), "ExportNavField"); }
+  void NavPaths(fiesta_nav_field *f, const double *starts_xyz, long n, int max_len, int32_t *status, int32_t *len, double *cost,
+                int32_t *vox_xyz) {
+    check(fiesta_nav_paths(f, starts_xyz, n, max_len, status, len, cost, vox_xyz), "NavPaths");
+  }
   void GetDistanceBatchDevice(const double *d_pos_xyz, long n, double *d_dist, void *stream) {
     check(fiesta_get_distance_batch_device(h_, d_pos_xyz, n, d_dist, stream), "GetDistanceBatchDevice");
   }
