@@ -47,6 +47,11 @@ class NavStats(C.Structure):
         ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
 
 
+class FrontierStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("box_voxels", "frontier_voxels", "clusters", "kept_clusters", "kept_voxels")] + [
+        ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
+
+
 class Stats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
         "occupancy_updates", "inserts", "deletes", "voxels_changed", "expansions", "voxels_reset", "tile_visits", "generations",
@@ -76,6 +81,8 @@ SYMBOLS = [
     "fiesta_check_segments", "fiesta_check_segments_device", "fiesta_get_distance_batch_device",
     "fiesta_get_dist_grad_trilinear_batch_device", "fiesta_host_mirror_check_segments",
     "fiesta_nav_create", "fiesta_nav_destroy", "fiesta_nav_compute", "fiesta_nav_export", "fiesta_nav_paths",
+    "fiesta_frontiers_create", "fiesta_frontiers_destroy", "fiesta_frontiers_compute", "fiesta_frontiers_clusters",
+    "fiesta_frontiers_voxels", "fiesta_frontiers_export",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -133,6 +140,13 @@ def load_library():
         L.fiesta_nav_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_int, C.c_void_p]
         L.fiesta_nav_export.argtypes = [C.c_void_p, C.c_void_p]
         L.fiesta_nav_paths.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 4
+        L.fiesta_frontiers_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+        L.fiesta_frontiers_destroy.argtypes = [C.c_void_p]
+        L.fiesta_frontiers_destroy.restype = None
+        L.fiesta_frontiers_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int64, C.c_void_p]
+        L.fiesta_frontiers_clusters.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 5
+        L.fiesta_frontiers_voxels.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
+        L.fiesta_frontiers_export.argtypes = [C.c_void_p, C.c_void_p]
         L.fiesta_get_distance_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
         L.fiesta_get_dist_grad_trilinear_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
@@ -285,6 +299,65 @@ class NavField:
     def close(self):
         if self._h:
             self._m._L.fiesta_nav_destroy(self._h)
+            self._h = None
+
+
+class Frontiers:
+    """fiesta_frontiers: the free voxels of a voxel box that border never-observed space, in 26-connected clusters, with cluster
+    statistics and member lists.  The buffers grow to the largest box computed; close() it before the map."""
+
+    def __init__(self, m):
+        self._m = m
+        h = C.c_void_p()
+        m._ck(m._L.fiesta_frontiers_create(m._h, C.byref(h)), "fiesta_frontiers_create")
+        self._h = h
+        self.shape = None
+        self.stats = None
+
+    def compute(self, box_lo, box_hi, clearance=0.0, min_cluster_size=1):
+        """Frontiers of the inclusive voxel box [box_lo, box_hi] at the clearance (metres) -> stats dict."""
+        lo, hi = np.ascontiguousarray(box_lo, dtype=np.int32), np.ascontiguousarray(box_hi, dtype=np.int32)
+        if lo.shape != (3,) or hi.shape != (3,):
+            raise ValueError("Frontiers.compute: box_lo and box_hi must be 3 voxel coordinates each")
+        st = FrontierStats()
+        self._m._ck(self._m._L.fiesta_frontiers_compute(self._h, lo.ctypes, hi.ctypes, C.c_double(float(clearance)),
+                                                         C.c_int64(int(min_cluster_size)), C.byref(st)), "Frontiers.compute")
+        self.shape = tuple(int(b - a + 1) for a, b in zip(lo, hi))
+        self.stats = {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved_f"}
+        return dict(self.stats)
+
+    def _need(self, what):
+        if self.stats is None:
+            raise FiestaError("Frontiers.%s: no frontiers have been computed" % what)
+
+    def clusters(self, cap=None):
+        """The kept clusters (the first `cap`): dict of size (K,) int64, rep / bbox_lo / bbox_hi (K, 3) int32 grid voxels and
+        centroid (K, 3) float64 metres."""
+        self._need("clusters")
+        k = self.stats["kept_clusters"] if cap is None else min(int(cap), self.stats["kept_clusters"])
+        out = dict(size=np.empty(k, np.int64), rep=np.empty((k, 3), np.int32), bbox_lo=np.empty((k, 3), np.int32),
+                   bbox_hi=np.empty((k, 3), np.int32), centroid=np.empty((k, 3)))
+        self._m._ck(self._m._L.fiesta_frontiers_clusters(self._h, C.c_int64(k), *(out[n].ctypes for n in out)), "Frontiers.clusters")
+        return out
+
+    def voxels(self, cap=None):
+        """Members of the kept clusters (the first `cap`) as (n, 3) int32 grid voxels, cluster by cluster."""
+        self._need("voxels")
+        n = self.stats["kept_voxels"] if cap is None else min(int(cap), self.stats["kept_voxels"])
+        out = np.empty((n, 3), np.int32)
+        self._m._ck(self._m._L.fiesta_frontiers_voxels(self._h, C.c_int64(n), out.ctypes), "Frontiers.voxels")
+        return out
+
+    def export(self):
+        """Cluster labels as a (Bx, By, Bz) int32 array: the cluster id, -1 elsewhere."""
+        self._need("export")
+        out = np.empty(self.shape, np.int32)
+        self._m._ck(self._m._L.fiesta_frontiers_export(self._h, out.ctypes), "Frontiers.export")
+        return out
+
+    def close(self):
+        if self._h:
+            self._m._L.fiesta_frontiers_destroy(self._h)
             self._h = None
 
 
@@ -457,6 +530,10 @@ class ESDFMap:
     def NavField(self):
         """Cost-to-go field of a voxel box through free space at a clearance, with path extraction (fiesta_nav_*)."""
         return NavField(self)
+
+    def Frontiers(self):
+        """Frontier voxels of a box (free voxels bordering unknown space) in clusters, with statistics (fiesta_frontiers_*)."""
+        return Frontiers(self)
 
     def RaycastFrame(self, xyz, T, min_ray_length, max_ray_length):
         """xyz: (n,3) float32 host array, or an integer device pointer paired with `n` as a tuple (ptr, n)."""

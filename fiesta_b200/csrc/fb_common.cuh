@@ -200,6 +200,36 @@ cudaError_t fb_nav_compute(const FbGeom &g, const uint32_t *cobs, const FbNavArg
 int fb_nav_relax_blocks(int device);
 cudaError_t fb_nav_paths(const FbGeom &g, const FbNavBox &b, const double *D, const double *w, const double *starts, long long n, int max_len,
                          int32_t *status, int32_t *len, double *cost, int32_t *vox, cudaStream_t s);
+// frontier extraction (fb_frontier.cu)
+struct FbFrCtr {
+  unsigned long long frontier;     // frontier voxels of the box
+  unsigned long long roots;        // clusters before the size filter
+  unsigned long long kept_voxels;  // members of the kept clusters
+  unsigned sel[3];                 // CUB selection counts: roots, kept clusters, kept members
+  unsigned pad;
+};
+struct FbFrBufs {                  // device buffers of one fiesta_frontiers object, grown by fb_frontier_compute
+  FbDevBuf<uint32_t> P;            // box: union-find parent words (FR_NONE off the frontier)
+  FbDevBuf<int32_t> L;             // box: cluster label, -1 elsewhere (fiesta_frontiers_export)
+  // per cluster before the size filter (C of them): root box index, size, kept ids in order, pre-filter id -> kept id or -1,
+  // grid-coordinate sums [3C], bounding boxes [lo 3C][hi 3C]
+  FbDevBuf<uint32_t> roots, size, kept;
+  FbDevBuf<int32_t> newid, box;
+  FbDevBuf<unsigned long long> sum;
+  // outputs per kept cluster, at pre-filter capacity C: size, [rep 3C][bbox lo 3C][bbox hi 3C], centroid [3C]
+  FbDevBuf<int64_t> o_size;
+  FbDevBuf<int32_t> o_i32;
+  FbDevBuf<double> o_cen;
+  // per member: sort keys and box indices (double-buffered), then the grid xyz of the sorted members
+  FbDevBuf<uint32_t> mkey[2], mval[2];
+  FbDevBuf<int32_t> m_xyz;
+  FbDevBuf<char> tmp;              // CUB temporary storage
+  FbDevBuf<FbFrCtr> ctr;
+  FbHostBuf<FbFrCtr> h_ctr;
+  unsigned C = 0;                  // pre-filter clusters of the last compute: the stride of o_i32
+};
+int fb_frontier_compute(const FbGeom &g, const uint32_t *cobs, const double *occ, double l_occ, const FbNavBox &b, double r,
+                        long long min_size, FbFrBufs &B, cudaStream_t s, int *launches);
 struct FbDepthRel { double m[16]; };
 struct fiesta_depth_params;
 cudaError_t fb_depth_to_cloud(const uint16_t *d_img, const uint16_t *d_last, int rows, int cols, const fiesta_depth_params &p, int filter_on,

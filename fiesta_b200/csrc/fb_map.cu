@@ -1075,6 +1075,116 @@ int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, i
   return FIESTA_OK;
 }
 
+// ---- frontier extraction (fb_frontier.h, fb_frontier.cu): free voxels of a box that border unknown space, clustered
+struct fiesta_frontiers {
+  fiesta_map *m = nullptr;
+  FbFrBufs B;
+  cudaEvent_t ev[2] = {};
+  FbNavBox box{};
+  fiesta_frontier_stats st{};
+  bool valid = false;               // B holds the result of a compute over `box`
+};
+void fiesta_frontiers_destroy(fiesta_frontiers *f) {
+  if (!f) return;
+  cudaSetDevice(f->m->device);
+  cudaStreamSynchronize(f->m->stream);
+  for (cudaEvent_t e : f->ev) if (e) cudaEventDestroy(e);
+  delete f;
+}
+int fiesta_frontiers_create(fiesta_map *m, fiesta_frontiers **out) {
+  if (!m || !out) { fb_set_error("fiesta_frontiers_create: null argument"); return FIESTA_ERR_INVALID; }
+  *out = nullptr;
+  CK(cudaSetDevice(m->device));
+  std::unique_ptr<fiesta_frontiers, void (*)(fiesta_frontiers *)> f(new (std::nothrow) fiesta_frontiers(), fiesta_frontiers_destroy);
+  if (!f) { fb_set_error("out of host memory"); return FIESTA_ERR_INVALID; }
+  f->m = m;
+  for (cudaEvent_t &e : f->ev) CK(cudaEventCreate(&e));
+  CK(f->B.ctr.alloc(1));
+  CK(f->B.h_ctr.alloc(1));
+  *out = f.release();
+  return FIESTA_OK;
+}
+int fiesta_frontiers_compute(fiesta_frontiers *f, const int box_lo[3], const int box_hi[3], double clearance, int64_t min_cluster_size,
+                             fiesta_frontier_stats *stats) {
+  const char *fn = "fiesta_frontiers_compute";
+  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (!segment_args_ok(fn, 0, clearance, 0, true)) return FIESTA_ERR_INVALID;
+  if (min_cluster_size < 1) { fb_set_error("%s: min_cluster_size must be >= 1", fn); return FIESTA_ERR_INVALID; }
+  fiesta_map *m = f->m;
+  const int gs[3] = {m->g.gx, m->g.gy, m->g.gz};
+  FbNavBox b{};
+  for (int k = 0; k < 3; ++k) {
+    if (!(box_lo[k] >= 0 && box_lo[k] <= box_hi[k] && box_hi[k] < gs[k])) {
+      fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
+      return FIESTA_ERR_INVALID;
+    }
+    b.lo[k] = box_lo[k];
+    b.n[k] = box_hi[k] - box_lo[k] + 1;
+  }
+  CK(cudaSetDevice(m->device));
+  f->valid = false;
+  int launches = 0;
+  CK(cudaEventRecord(f->ev[0], m->stream));
+  const int r = fb_frontier_compute(m->g, m->cobs, m->occ, m->l_occ, b, clearance, (long long)min_cluster_size, f->B, m->stream, &launches);
+  m->st.kernel_launches += launches;
+  if (r != FIESTA_OK) return r;
+  CK(cudaEventRecord(f->ev[1], m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  const FbFrCtr &c = *f->B.h_ctr;
+  f->st = fiesta_frontier_stats{};
+  f->st.box_voxels = (int64_t)b.n[0] * b.n[1] * b.n[2];
+  f->st.frontier_voxels = (int64_t)c.frontier;
+  f->st.clusters = (int64_t)c.roots;
+  f->st.kept_clusters = (int64_t)c.sel[1];
+  f->st.kept_voxels = (int64_t)c.kept_voxels;
+  CK(cudaEventElapsedTime(&f->st.ms_compute, f->ev[0], f->ev[1]));
+  f->box = b;
+  f->valid = true;
+  if (stats) *stats = f->st;
+  return FIESTA_OK;
+}
+int fiesta_frontiers_clusters(const fiesta_frontiers *f, int64_t cap, int64_t *size, int32_t *rep_xyz, int32_t *bbox_lo_xyz,
+                              int32_t *bbox_hi_xyz, double *centroid_xyz) {
+  const char *fn = "fiesta_frontiers_clusters";
+  if (!f || cap < 0 || (cap > 0 && !(size && rep_xyz && bbox_lo_xyz && bbox_hi_xyz && centroid_xyz))) {
+    fb_set_error("%s: null buffer or negative capacity", fn);
+    return FIESTA_ERR_INVALID;
+  }
+  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
+  const size_t n = (size_t)(cap < f->st.kept_clusters ? cap : f->st.kept_clusters), C = f->B.C;
+  if (n == 0) return FIESTA_OK;
+  const fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  CK(cudaMemcpyAsync(size, f->B.o_size, n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(rep_xyz, f->B.o_i32, n * 12, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(bbox_lo_xyz, f->B.o_i32 + 3 * C, n * 12, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(bbox_hi_xyz, f->B.o_i32 + 6 * C, n * 12, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(centroid_xyz, f->B.o_cen, n * 24, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+int fiesta_frontiers_voxels(const fiesta_frontiers *f, int64_t cap, int32_t *vox_xyz) {
+  const char *fn = "fiesta_frontiers_voxels";
+  if (!f || cap < 0 || (cap > 0 && !vox_xyz)) { fb_set_error("%s: null buffer or negative capacity", fn); return FIESTA_ERR_INVALID; }
+  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
+  const size_t n = (size_t)(cap < f->st.kept_voxels ? cap : f->st.kept_voxels);
+  if (n == 0) return FIESTA_OK;
+  const fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  CK(cudaMemcpyAsync(vox_xyz, f->B.m_xyz, n * 12, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+int fiesta_frontiers_export(const fiesta_frontiers *f, int32_t *labels) {
+  if (!f || !labels) { fb_set_error("fiesta_frontiers_export: null argument"); return FIESTA_ERR_INVALID; }
+  if (!f->valid) { fb_set_error("fiesta_frontiers_export: no frontiers have been computed"); return FIESTA_ERR_INVALID; }
+  const fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  CK(cudaMemcpyAsync(labels, f->B.L, (size_t)f->st.box_voxels * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+
 // ---- planner query plan: fixed batch size, pinned host buffers, the copy-in / kernel / copy-out sequence captured once as a
 // CUDA graph; a run is one graph launch + one stream synchronisation (SURVEY.md 8(f) #3).
 struct fiesta_query_plan {

@@ -268,6 +268,53 @@ int fiesta_nav_export(const fiesta_nav_field *f, double *out);   /* box_voxels d
 int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, int32_t max_len, int32_t *status, int32_t *len,
                      double *cost, int32_t *vox_xyz /* n * max_len * 3 */);
 
+/* ---- frontier extraction (exploration planners: where does observed free space end?) ----
+ * The free voxels of an inclusive voxel box [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis) that border never-observed
+ * space, grouped into clusters, as a snapshot of the integrated records and log-odds at the time of the call (observations that
+ * UpdateOccupancy has not integrated yet are not part of it).
+ *   unknown      a grid voxel whose distance reads -10000 in fiesta_export_distance (never observed).  Unreached voxels and
+ *                voxels reset by a local-map update are observed.
+ *   frontier     a box voxel that is observed, not occupied (GetOccupancy(Vector3i) == 0: log-odds <= l_occ), does not block at
+ *                the clearance in the sense of fiesta_check_segments without FIESTA_SEGMENT_UNKNOWN_BLOCKS (so it is a
+ *                traversable voxel of a cost-to-go field at the same clearance, usable as a nav goal or path start), and has
+ *                an unknown face neighbour inside the grid; the neighbour may lie outside the box, the map's outer faces do not
+ *                count.
+ *   clusters     the 26-connected components of the box's frontier voxels (a cluster cut by a box face stays cut); clusters of
+ *                fewer than min_cluster_size voxels are dropped; the kept ones are numbered 0..K-1 by their smallest member in
+ *                x, y, z loop order (the box index below).
+ *   per cluster  size; rep = its first member (grid voxel xyz); bbox lo / hi (grid voxels, inclusive); centroid (metres) =
+ *                ((double)S / (double)size + 0.5) * resolution + origin per axis, S the exact sum of the members' grid
+ *                coordinates, each operation rounded separately.
+ *   voxels       the kept clusters' members as grid voxel xyz, cluster by cluster, in loop order within a cluster.
+ *   labels       fiesta_frontiers_export: one int32 per box voxel, index ((x-lo.x)*By + (y-lo.y))*Bz + (z-lo.z) as in
+ *                fiesta_nav_export: the cluster id, or -1 off the frontier or in a dropped cluster.
+ * Every output is integer or one fixed fp64 expression: the same bits on every run and as a sequential definition
+ * (tests/frontierref.py).  fiesta_frontiers_clusters / _voxels write the first min(cap, n) entries (n = stats.kept_clusters /
+ * stats.kept_voxels of the last compute), as fiesta_get_point_cloud does.
+ * The object owns its device buffers, which grow to the largest box and result used: 8 bytes per box voxel, plus 132 bytes per
+ * cluster before the size filter and 28 bytes per kept member, with the library's 50 % growth headroom (about 1.6 GB for a
+ * 512^3 box).  It runs on the map's stream; the calls are synchronous.  Destroy it before the map.  Errors:
+ * FIESTA_ERR_INVALID for a box outside the grid or inverted, a clearance fiesta_check_segments rejects (NaN, < 0, >= 10000),
+ * min_cluster_size < 1, null buffers, a negative cap, or reads before a compute; nothing changes then.  FIESTA_ERR_CUDA when the
+ * buffers cannot be allocated; the map is untouched and a new compute is needed before the results can be read. */
+typedef struct fiesta_frontiers fiesta_frontiers;
+typedef struct fiesta_frontier_stats {
+  int64_t box_voxels;
+  int64_t frontier_voxels;                /* frontier voxels of the box, before the size filter */
+  int64_t clusters, kept_clusters;        /* clusters before and after the size filter */
+  int64_t kept_voxels;                    /* members of the kept clusters */
+  float ms_compute;                       /* device time of the compute */
+  float reserved_f[1];
+} fiesta_frontier_stats;
+int fiesta_frontiers_create(fiesta_map *m, fiesta_frontiers **out);
+void fiesta_frontiers_destroy(fiesta_frontiers *f);
+int fiesta_frontiers_compute(fiesta_frontiers *f, const int box_lo[3], const int box_hi[3], double clearance, int64_t min_cluster_size,
+                             fiesta_frontier_stats *stats /* nullable */);
+int fiesta_frontiers_clusters(const fiesta_frontiers *f, int64_t cap, int64_t *size, int32_t *rep_xyz /* cap * 3 */,
+                              int32_t *bbox_lo_xyz /* cap * 3 */, int32_t *bbox_hi_xyz /* cap * 3 */, double *centroid_xyz /* cap * 3 */);
+int fiesta_frontiers_voxels(const fiesta_frontiers *f, int64_t cap, int32_t *vox_xyz /* cap * 3 */);
+int fiesta_frontiers_export(const fiesta_frontiers *f, int32_t *labels);   /* box_voxels int32 */
+
 /* ---- stream-ordered queries on DEVICE buffers (GPU planners whose positions already live in HBM) ----
  * The same queries on device pointers valid on the map's device, enqueued on `stream` (a cudaStream_t; 0 = the legacy default
  * stream); they return without synchronising the host.  Ordering: the query sees every map update issued before the call (the

@@ -167,6 +167,25 @@ class ESDFMap {
                 int32_t *vox_xyz) {
     check(fiesta_nav_paths(f, starts_xyz, n, max_len, status, len, cost, vox_xyz), "NavPaths");
   }
+  // Frontier extraction for exploration planners (fiesta_frontiers_* in fiesta_b200.h): the free voxels of a box that border
+  // unknown space, in 26-connected clusters with statistics and member lists.  Destroy with fiesta_frontiers_destroy before the map.
+  fiesta_frontiers *MakeFrontiers() {
+    fiesta_frontiers *f = nullptr;
+    check(fiesta_frontiers_create(h_, &f), "MakeFrontiers");
+    return f;
+  }
+  fiesta_frontier_stats ComputeFrontiers(fiesta_frontiers *f, const int box_lo[3], const int box_hi[3], double clearance,
+                                         long min_cluster_size) {
+    fiesta_frontier_stats st = {};
+    check(fiesta_frontiers_compute(f, box_lo, box_hi, clearance, min_cluster_size, &st), "ComputeFrontiers");
+    return st;
+  }
+  void FrontierClusters(const fiesta_frontiers *f, long cap, int64_t *size, int32_t *rep_xyz, int32_t *bbox_lo_xyz, int32_t *bbox_hi_xyz,
+                        double *centroid_xyz) {
+    check(fiesta_frontiers_clusters(f, cap, size, rep_xyz, bbox_lo_xyz, bbox_hi_xyz, centroid_xyz), "FrontierClusters");
+  }
+  void FrontierVoxels(const fiesta_frontiers *f, long cap, int32_t *vox_xyz) { check(fiesta_frontiers_voxels(f, cap, vox_xyz), "FrontierVoxels"); }
+  void ExportFrontierLabels(const fiesta_frontiers *f, int32_t *labels) { check(fiesta_frontiers_export(f, labels), "ExportFrontierLabels"); }
   void GetDistanceBatchDevice(const double *d_pos_xyz, long n, double *d_dist, void *stream) {
     check(fiesta_get_distance_batch_device(h_, d_pos_xyz, n, d_dist, stream), "GetDistanceBatchDevice");
   }
