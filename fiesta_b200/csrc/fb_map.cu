@@ -328,9 +328,10 @@ static int flush_events(fiesta_map *m) {
   m->X.key_base += m->n_ev;
   m->st.kernel_launches++;
   CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(m->stream));                                   // the pinned buffer is reused immediately
   m->n_ev = 0;
-  return FIESTA_OK;
+  // synchronises (the pinned buffer is reused immediately) and refreshes the touched-tile count the events just queued:
+  // CheckUpdate reads it, and an export between SetOccupancy and CheckUpdate flushes the staged events
+  return fetch_counters(m);
 }
 static inline int stage_event(fiesta_map *m, const int *v, int occ) {
   if (m->n_ev == m->h_ev.cap) { int r = flush_events(m); if (r) return r; }

@@ -50,6 +50,23 @@ def test_degenerate_clouds(oracle_built, mode):
     assert dev.stats()["rays_dropped"] == ora.hung_rays()
 
 
+@pytest.mark.parametrize("mode", ["fast", "exact"])
+def test_check_update_after_export(oracle_built, mode):
+    """An export between SetOccupancy and CheckUpdate sends the staged events to the device; CheckUpdate
+    (!occupancy_queue_.empty(), ESDFMap.cpp:229) must still report them."""
+    dev, ora = pair(oracle_built, mode, params=scenes.PARAMS_TOGGLE)
+    vox = np.array([[3, 4, 5], [10, 11, 12], [63, 63, 31]], np.int32)
+    for m in (dev, ora):
+        m.SetOccupancyBatchVox(vox, np.ones(len(vox), np.uint8))
+    assert same_counters(dev, ora)
+    assert dev.CheckUpdate() and ora.CheckUpdate()
+    assert dev.UpdateOccupancy(True) == ora.UpdateOccupancy(True)
+    dev.UpdateESDF(); ora.UpdateESDF()
+    assert dev.CheckUpdate() == ora.CheckUpdate()
+    r = compare(dev, ora)
+    assert r["occ"] == 0 and r["dist"] == 0, r
+
+
 def test_per_call_api_and_sentinels(oracle_built):
     """int SetOccupancy(pos|vox, occ) return values and queries (ESDFMap.cpp:401-437, 452-540), call by call."""
     dev, ora = pair(oracle_built, "exact", params=scenes.PARAMS_TOGGLE)
