@@ -52,6 +52,15 @@ class FrontierStats(C.Structure):
         ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
 
 
+class SensorModel(C.Structure):
+    _fields_ = [("max_range", C.c_double), ("tan_half_fov", C.c_double * 2)]
+
+
+class ViewpointStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("candidates_scored", "pairs_walked", "pairs_visible")] + [
+        ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
+
+
 class Stats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
         "occupancy_updates", "inserts", "deletes", "voxels_changed", "expansions", "voxels_reset", "tile_visits", "generations",
@@ -82,7 +91,7 @@ SYMBOLS = [
     "fiesta_get_dist_grad_trilinear_batch_device", "fiesta_host_mirror_check_segments",
     "fiesta_nav_create", "fiesta_nav_destroy", "fiesta_nav_compute", "fiesta_nav_export", "fiesta_nav_paths",
     "fiesta_frontiers_create", "fiesta_frontiers_destroy", "fiesta_frontiers_compute", "fiesta_frontiers_clusters",
-    "fiesta_frontiers_voxels", "fiesta_frontiers_export",
+    "fiesta_frontiers_voxels", "fiesta_frontiers_export", "fiesta_frontiers_score_viewpoints",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -147,6 +156,8 @@ def load_library():
         L.fiesta_frontiers_clusters.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 5
         L.fiesta_frontiers_voxels.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
         L.fiesta_frontiers_export.argtypes = [C.c_void_p, C.c_void_p]
+        L.fiesta_frontiers_score_viewpoints.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
+                                                        C.POINTER(SensorModel), C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.fiesta_get_distance_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
         L.fiesta_get_dist_grad_trilinear_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
@@ -354,6 +365,26 @@ class Frontiers:
         out = np.empty(self.shape, np.int32)
         self._m._ck(self._m._L.fiesta_frontiers_export(self._h, out.ctypes), "Frontiers.export")
         return out
+
+    def score_viewpoints(self, cluster, positions, orientations, max_range, tan_half_fov, clearance=0.0, unknown_blocks=False):
+        """How many members of its kept cluster a sensor at each candidate would see (fiesta_frontiers_score_viewpoints).
+        cluster (n,) kept cluster ids, positions (n, 3) metres, orientations (n_orient, 3, 3) world-to-sensor rows (optical axis,
+        horizontal, vertical), tan_half_fov (horizontal, vertical) -> (status (n,) int32, score (n, n_orient) int32, stats dict)."""
+        self._need("score_viewpoints")
+        cl = np.ascontiguousarray(cluster, dtype=np.int32).reshape(-1)
+        pos = _f64(positions).reshape(-1, 3)
+        R = _f64(orientations).reshape(-1, 9)
+        if len(cl) != len(pos):
+            raise ValueError("Frontiers.score_viewpoints: %d cluster ids for %d positions" % (len(cl), len(pos)))
+        n, k = len(pos), len(R)
+        status, score = np.empty(n, np.int32), np.empty((n, k), np.int32)
+        sm = SensorModel(float(max_range), (C.c_double * 2)(*[float(x) for x in tan_half_fov]))
+        st = ViewpointStats()
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        self._m._ck(self._m._L.fiesta_frontiers_score_viewpoints(self._h, cl.ctypes, pos.ctypes, C.c_int64(n), R.ctypes, C.c_int32(k),
+                                                                  C.byref(sm), r, flags, status.ctypes, score.ctypes, C.byref(st)),
+                    "Frontiers.score_viewpoints")
+        return status, score, {n_: getattr(st, n_) for n_, _ in st._fields_ if n_ != "reserved_f"}
 
     def close(self):
         if self._h:

@@ -230,6 +230,24 @@ struct FbFrBufs {                  // device buffers of one fiesta_frontiers obj
 };
 int fb_frontier_compute(const FbGeom &g, const uint32_t *cobs, const double *occ, double l_occ, const FbNavBox &b, double r,
                         long long min_size, FbFrBufs &B, cudaStream_t s, int *launches);
+// viewpoint coverage of frontier clusters (fb_view.cu)
+struct FbViewCtr {
+  unsigned long long scored, walked, visible;   // status-0 candidates, pairs in range and view, walked pairs with a clear line of sight
+};
+struct FbViewBufs {                // device buffers of fiesta_frontiers_score_viewpoints, kept on the frontier object
+  FbDevBuf<double> pos;            // per candidate: position [3n]
+  FbDevBuf<int32_t> cl, status;    //                cluster id, status
+  FbDevBuf<long long> work;        //                [n + 1] chunk counts, scanned in place to each one's first chunk (work[n]: total)
+  FbDevBuf<int32_t> score;         //                [n * n_orient]
+  FbDevBuf<long long> moff;        // per kept cluster: its first member in the member list
+  FbDevBuf<double> orient;         // [9 * n_orient]
+  FbDevBuf<FbViewCtr> ctr;
+  FbHostBuf<FbViewCtr> h_ctr;
+};
+// Expects V.pos / cl / orient filled for n >= 1 candidates and V.score / ctr zeroed; size / m_xyz are the frontier result's.
+int fb_view_score(const FbGeom &g, const uint32_t *cobs, const int64_t *size, const int32_t *m_xyz, unsigned K, FbViewBufs &V,
+                  FbDevBuf<char> &tmp, long long n, int n_orient, const fiesta_sensor_model &sm, double clearance, int unknown_blocks,
+                  cudaStream_t s, int *launches);
 struct FbDepthRel { double m[16]; };
 struct fiesta_depth_params;
 cudaError_t fb_depth_to_cloud(const uint16_t *d_img, const uint16_t *d_last, int rows, int cols, const fiesta_depth_params &p, int filter_on,

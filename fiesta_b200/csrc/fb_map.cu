@@ -1080,6 +1080,7 @@ int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, i
 struct fiesta_frontiers {
   fiesta_map *m = nullptr;
   FbFrBufs B;
+  FbViewBufs V;                     // fiesta_frontiers_score_viewpoints
   cudaEvent_t ev[2] = {};
   FbNavBox box{};
   fiesta_frontier_stats st{};
@@ -1183,6 +1184,76 @@ int fiesta_frontiers_export(const fiesta_frontiers *f, int32_t *labels) {
   CK(cudaSetDevice(m->device));
   CK(cudaMemcpyAsync(labels, f->B.L, (size_t)f->st.box_voxels * 4, cudaMemcpyDeviceToHost, m->stream));
   CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+// viewpoint coverage of the clusters (fb_view.h, fb_view.cu)
+int fiesta_frontiers_score_viewpoints(fiesta_frontiers *f, const int32_t *cluster, const double *pos_xyz, int64_t n, const double *orient,
+                                      int32_t n_orient, const fiesta_sensor_model *sensor, double clearance, int flags, int32_t *status,
+                                      int32_t *score, fiesta_viewpoint_stats *stats) {
+  const char *fn = "fiesta_frontiers_score_viewpoints";
+  if (!f || !sensor || !orient) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (!segment_args_ok(fn, n, clearance, flags, cluster && pos_xyz && status && score)) return FIESTA_ERR_INVALID;
+  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
+  if (n_orient < 1) { fb_set_error("%s: n_orient must be >= 1", fn); return FIESTA_ERR_INVALID; }
+  const fiesta_sensor_model sm = *sensor;
+  const double sv[3] = {sm.max_range, sm.tan_half_fov[0], sm.tan_half_fov[1]};
+  for (double x : sv)
+    if (!(std::isfinite(x) && x > 0)) { fb_set_error("%s: max_range and tan_half_fov must be finite and > 0", fn); return FIESTA_ERR_INVALID; }
+  if (n_orient > FIESTA_VIEWPOINT_MAX_ORIENT) {
+    fb_set_error("%s: at most %d orientations per call", fn, FIESTA_VIEWPOINT_MAX_ORIENT);
+    return FIESTA_ERR_LIMIT;
+  }
+  for (int k = 0; k < 9 * n_orient; ++k)
+    if (!std::isfinite(orient[k])) { fb_set_error("%s: orientation entry %d is not finite", fn, k); return FIESTA_ERR_INVALID; }
+  const int64_t K = f->st.kept_clusters;
+  for (int64_t i = 0; i < n; ++i)
+    if (!(cluster[i] >= 0 && cluster[i] < K)) {
+      fb_set_error("%s: cluster[%lld] = %d is not a kept cluster id (there are %lld)", fn, (long long)i, (int)cluster[i], (long long)K);
+      return FIESTA_ERR_INVALID;
+    }
+  if (n >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 candidates per call", fn); return FIESTA_ERR_LIMIT; }
+  if (stats) *stats = fiesta_viewpoint_stats{};
+  if (n == 0) return FIESTA_OK;
+  fiesta_map *m = f->m;
+  const cudaStream_t s = m->stream;
+  FbViewBufs &V = f->V;
+  CK(cudaSetDevice(m->device));
+  cudaError_t e = V.pos.grow((size_t)n * 3, s);
+  if (e == cudaSuccess) e = V.cl.grow((size_t)n, s);
+  if (e == cudaSuccess) e = V.status.grow((size_t)n, s);
+  if (e == cudaSuccess) e = V.work.grow((size_t)n + 1, s);
+  if (e == cudaSuccess) e = V.score.grow((size_t)n * n_orient, s);
+  if (e == cudaSuccess) e = V.moff.grow((size_t)K, s);
+  if (e == cudaSuccess) e = V.orient.grow(9 * FIESTA_VIEWPOINT_MAX_ORIENT, s);
+  if (e == cudaSuccess) e = V.ctr.grow(1, s);
+  if (e == cudaSuccess && !V.h_ctr) e = V.h_ctr.alloc(1);
+  if (e != cudaSuccess) {
+    cudaGetLastError();                                                   // not sticky: later calls must not see it
+    fb_set_error("%s: cannot allocate the buffers of %lld candidates: %s", fn, (long long)n, cudaGetErrorString(e));
+    return FIESTA_ERR_CUDA;
+  }
+  CK(cudaMemcpyAsync(V.pos, pos_xyz, (size_t)n * 24, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(V.cl, cluster, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(V.orient, orient, (size_t)n_orient * 72, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(V.score, 0, (size_t)n * n_orient * 4, s));
+  CK(cudaMemsetAsync(V.ctr, 0, sizeof(FbViewCtr), s));
+  int launches = 0;
+  CK(cudaEventRecord(f->ev[0], s));
+  const int r = fb_view_score(m->g, m->cobs, f->B.o_size, f->B.m_xyz, (unsigned)K, V, f->B.tmp, (long long)n, (int)n_orient, sm, clearance,
+                              flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, s, &launches);
+  m->st.kernel_launches += launches;
+  if (r != FIESTA_OK) return r;
+  CK(cudaEventRecord(f->ev[1], s));
+  CK(cudaMemcpyAsync(V.h_ctr, V.ctr, sizeof(FbViewCtr), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(status, V.status, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(score, V.score, (size_t)n * n_orient * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (stats) {
+    stats->candidates_scored = (int64_t)V.h_ctr->scored;
+    stats->pairs_walked = (int64_t)V.h_ctr->walked;
+    stats->pairs_visible = (int64_t)V.h_ctr->visible;
+    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
+  }
   return FIESTA_OK;
 }
 

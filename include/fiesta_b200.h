@@ -315,6 +315,48 @@ int fiesta_frontiers_clusters(const fiesta_frontiers *f, int64_t cap, int64_t *s
 int fiesta_frontiers_voxels(const fiesta_frontiers *f, int64_t cap, int32_t *vox_xyz /* cap * 3 */);
 int fiesta_frontiers_export(const fiesta_frontiers *f, int32_t *labels);   /* box_voxels int32 */
 
+/* ---- viewpoint coverage (exploration planners: where should the sensor stand to look past a frontier?) ----
+ * Scores candidate sensor poses by the members of a frontier cluster they would see.  Candidate i is a position pos[i] (metres)
+ * tagged with a kept cluster id cluster[i] of the last fiesta_frontiers_compute; the n_orient (1..32) orientations are shared by
+ * all candidates, each a row-major 3x3 world-to-sensor matrix R: row 0 is the optical axis, row 1 the axis the horizontal field of
+ * view spans, row 2 the vertical one.  The rows are used exactly as given (no orthonormality check, no trigonometry).
+ *   status     2 = pos fails PosInMap or has a NaN coordinate; 1 = its voxel Pos2Vox(pos) is outside the grid (upper faces),
+ *              never observed or has GetDistance(Vector3i) <= clearance, whatever the flags (so every status-0 candidate is a
+ *              traversable voxel of a cost-to-go field at the same clearance, with or without FIESTA_SEGMENT_UNKNOWN_BLOCKS);
+ *              0 = scored.  A candidate with status 1 or 2 scores 0 for every orientation.
+ *   pair       for a status-0 candidate p and a member voxel v of its cluster, each fp64 operation rounded on its own:
+ *              c_k = ((double)v_k + 0.5) * resolution + origin_k (Vox2Pos), d_k = c_k - p_k;
+ *              in range: (d0*d0 + d1*d1) + d2*d2 <= max_range * max_range;
+ *              in view of orientation j: s_k = (R[k][0]*d0 + R[k][1]*d1) + R[k][2]*d2 with
+ *              s0 > 0 && fabs(s1) <= tan_half_fov[0] * s0 && fabs(s2) <= tan_half_fov[1] * s0;
+ *              visible: fiesta_check_segments on {p, c} at clearance 0 with `flags` returns status 0 (no obstacle voxel on the
+ *              exact walk and, with FIESTA_SEGMENT_UNKNOWN_BLOCKS, no never-observed one).
+ *   score      score[i * n_orient + j] = the members of cluster[i] in range, in view of orientation j and visible.
+ * Line of sight reads the records at the time of the call; the members are those of the last compute.  Every output is an integer
+ * decided by fixed fp64 expressions and the integer walk: the same bits on every run and as a sequential definition
+ * (tests/viewref.py).  Memory on the frontier object, grown as needed: 40 + 4 * n_orient bytes per candidate and 8 per kept
+ * cluster, plus scan storage.  Host pointers, the map's stream, synchronous.  Errors (nothing is written and the frontier result
+ * stays valid): FIESTA_ERR_INVALID before any compute, for a cluster id outside [0, kept_clusters), n < 0, n_orient < 1, a
+ * non-finite or <= 0 max_range or tangent, a non-finite orientation entry, a clearance or flags that fiesta_check_segments
+ * rejects, or null buffers with n > 0 (sensor and orient are always needed); FIESTA_ERR_LIMIT for n_orient > 32 (call again
+ * with the rest) or n >= 2^31 - 1; FIESTA_ERR_CUDA when the buffers cannot be allocated. */
+typedef struct fiesta_sensor_model {
+  double max_range;                       /* metres, Euclidean from the sensor position to the voxel centre */
+  double tan_half_fov[2];                 /* horizontal (row 1), vertical (row 2) */
+} fiesta_sensor_model;
+typedef struct fiesta_viewpoint_stats {
+  int64_t candidates_scored;              /* status-0 candidates */
+  int64_t pairs_walked;                   /* (candidate, member) pairs in range and in view of at least one orientation */
+  int64_t pairs_visible;                  /* walked pairs with a clear line of sight */
+  float ms_compute;                       /* device time of the scoring */
+  float reserved_f[1];
+} fiesta_viewpoint_stats;
+#define FIESTA_VIEWPOINT_MAX_ORIENT 32
+int fiesta_frontiers_score_viewpoints(fiesta_frontiers *f, const int32_t *cluster, const double *pos_xyz, int64_t n,
+                                      const double *orient /* n_orient * 9 */, int32_t n_orient, const fiesta_sensor_model *sensor,
+                                      double clearance, int flags, int32_t *status, int32_t *score /* n * n_orient, row i = candidate i */,
+                                      fiesta_viewpoint_stats *stats /* nullable */);
+
 /* ---- stream-ordered queries on DEVICE buffers (GPU planners whose positions already live in HBM) ----
  * The same queries on device pointers valid on the map's device, enqueued on `stream` (a cudaStream_t; 0 = the legacy default
  * stream); they return without synchronising the host.  Ordering: the query sees every map update issued before the call (the

@@ -186,6 +186,13 @@ class ESDFMap {
   }
   void FrontierVoxels(const fiesta_frontiers *f, long cap, int32_t *vox_xyz) { check(fiesta_frontiers_voxels(f, cap, vox_xyz), "FrontierVoxels"); }
   void ExportFrontierLabels(const fiesta_frontiers *f, int32_t *labels) { check(fiesta_frontiers_export(f, labels), "ExportFrontierLabels"); }
+  fiesta_viewpoint_stats ScoreViewpoints(fiesta_frontiers *f, const int32_t *cluster, const double *pos_xyz, long n, const double *orient,
+                                         int n_orient, const fiesta_sensor_model &sensor, double clearance, int flags, int32_t *status,
+                                         int32_t *score) {
+    fiesta_viewpoint_stats st = {};
+    check(fiesta_frontiers_score_viewpoints(f, cluster, pos_xyz, n, orient, n_orient, &sensor, clearance, flags, status, score, &st), "ScoreViewpoints");
+    return st;
+  }
   void GetDistanceBatchDevice(const double *d_pos_xyz, long n, double *d_dist, void *stream) {
     check(fiesta_get_distance_batch_device(h_, d_pos_xyz, n, d_dist, stream), "GetDistanceBatchDevice");
   }
