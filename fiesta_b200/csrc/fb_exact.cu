@@ -312,15 +312,18 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
     st->voxels_changed = h->voxels_changed; st->expansions = h->expansions;
     if (xdbg) {
       static unsigned long long hd[FB_X_DBG_WORDS];
+      static double cyc_per_us = 0;                            // clock64 counts SM cycles: convert with this device's SM clock
+      if (cyc_per_us == 0) { int dev = 0, khz = 0; CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev)); cyc_per_us = khz / 1000.0; }
       CK(cudaMemcpy(hd, X->d_dbg, sizeof(hd), cudaMemcpyDeviceToHost));
       static const char *cat[14] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top", "empty-barrier", "reseed.rounds", "reseed.assemble"};
       fprintf(stderr, "[x] reseed rounds %u; phases (us, count):", st->reseed_rounds);
-      for (int c = 0; c < 14; ++c) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[3 * 1024 + 2 * c] / 1965.0, hd[3 * 1024 + 2 * c + 1]);
+      for (int c = 0; c < 14; ++c) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[3 * 1024 + 2 * c] / cyc_per_us, hd[3 * 1024 + 2 * c + 1]);
       fprintf(stderr, "\n");
-      { double wm = 0; for (int q = 0; q < 4096; ++q) wm += hd[3 * 1024 + 32 + 1024 + q] / 1965.0; fprintf(stderr, "[x] sum over rounds of the longest per-CTA work time: %.0f us (the rest of round1+rounds+dense+s.round1+s.rounds is barrier + skew)\n", wm); }
+      { double wm = 0; for (int q = 0; q < 4096; ++q) wm += hd[3 * 1024 + 32 + 1024 + q] / cyc_per_us; fprintf(stderr, "[x] sum over rounds of the longest per-CTA work time: %.0f us (the rest of round1+rounds+dense+s.round1+s.rounds is barrier + skew)\n", wm); }
       for (int gq = 0; gq < 2; ++gq) { fprintf(stderr, "[x] gen %d work lists:", gq); for (int r = 0; r < 512 && hd[3 * 1024 + 32 + gq * 512 + r]; ++r) fprintf(stderr, " %llu", hd[3 * 1024 + 32 + gq * 512 + r]); fprintf(stderr, "\n"); }
+      fprintf(stderr, "[x] work-list entries: evaluated %llu refreshed %llu reseeded %llu\n", hd[3 * 1024 + 2 * 14], hd[3 * 1024 + 2 * 14 + 1], hd[3 * 1024 + 2 * 15]);
       fprintf(stderr, "[x] gens %u rounds %u dense %u deps %u nE0 %u |", st->generations, st->eval_rounds, st->dense_rounds, st->dependants, nE);
-      for (unsigned q = 0; q < st->generations && q < 1024; ++q) fprintf(stderr, " %llu/%llu/%.1fus", hd[3 * q], hd[3 * q + 1], hd[3 * q + 2] / 1965.0);
+      for (unsigned q = 0; q < st->generations && q < 1024; ++q) fprintf(stderr, " %llu/%llu/%.1fus", hd[3 * q], hd[3 * q + 1], hd[3 * q + 2] / cyc_per_us);
       fprintf(stderr, "\n");
     }
   }

@@ -40,8 +40,10 @@
 #define X_NOFF 129
 #define X_MAX_ROUNDS 4000000u
 #define XGB 8                         // writer words loaded per batch by a gather (24 / XGB batches)
+#define XRC 8                         // directions listed per chunk after a re-seeding change (24 / XRC chunks)
 #define XDBG_GENS 1024                // trace layout (FIESTA_DEBUG_X): [3 * XDBG_GENS] per generation {nE, rounds, cycles},
-#define XDBG_PHASE (3 * XDBG_GENS)    // then 16 x {cycles, count} per phase category, then 2 x 512 work-list sizes per round
+#define XDBG_PHASE (3 * XDBG_GENS)    // then 16 x {cycles, count} per phase category (14: summed work / flip list lengths, 15: summed
+                                      // re-seeding list lengths), then 2 x 512 work-list sizes per round
 #define XDBG_ROUNDS (XDBG_PHASE + 32)
 #define XDBG_WMAX (XDBG_ROUNDS + 1024)      // 4096 slots: per round of the fixpoint, the longest work time of any CTA (cycles)
 
@@ -470,6 +472,24 @@ __device__ __forceinline__ unsigned x_block_scan(XShared &sh, unsigned c, unsign
   return __shfl_sync(0xffffffffu, s - v, (int)wid) + incl - c;
 }
 
+// Reserves n (< 16) consecutive slots per lane of the lanes active here behind `counter`: one atomic per warp.  The exclusive
+// prefix of n over the active lanes is built from one ballot per bit of n.
+__device__ __forceinline__ unsigned x_warp_append_n(unsigned *counter, unsigned n, unsigned lane) {
+  const unsigned act = __activemask(), below = (1u << lane) - 1u;
+  unsigned pre = 0, total = 0;
+#pragma unroll
+  for (int bit = 0; bit < 4; ++bit) {
+    const unsigned m = __ballot_sync(act, (n >> bit) & 1u);
+    pre += (unsigned)__popc(m & below) << bit;
+    total += (unsigned)__popc(m) << bit;
+  }
+  if (total == 0u) return 0u;
+  const int leader = __ffs(act) - 1;
+  unsigned base = 0;
+  if ((int)lane == leader) base = atomicAdd(counter, total);
+  return __shfl_sync(act, base, leader) + pre;
+}
+
 // One evaluation of the re-seeding rule: dependant i takes the closest obstacle of the FIRST neighbour in dirs_ order that
 // has a valid one (:308-321); dependants processed earlier expose their new value, later ones their (deleted) old one.
 __device__ __forceinline__ uint32_t x_reseed_eval(const XArgs &a, unsigned i, int x, int y, int z, unsigned &kc) {
@@ -541,6 +561,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       const unsigned nw = r == 1u ? a.ndep : __ldcg(&ctl->nW[in]);
       if (gtid == 0) ctl->nW[zz] = 0;
       if (r > 1u && nw == 0u) break;
+      if (a.dbg && gtid == 0) a.dbg[XDBG_PHASE + 2 * 15] += nw;
       ++reseed_rounds; ++wclock;
       if (nw <= 2u * gwarps) {
         // short list: one WARP per dependant, lane k = neighbour k -- the 24 look-ups (position in deps, code, Exist bit) run side
@@ -592,25 +613,35 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
         a.nk[i] = (uint8_t)kc;
         if (res == was) continue;
         a.nc[i] = res;
-        for (int k = 0; k < 24; ++k) {                         // later dependants that look at this one
-          const int nx = x + x_dirs[k][0], ny = y + x_dirs[k][1], nz = z + x_dirs[k][2];
-          if (!x_in_grid(g, nx, ny, nz)) continue;
-          const unsigned o = __ldcg(&a.ord[x_vi(g, nx, ny, nz)]);
-          bool push = o != XNONE && o > i;
-          if (push) {
-            const unsigned so = __ldcg(&a.wstamp[o]);
-            push = so != wclock;                               // not listed for the next round yet
-            // A dependant that is NOT being evaluated in this round holds a stable choice: it looks at this voxel through
-            // direction k^1 and only cares if that direction comes before its current source (and this one became valid) or
-            // is its current source.  One that is being evaluated right now may have missed the new value: always listed.
-            if (push && r > 1u && so != wclock - 1u) {
-              const unsigned ko = __ldcg(&a.nk[o]), kd = (unsigned)k ^ 1u;
-              push = kd == ko || (kd < ko && res >= 2u);
-            }
-            push = push && atomicExch(&a.wstamp[o], wclock) != wclock;
+        // later dependants that look at this one, XRC directions at a time: every stage issues its loads (or atomics) for
+        // all of them before the next stage looks at the results, and the chunk ends with one append per warp -- a few
+        // round trips per chunk instead of up to five per direction, one after the other
+#pragma unroll
+        for (int k0 = 0; k0 < 24; k0 += XRC) {
+          unsigned o[XRC], so[XRC], ko[XRC];
+#pragma unroll
+          for (int t = 0; t < XRC; ++t) {
+            const int k = k0 + t, nx = x + x_dc(k, 0), ny = y + x_dc(k, 1), nz = z + x_dc(k, 2);
+            o[t] = x_in_grid(g, nx, ny, nz) ? __ldcg(&a.ord[x_vi(g, nx, ny, nz)]) : XNONE;
           }
-          const unsigned slot2 = fb_warp_append(&ctl->nW[out], push);
-          if (push) a.W[out][slot2] = o;
+#pragma unroll
+          for (int t = 0; t < XRC; ++t) so[t] = (o[t] != XNONE && o[t] > i) ? __ldcg(&a.wstamp[o[t]]) : wclock;   // wclock = not a candidate
+          // A dependant that is NOT being evaluated in this round holds a stable choice: it looks at this voxel through
+          // direction k^1 and only cares if that direction comes before its current source (and this one became valid) or
+          // is its current source.  One that is being evaluated right now may have missed the new value: always listed.
+#pragma unroll
+          for (int t = 0; t < XRC; ++t) ko[t] = (so[t] != wclock && r > 1u && so[t] != wclock - 1u) ? __ldcg(&a.nk[o[t]]) : XNONE;
+          unsigned pm = 0;
+#pragma unroll
+          for (int t = 0; t < XRC; ++t) {
+            const unsigned kd = (unsigned)(k0 + t) ^ 1u;
+            bool push = so[t] != wclock;                       // not listed for the next round yet
+            if (push && ko[t] != XNONE) push = kd == ko[t] || (kd < ko[t] && res >= 2u);
+            if (push && atomicExch(&a.wstamp[o[t]], wclock) != wclock) pm |= 1u << t;
+          }
+          unsigned slot2 = x_warp_append_n(&ctl->nW[out], (unsigned)__popc(pm), lane);
+#pragma unroll
+          for (int t = 0; t < XRC; ++t) if ((pm >> t) & 1u) a.W[out][slot2++] = o[t];
         }
       }
       x_gsync(&ctl->bar, bar_target);
@@ -685,6 +716,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       if (gtid == 0) { ctl->nW[zz] = 0; ctl->nF[zz] = 0; }
       if (r > 1u && nw == 0u && nf == 0u) break;
       if (r > X_MAX_ROUNDS) { if (gtid == 0) ctl->err = 2u; break; }   // cannot happen (element i is final after i+1 rounds at the latest); never spin forever on the GPU
+      if (a.dbg && gtid == 0) { a.dbg[XDBG_PHASE + 2 * 14] += nw; a.dbg[XDBG_PHASE + 2 * 14 + 1] += nf; }
       ++rounds; ++wclock;
       const bool dense = big && r > 1u && nw > a.dense_min;   // more than one wave of warps: evaluate through the summaries
       if (dense) {                                             // bring the summaries up to date first, then evaluate through them

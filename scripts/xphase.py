@@ -1,0 +1,115 @@
+"""Phase split of k_x_relax (EXACT UpdateESDF) over the frames bench.py times.
+
+    python scripts/xphase.py [--workload lidar512] [--warmup 3] [--steps 20] [--out FILE]
+
+Runs frames 0 .. warmup+steps-1 of the workload in EXACT mode with FIESTA_DEBUG_X=1 (the kernel then times its phases with
+clock64; the library converts cycles with the device's SM clock) and sums, over the timed frames warmup .. warmup+steps-1:
+the time of every phase, the evaluation rounds, the work-list entries evaluated and refreshed, and the re-seeding list
+entries.  It also prints, per frame, the (nE, rounds) list of every generation.  The numbers of generations and every nE
+are fixed by the sequential result; rounds and list lengths vary from run to run (a round reads words flipped in the same
+round).  The output is plain text, one item per line, so two runs can be diffed.  Needs a GPU.
+"""
+import argparse
+import os
+import re
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+PHASES = ["S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
+          "empty-barrier", "reseed.rounds", "reseed.assemble"]
+
+
+def child(wl, nframes):
+    """Runs the frames; the library writes its [x] lines to stderr, each frame is preceded by a marker line."""
+    sys.path.insert(0, ROOT)
+    import numpy as np
+    import bench
+    import fiesta_b200
+    from tests import scenes
+    w = bench.WORKLOADS[wl]
+    frames = bench.make_frames(wl, nframes)
+    m = fiesta_b200.ESDFMap(w["origin"], w["res"], w["size"], device=0, mode="exact")
+    m.SetParameters(*bench.wl_params(wl))
+    if w["kind"] == "stress":
+        allv = scenes.all_voxels(m.grid_size)
+        m.SetOccupancyBatchVox(allv, np.zeros(len(allv), np.uint8)); m.UpdateOccupancy(True); m.UpdateESDF()
+    dparams = fiesta_b200.DepthParams(scenes.FX, scenes.FY, scenes.CX, scenes.CY, *w["filter"]) if w["kind"] == "depth" else None
+    for f, fr in enumerate(frames):
+        sys.stderr.write("[frame] %d\n" % f); sys.stderr.flush()
+        if w["kind"] == "lidar":
+            m.RaycastFrame(fr["pts"], fr["T"], w["min_len"], w["max_len"])
+        elif w["kind"] == "depth":
+            m.DepthFrame(fr["img"], dparams, fr["T"], fr["m_rel"], w["min_len"], w["max_len"])
+        else:
+            m.SetOccupancyBatchVox(fr["vox"], fr["occ"])
+        if m.CheckUpdate():
+            m.SetOriginalRange(); m.UpdateOccupancy(True); m.UpdateESDF()
+        m.synchronize()
+        sys.stderr.write("[expansions] %d\n" % m.stats()["expansions"]); sys.stderr.flush()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="lidar512")
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--out", help="also write the report to this file")
+    ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
+    args = ap.parse_args()
+    if args.child:
+        child(args.workload, args.warmup + args.steps)
+        return
+    env = dict(os.environ, FIESTA_DEBUG_X="1")
+    cmd = [sys.executable, os.path.abspath(__file__), "--child", "--workload", args.workload, "--warmup", str(args.warmup), "--steps", str(args.steps)]
+    p = subprocess.run(cmd, env=env, stdout=subprocess.DEVNULL, stderr=subprocess.PIPE, text=True)
+    if p.returncode:
+        sys.stderr.write(p.stderr[-4000:])
+        raise SystemExit(p.returncode)
+    lo, hi = args.warmup, args.warmup + args.steps
+    us = {k: 0.0 for k in PHASES}
+    tot = dict(rounds=0, evaluated=0, refreshed=0, reseeded=0, reseed_rounds=0, generations=0, expansions=0)
+    gens = {}
+    f = -1
+    for line in p.stderr.splitlines():
+        if line.startswith("[frame] "):
+            f = int(line.split()[1]); gens[f] = []
+            continue
+        if not lo <= f < hi:
+            if line.startswith("[x] gens "):
+                gens[f] = [tuple(int(v) for v in t.split("/")[:2]) for t in line.split("|", 1)[1].split()]
+            continue
+        if line.startswith("[expansions] "):
+            tot["expansions"] += int(line.split()[1])
+        elif line.startswith("[x] reseed rounds"):
+            tot["reseed_rounds"] += int(re.match(r"\[x\] reseed rounds (\d+)", line).group(1))
+            for name, t, _ in re.findall(r" (\S+) ([\d.]+)/(\d+)", line.split(":", 1)[1]):
+                us[name] += float(t)
+        elif line.startswith("[x] work-list entries:"):
+            mm = re.search(r"evaluated (\d+) refreshed (\d+) reseeded (\d+)", line)
+            tot["evaluated"] += int(mm.group(1)); tot["refreshed"] += int(mm.group(2)); tot["reseeded"] += int(mm.group(3))
+        elif line.startswith("[x] gens "):
+            mm = re.match(r"\[x\] gens (\d+) rounds (\d+)", line)
+            tot["generations"] += int(mm.group(1)); tot["rounds"] += int(mm.group(2))
+            gens[f] = [tuple(int(v) for v in t.split("/")[:2]) for t in line.split("|", 1)[1].split()]
+    out = ["workload %s, frames %d-%d, phase totals of k_x_relax (ms):" % (args.workload, lo, hi - 1)]
+    for k in PHASES:
+        if k != "empty-barrier":
+            out.append("  %-16s %9.2f" % (k, us[k] / 1000.0))
+    out.append("  %-16s %9.2f" % ("sum", sum(v for k, v in us.items() if k != "empty-barrier") / 1000.0))
+    out.append("  %-16s %9.2f us per empty grid barrier (mean over the frames)" % ("empty-barrier", us["empty-barrier"] / max(1, hi - lo)))
+    for k in ("generations", "rounds", "evaluated", "refreshed", "reseed_rounds", "reseeded", "expansions"):
+        out.append("total %s %d" % (k, tot[k]))
+    for fr in sorted(gens):
+        out.append("frame %d nE %s" % (fr, " ".join(str(n) for n, _ in gens[fr])))
+    for fr in sorted(gens):
+        out.append("frame %d rounds %s" % (fr, " ".join(str(r) for _, r in gens[fr])))
+    text = "\n".join(out) + "\n"
+    sys.stdout.write(text)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        open(args.out, "w").write(text)
+
+
+if __name__ == "__main__":
+    main()
