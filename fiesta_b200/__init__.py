@@ -61,6 +61,11 @@ class ViewpointStats(C.Structure):
         ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
 
 
+class CorridorStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("boxes", "layers_tested", "layers_grown", "mask_voxels")] + [
+        ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
+
+
 class Stats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
         "occupancy_updates", "inserts", "deletes", "voxels_changed", "expansions", "voxels_reset", "tile_visits", "generations",
@@ -92,6 +97,7 @@ SYMBOLS = [
     "fiesta_nav_create", "fiesta_nav_destroy", "fiesta_nav_compute", "fiesta_nav_export", "fiesta_nav_paths",
     "fiesta_frontiers_create", "fiesta_frontiers_destroy", "fiesta_frontiers_compute", "fiesta_frontiers_clusters",
     "fiesta_frontiers_voxels", "fiesta_frontiers_export", "fiesta_frontiers_score_viewpoints",
+    "fiesta_inflate_boxes", "fiesta_corridors",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -158,6 +164,8 @@ def load_library():
         L.fiesta_frontiers_export.argtypes = [C.c_void_p, C.c_void_p]
         L.fiesta_frontiers_score_viewpoints.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
                                                         C.POINTER(SensorModel), C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.fiesta_inflate_boxes.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 4
+        L.fiesta_corridors.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 7
         L.fiesta_get_distance_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
         L.fiesta_get_dist_grad_trilinear_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
@@ -414,6 +422,7 @@ class ESDFMap:
         self._L.fiesta_grid_size(self._h, g)
         self.grid_size = tuple(int(x) for x in g)
         self.resolution = float(resolution)
+        self.origin = tuple(float(x) for x in origin)
         self.device = int(device)
 
     def _ck(self, rc, what):
@@ -548,6 +557,59 @@ class ESDFMap:
         self._ck(self._L.fiesta_get_dist_grad_trilinear_batch_device(self._h, pos.data_ptr(), pos.shape[0], d.data_ptr(), g.data_ptr(), stream),
                  "GetDistWithGradTrilinearBatchDevice")
         return d, g
+
+    # --- safe flight corridors: free axis-aligned voxel boxes in a limit box (fiesta_inflate_boxes, fiesta_corridors) ---
+    def _corridor_args(self, box_lo, box_hi, max_steps, what):
+        lo, hi = np.ascontiguousarray(box_lo, dtype=np.int32), np.ascontiguousarray(box_hi, dtype=np.int32)
+        ms = np.ascontiguousarray(max_steps, dtype=np.int32)
+        if lo.shape != (3,) or hi.shape != (3,) or ms.shape != (3,):
+            raise ValueError("%s: box_lo, box_hi and max_steps must be 3 integers each" % what)
+        return lo, hi, ms
+
+    def InflateBoxes(self, seed_lo, seed_hi, box_lo, box_hi, max_steps, clearance, unknown_blocks=False):
+        """Inflate n independent seed boxes (n, 3) inclusive grid voxels inside the limit box [box_lo, box_hi] ->
+        (status (n,) int32, lo (n, 3), hi (n, 3) int32 (-1 unless status 0), stats dict)."""
+        lo, hi, ms = self._corridor_args(box_lo, box_hi, max_steps, "InflateBoxes")
+        slo = np.ascontiguousarray(seed_lo, dtype=np.int32).reshape(-1, 3)
+        shi = np.ascontiguousarray(seed_hi, dtype=np.int32).reshape(-1, 3)
+        if len(slo) != len(shi):
+            raise ValueError("InflateBoxes: %d lower and %d upper seed corners" % (len(slo), len(shi)))
+        n = len(slo)
+        status, olo, ohi = np.empty(n, np.int32), np.empty((n, 3), np.int32), np.empty((n, 3), np.int32)
+        st = CorridorStats()
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        self._ck(self._L.fiesta_inflate_boxes(self._h, lo.ctypes, hi.ctypes, slo.ctypes, shi.ctypes, C.c_int64(n), ms.ctypes, r, flags,
+                                              status.ctypes, olo.ctypes, ohi.ctypes, C.byref(st)), "InflateBoxes")
+        return status, olo, ohi, {k: getattr(st, k) for k, _ in st._fields_ if k != "reserved_f"}
+
+    def Corridors(self, paths, box_lo, box_hi, max_steps, clearance, unknown_blocks=False):
+        """Chains of overlapping free boxes along paths inside the limit box [box_lo, box_hi].  paths: a list of (L_i, 3) grid-voxel
+        arrays, or the (status, len, cost, vox) tuple of NavField.paths (path i is vox[i, :len[i]]) -> (status (n,), n_boxes (n,),
+        blocked_at (n,) int32, [(lo (k, 3), hi (k, 3), first (k,)) per path], stats dict)."""
+        lo, hi, ms = self._corridor_args(box_lo, box_hi, max_steps, "Corridors")
+        if isinstance(paths, tuple) and len(paths) == 4:
+            _, ln, _, vox = paths
+            paths = [vox[i, :int(ln[i])] for i in range(len(ln))]
+        P = [np.ascontiguousarray(p, dtype=np.int32).reshape(-1, 3) for p in paths]
+        n = len(P)
+        off = np.zeros(n + 1, np.int64)
+        off[1:] = np.cumsum([len(p) for p in P])
+        vox = np.ascontiguousarray(np.concatenate(P) if n else np.zeros((0, 3), np.int32))
+        T = int(off[-1])
+        status, nb, bl = np.empty(n, np.int32), np.empty(n, np.int32), np.empty(n, np.int32)
+        blo, bhi, first = np.empty((T, 3), np.int32), np.empty((T, 3), np.int32), np.empty(T, np.int32)
+        st = CorridorStats()
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        self._ck(self._L.fiesta_corridors(self._h, lo.ctypes, hi.ctypes, vox.ctypes, off.ctypes, C.c_int64(n), ms.ctypes, r, flags,
+                                          status.ctypes, nb.ctypes, bl.ctypes, blo.ctypes, bhi.ctypes, first.ctypes, C.byref(st)),
+                 "Corridors")
+        boxes = [(blo[off[i]:off[i] + nb[i]], bhi[off[i]:off[i] + nb[i]], first[off[i]:off[i] + nb[i]]) for i in range(n)]
+        return status, nb, bl, boxes, {k: getattr(st, k) for k, _ in st._fields_ if k != "reserved_f"}
+
+    def box_corners(self, lo, hi):
+        """Metric corners of inclusive voxel boxes: (lo * resolution + origin, (hi + 1) * resolution + origin)."""
+        o = np.asarray(self.origin)
+        return np.asarray(lo) * self.resolution + o, (np.asarray(hi) + 1) * self.resolution + o
 
     # --- Fiesta::RaycastMultithread (Fiesta.h:281-303), serial semantics ---
     def QueryPlan(self, n):

@@ -248,6 +248,25 @@ struct FbViewBufs {                // device buffers of fiesta_frontiers_score_v
 int fb_view_score(const FbGeom &g, const uint32_t *cobs, const int64_t *size, const int32_t *m_xyz, unsigned K, FbViewBufs &V,
                   FbDevBuf<char> &tmp, long long n, int n_orient, const fiesta_sensor_model &sm, double clearance, int unknown_blocks,
                   cudaStream_t s, int *launches);
+// safe flight corridors (fb_corridor.cu); L_lo / L_hi: the limit box, inclusive grid voxels
+struct FbCorrCtr {
+  unsigned long long boxes, tested, grown;   // boxes written (seeds inflated), layer tests, grown layers
+};
+struct FbCorrBufs {                // device buffers of fiesta_inflate_boxes / fiesta_corridors, kept on the map
+  FbDevBuf<uint32_t> mask;         // the limit box's traversable bits, z-rows then y-rows (fb_corridor.h)
+  FbDevBuf<int32_t> in;            // seeds [lo 3n][hi 3n], or path voxels [3 total]
+  FbDevBuf<int64_t> off;           // path offsets [n_paths + 1]
+  FbDevBuf<int32_t> out;           // seeds: [status n][lo 3n][hi 3n]; paths: [status][n_boxes][blocked_at] x n_paths, [lo 3T][hi 3T][first T]
+  FbDevBuf<FbCorrCtr> ctr;
+  FbHostBuf<FbCorrCtr> h_ctr;
+};
+cudaError_t fb_corr_launch_mask(const FbGeom &g, const uint32_t *cobs, const int *L_lo, const int *L_hi, double r, int unknown_blocks,
+                                uint32_t *mask, cudaStream_t s);
+cudaError_t fb_corr_launch_seeds(const int *L_lo, const int *L_hi, const int *max_steps, const uint32_t *mask, const int32_t *seeds,
+                                 long long n, int32_t *status, int32_t *out_lo, int32_t *out_hi, FbCorrCtr *ctr, cudaStream_t s);
+cudaError_t fb_corr_launch_paths(const int *L_lo, const int *L_hi, const int *max_steps, const uint32_t *mask, const int32_t *P,
+                                 const int64_t *off, long long n_paths, int32_t *status, int32_t *n_boxes, int32_t *blocked_at,
+                                 int32_t *box_lo, int32_t *box_hi, int32_t *first, FbCorrCtr *ctr, cudaStream_t s);
 struct FbDepthRel { double m[16]; };
 struct fiesta_depth_params;
 cudaError_t fb_depth_to_cloud(const uint16_t *d_img, const uint16_t *d_last, int rows, int cols, const fiesta_depth_params &p, int filter_on,

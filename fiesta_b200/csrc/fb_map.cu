@@ -15,6 +15,7 @@
 #include "fb_common.cuh"
 #include "fb_exact.h"
 #include "fb_segment.h"
+#include "fb_corridor.h"
 
 static thread_local std::string g_last_error;
 void fb_set_error(const char *fmt, ...) {
@@ -61,6 +62,7 @@ struct fiesta_map {
   // queries
   FbDevBuf<double> d_qin, d_qout;
   FbDevBuf<char> d_seg;             // fiesta_check_segments: [ab 6n][hit_t n][min_dist n] doubles, [hit_idx n] int64, [status n] int32
+  FbCorrBufs corr;                  // fiesta_inflate_boxes / fiesta_corridors
   cudaEvent_t ev[4] = {};
   cudaEvent_t ev_q[2] = {};         // device queries: map stream -> caller's stream, and back
   FbDevBuf<unsigned long long> d_dbg;
@@ -1255,6 +1257,122 @@ int fiesta_frontiers_score_viewpoints(fiesta_frontiers *f, const int32_t *cluste
     CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
   }
   return FIESTA_OK;
+}
+
+// ---- safe flight corridors (fb_corridor.h, fb_corridor.cu): free boxes inflated in a limit box, and chains of them along paths
+static bool corridor_args_ok(const char *fn, const fiesta_map *m, const int *box_lo, const int *box_hi, const int32_t *max_steps,
+                             int64_t n, double clearance, int flags, bool buffers) {
+  if (!m || !box_lo || !box_hi || !max_steps) { fb_set_error("%s: null argument", fn); return false; }
+  if (!segment_args_ok(fn, n, clearance, flags, buffers)) return false;
+  const int gs[3] = {m->g.gx, m->g.gy, m->g.gz};
+  for (int k = 0; k < 3; ++k) {
+    if (!(box_lo[k] >= 0 && box_lo[k] <= box_hi[k] && box_hi[k] < gs[k])) {
+      fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
+      return false;
+    }
+    if (max_steps[k] < 0) { fb_set_error("%s: max_steps must be >= 0", fn); return false; }
+  }
+  return true;
+}
+// Grow the buffers, then record the start event and build the limit box's masks.
+static int corridor_begin(fiesta_map *m, const char *fn, const int *box_lo, const int *box_hi, double clearance, int flags,
+                          size_t in_words, size_t off_words, size_t out_words) {
+  FbCorrBufs &B = m->corr;
+  const FbCorrMask M = fb_corr_mask_geom(box_lo, box_hi);
+  const cudaStream_t s = m->stream;
+  CK(cudaSetDevice(m->device));
+  cudaError_t e = B.mask.grow((size_t)fb_corr_mask_words(M), s);
+  if (e == cudaSuccess) e = B.in.grow(in_words, s);
+  if (e == cudaSuccess && off_words) e = B.off.grow(off_words, s);
+  if (e == cudaSuccess) e = B.out.grow(out_words, s);
+  if (e == cudaSuccess) e = B.ctr.grow(1, s);
+  if (e == cudaSuccess && !B.h_ctr) e = B.h_ctr.alloc(1);
+  if (e != cudaSuccess) {
+    cudaGetLastError();                                                   // not sticky: later calls must not see it
+    fb_set_error("%s: cannot allocate the buffers: %s", fn, cudaGetErrorString(e));
+    return FIESTA_ERR_CUDA;
+  }
+  CK(cudaEventRecord(m->ev[0], s));
+  CK(cudaMemsetAsync(B.ctr, 0, sizeof(FbCorrCtr), s));
+  CK(fb_corr_launch_mask(m->g, m->cobs, box_lo, box_hi, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, B.mask, s));
+  m->st.kernel_launches += 2;
+  return FIESTA_OK;
+}
+// After the copies out have been enqueued: synchronise and fill the statistics.
+static int corridor_end(fiesta_map *m, const int *box_lo, const int *box_hi, fiesta_corridor_stats *stats) {
+  FbCorrBufs &B = m->corr;
+  CK(cudaEventRecord(m->ev[1], m->stream));
+  CK(cudaMemcpyAsync(B.h_ctr, B.ctr, sizeof(FbCorrCtr), cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  if (stats) {
+    *stats = fiesta_corridor_stats{};
+    stats->boxes = (int64_t)B.h_ctr->boxes;
+    stats->layers_tested = (int64_t)B.h_ctr->tested;
+    stats->layers_grown = (int64_t)B.h_ctr->grown;
+    stats->mask_voxels = 1;
+    for (int k = 0; k < 3; ++k) stats->mask_voxels *= (int64_t)(box_hi[k] - box_lo[k] + 1);
+    CK(cudaEventElapsedTime(&stats->ms_compute, m->ev[0], m->ev[1]));
+  }
+  return FIESTA_OK;
+}
+int fiesta_inflate_boxes(fiesta_map *m, const int box_lo[3], const int box_hi[3], const int32_t *seed_lo_xyz, const int32_t *seed_hi_xyz,
+                         int64_t n, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *out_lo_xyz,
+                         int32_t *out_hi_xyz, fiesta_corridor_stats *stats) {
+  const char *fn = "fiesta_inflate_boxes";
+  if (!corridor_args_ok(fn, m, box_lo, box_hi, max_steps, n, clearance, flags, seed_lo_xyz && seed_hi_xyz && status && out_lo_xyz && out_hi_xyz))
+    return FIESTA_ERR_INVALID;
+  if (n >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 seeds per call", fn); return FIESTA_ERR_LIMIT; }
+  if (stats) *stats = fiesta_corridor_stats{};
+  if (n == 0) return FIESTA_OK;
+  int r;
+  if ((r = corridor_begin(m, fn, box_lo, box_hi, clearance, flags, (size_t)n * 6, 0, (size_t)n * 7))) return r;
+  FbCorrBufs &B = m->corr;
+  const cudaStream_t s = m->stream;
+  int32_t *d_st = B.out, *d_lo = d_st + n, *d_hi = d_lo + 3 * n;
+  CK(cudaMemcpyAsync(B.in, seed_lo_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(B.in + 3 * n, seed_hi_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, s));
+  CK(fb_corr_launch_seeds(box_lo, box_hi, max_steps, B.mask, B.in, n, d_st, d_lo, d_hi, B.ctr, s));
+  m->st.kernel_launches++;
+  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out_lo_xyz, d_lo, (size_t)n * 12, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out_hi_xyz, d_hi, (size_t)n * 12, cudaMemcpyDeviceToHost, s));
+  return corridor_end(m, box_lo, box_hi, stats);
+}
+int fiesta_corridors(fiesta_map *m, const int box_lo[3], const int box_hi[3], const int32_t *path_vox_xyz, const int64_t *path_off,
+                     int64_t n_paths, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *n_boxes,
+                     int32_t *blocked_at, int32_t *box_lo_xyz, int32_t *box_hi_xyz, int32_t *first, fiesta_corridor_stats *stats) {
+  const char *fn = "fiesta_corridors";
+  if (!corridor_args_ok(fn, m, box_lo, box_hi, max_steps, n_paths, clearance, flags, path_off && status && n_boxes && blocked_at))
+    return FIESTA_ERR_INVALID;
+  if (n_paths > 0 && path_off[0] != 0) { fb_set_error("%s: path_off[0] must be 0", fn); return FIESTA_ERR_INVALID; }
+  for (int64_t p = 0; p < n_paths; ++p)
+    if (path_off[p + 1] < path_off[p]) { fb_set_error("%s: path_off decreases at %lld", fn, (long long)p); return FIESTA_ERR_INVALID; }
+  const int64_t total = n_paths > 0 ? path_off[n_paths] : 0;
+  if (total > 0 && !(path_vox_xyz && box_lo_xyz && box_hi_xyz && first)) { fb_set_error("%s: null buffer", fn); return FIESTA_ERR_INVALID; }
+  if (total >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 path voxels per call", fn); return FIESTA_ERR_LIMIT; }
+  if (stats) *stats = fiesta_corridor_stats{};
+  if (total == 0) {                                                       // only empty paths: status 0, no boxes
+    for (int64_t p = 0; p < n_paths; ++p) { status[p] = FB_CORR_OK; n_boxes[p] = 0; blocked_at[p] = -1; }
+    return FIESTA_OK;
+  }
+  const size_t T = (size_t)total, np = (size_t)n_paths;
+  int r;
+  if ((r = corridor_begin(m, fn, box_lo, box_hi, clearance, flags, T * 3, np + 1, np * 3 + T * 7))) return r;
+  FbCorrBufs &B = m->corr;
+  const cudaStream_t s = m->stream;
+  int32_t *d_st = B.out, *d_nb = d_st + np, *d_bl = d_nb + np, *d_lo = d_bl + np, *d_hi = d_lo + 3 * T, *d_first = d_hi + 3 * T;
+  CK(cudaMemcpyAsync(B.in, path_vox_xyz, T * 12, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(B.off, path_off, (np + 1) * 8, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(d_lo, 0xff, T * 28, s));                            // -1 in every slot no box is written to
+  CK(fb_corr_launch_paths(box_lo, box_hi, max_steps, B.mask, B.in, B.off, n_paths, d_st, d_nb, d_bl, d_lo, d_hi, d_first, B.ctr, s));
+  m->st.kernel_launches++;
+  CK(cudaMemcpyAsync(status, d_st, np * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(n_boxes, d_nb, np * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(blocked_at, d_bl, np * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(box_lo_xyz, d_lo, T * 12, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(box_hi_xyz, d_hi, T * 12, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(first, d_first, T * 4, cudaMemcpyDeviceToHost, s));
+  return corridor_end(m, box_lo, box_hi, stats);
 }
 
 // ---- planner query plan: fixed batch size, pinned host buffers, the copy-in / kernel / copy-out sequence captured once as a

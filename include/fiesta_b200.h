@@ -357,6 +357,53 @@ int fiesta_frontiers_score_viewpoints(fiesta_frontiers *f, const int32_t *cluste
                                       double clearance, int flags, int32_t *status, int32_t *score /* n * n_orient, row i = candidate i */,
                                       fiesta_viewpoint_stats *stats /* nullable */);
 
+/* ---- safe flight corridors (corridor-based trajectory planners: free convex regions around a path) ----
+ * Free axis-aligned voxel boxes, inflated face by face, and chains of them along paths in which consecutive boxes share a voxel.
+ * All boxes are inclusive voxel boxes; the limit box L = [box_lo, box_hi] satisfies 0 <= lo <= hi < grid size on every axis.
+ *   traversable  a voxel of L that does not block at `clearance` with `flags` in the sense of fiesta_check_segments
+ *                (GetDistance(Vector3i) <= clearance blocks; with FIESTA_SEGMENT_UNKNOWN_BLOCKS a never-observed voxel blocks too):
+ *                the traversable voxels of a cost-to-go field over L.
+ *   inflation    of a seed box S whose voxels are all traversable: B = S, all six faces active; rounds visit the faces in the
+ *                order -x, +x, -y, +y, -z, +z.  An active face that has reached L or max_steps[axis] (>= 0) layers beyond S's face
+ *                is deactivated; otherwise the one-voxel layer just outside it, spanning B's current extent on the other two
+ *                axes, is tested: if every voxel is traversable B grows by it, else the face is deactivated for good.  Stops when
+ *                no face is active.  The result is traversable and maximal: each face sits on L or its max_steps, or its next
+ *                layer holds a non-traversable voxel.  The face order is part of the definition.
+ *   corridor     of a path P[0..n-1] (grid voxels): status 2 and no boxes if some P[i] lies outside L.  Otherwise box 0 inflates
+ *                {P[0]}; after a box whose seed index is j, let i be the first index > j with P[i] outside it: none -> status
+ *                0; else the next box inflates AABB(P[i-1], P[i]) with seed index i, so consecutive boxes share P[i-1].  A seed
+ *                that holds a non-traversable voxel ends the corridor with status 1 and blocked_at = its seed index; the boxes
+ *                before it are kept.  An empty path has status 0 and no boxes; a path of n voxels has at most n boxes.  The
+ *                path of a cost-to-go field over the same L at the same clearance and flags, on unchanged records, never gets
+ *                status 1 (each of its moves spans a traversable box).
+ * The records are read as they are at the time of the call.  Every output is an integer: the same on every run and as the
+ * sequential rule (tests/corridorref.py).  Memory on the map, grown as needed: 2 bits per limit-box voxel (32 MB for a 512^3 box),
+ * 52 bytes per seed, or 40 per path voxel and 20 per path.  Host pointers, the map's stream, synchronous.  Errors (nothing is
+ * written): FIESTA_ERR_INVALID for a box outside the grid or inverted, a clearance or flags that fiesta_check_segments rejects, a
+ * negative max_steps entry, n or n_paths, offsets that do not start at 0 or that decrease, or null buffers where work exists
+ * (box_lo, box_hi and max_steps are always needed); FIESTA_ERR_LIMIT when n or the number of path voxels is >= 2^31 - 1;
+ * FIESTA_ERR_CUDA when the buffers cannot be allocated. */
+typedef struct fiesta_corridor_stats {
+  int64_t boxes;                          /* boxes written (corridors) or seeds inflated (inflate) */
+  int64_t layers_tested;                  /* layer tests of the sequential rule (grown + refused); schedule-independent */
+  int64_t layers_grown;
+  int64_t mask_voxels;                    /* limit-box voxels evaluated (0 when there is no seed or path voxel) */
+  float ms_compute;                       /* device time of the whole call */
+  float reserved_f[1];
+} fiesta_corridor_stats;
+/* Independent seeds: n inclusive seed boxes -> inflated boxes.  status 0 ok; 1 the seed holds a non-traversable voxel; 2 the seed
+ * is inverted or not inside L.  out_lo / out_hi are -1 for status 1 and 2. */
+int fiesta_inflate_boxes(fiesta_map *m, const int box_lo[3], const int box_hi[3], const int32_t *seed_lo_xyz, const int32_t *seed_hi_xyz,
+                         int64_t n, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *out_lo_xyz,
+                         int32_t *out_hi_xyz, fiesta_corridor_stats *stats /* nullable */);
+/* n_paths paths, their grid voxels (xyz int32) concatenated, with offsets path_off[0] = 0 <= ... <= path_off[n_paths] = total.
+ * Box k of path p is written to slot path_off[p] + k (k < n_boxes[p]) of box_lo_xyz / box_hi_xyz / first (total slots each);
+ * every other slot is -1.  first[slot] = the box's seed index within its path; blocked_at[p] = that index for status 1, else -1. */
+int fiesta_corridors(fiesta_map *m, const int box_lo[3], const int box_hi[3], const int32_t *path_vox_xyz, const int64_t *path_off,
+                     int64_t n_paths, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *n_boxes,
+                     int32_t *blocked_at, int32_t *box_lo_xyz, int32_t *box_hi_xyz, int32_t *first,
+                     fiesta_corridor_stats *stats /* nullable */);
+
 /* ---- stream-ordered queries on DEVICE buffers (GPU planners whose positions already live in HBM) ----
  * The same queries on device pointers valid on the map's device, enqueued on `stream` (a cudaStream_t; 0 = the legacy default
  * stream); they return without synchronising the host.  Ordering: the query sees every map update issued before the call (the

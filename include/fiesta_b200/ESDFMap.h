@@ -193,6 +193,24 @@ class ESDFMap {
     check(fiesta_frontiers_score_viewpoints(f, cluster, pos_xyz, n, orient, n_orient, &sensor, clearance, flags, status, score, &st), "ScoreViewpoints");
     return st;
   }
+  // Safe flight corridors (fiesta_inflate_boxes / fiesta_corridors in fiesta_b200.h): free axis-aligned voxel boxes in a limit box,
+  // and chains of them along paths in which consecutive boxes share a voxel.
+  fiesta_corridor_stats InflateBoxes(const int box_lo[3], const int box_hi[3], const int32_t *seed_lo_xyz, const int32_t *seed_hi_xyz,
+                                     long n, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *out_lo_xyz,
+                                     int32_t *out_hi_xyz) {
+    fiesta_corridor_stats st = {};
+    check(fiesta_inflate_boxes(h_, box_lo, box_hi, seed_lo_xyz, seed_hi_xyz, n, max_steps, clearance, flags, status, out_lo_xyz, out_hi_xyz, &st),
+          "InflateBoxes");
+    return st;
+  }
+  fiesta_corridor_stats Corridors(const int box_lo[3], const int box_hi[3], const int32_t *path_vox_xyz, const int64_t *path_off, long n_paths,
+                                  const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *n_boxes, int32_t *blocked_at,
+                                  int32_t *box_lo_xyz, int32_t *box_hi_xyz, int32_t *first) {
+    fiesta_corridor_stats st = {};
+    check(fiesta_corridors(h_, box_lo, box_hi, path_vox_xyz, path_off, n_paths, max_steps, clearance, flags, status, n_boxes, blocked_at,
+                           box_lo_xyz, box_hi_xyz, first, &st), "Corridors");
+    return st;
+  }
   void GetDistanceBatchDevice(const double *d_pos_xyz, long n, double *d_dist, void *stream) {
     check(fiesta_get_distance_batch_device(h_, d_pos_xyz, n, d_dist, stream), "GetDistanceBatchDevice");
   }
