@@ -47,6 +47,11 @@ class NavStats(C.Structure):
         ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
 
 
+class NavMatrixStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("sources_placed", "targets_placed", "passes", "generations", "tile_visits",
+                                         "sources_retired_early")] + [("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
+
+
 class FrontierStats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("box_voxels", "frontier_voxels", "clusters", "kept_clusters", "kept_voxels")] + [
         ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
@@ -95,6 +100,7 @@ SYMBOLS = [
     "fiesta_check_segments", "fiesta_check_segments_device", "fiesta_get_distance_batch_device",
     "fiesta_get_dist_grad_trilinear_batch_device", "fiesta_host_mirror_check_segments",
     "fiesta_nav_create", "fiesta_nav_destroy", "fiesta_nav_compute", "fiesta_nav_export", "fiesta_nav_paths",
+    "fiesta_nav_matrix",
     "fiesta_frontiers_create", "fiesta_frontiers_destroy", "fiesta_frontiers_compute", "fiesta_frontiers_clusters",
     "fiesta_frontiers_voxels", "fiesta_frontiers_export", "fiesta_frontiers_score_viewpoints",
     "fiesta_inflate_boxes", "fiesta_corridors",
@@ -155,6 +161,7 @@ def load_library():
         L.fiesta_nav_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_int, C.c_void_p]
         L.fiesta_nav_export.argtypes = [C.c_void_p, C.c_void_p]
         L.fiesta_nav_paths.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 4
+        L.fiesta_nav_matrix.argtypes = [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_int64, C.c_double, C.c_int] + [C.c_void_p] * 4
         L.fiesta_frontiers_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
         L.fiesta_frontiers_destroy.argtypes = [C.c_void_p]
         L.fiesta_frontiers_destroy.restype = None
@@ -314,6 +321,24 @@ class NavField:
         self._m._ck(self._m._L.fiesta_nav_paths(self._h, starts.ctypes, C.c_int64(n), C.c_int32(int(max_len)), st.ctypes, ln.ctypes,
                                                 cost.ctypes, vox.ctypes), "NavField.paths")
         return st, ln, cost, vox
+
+    def matrix(self, box_lo, box_hi, sources, targets, clearance, unknown_blocks=False):
+        """Geodesic costs from every source to every target (positions (n, 3) in metres) through the free space of the inclusive voxel
+        box [box_lo, box_hi] -> (cost (n_src, n_tgt), src_status (n_src,), tgt_status (n_tgt,), stats dict).  Row i is the field
+        of compute(goals=[source i]) read at the targets; NaN where a point's status is not 0.  The last computed field, its
+        export() and paths() are left as they were."""
+        lo, hi = np.ascontiguousarray(box_lo, dtype=np.int32), np.ascontiguousarray(box_hi, dtype=np.int32)
+        if lo.shape != (3,) or hi.shape != (3,):
+            raise ValueError("NavField.matrix: box_lo and box_hi must be 3 voxel coordinates each")
+        src, tgt = _f64(sources).reshape(-1, 3), _f64(targets).reshape(-1, 3)
+        ns, nt = len(src), len(tgt)
+        cost = np.empty((ns, nt))
+        ss, ts = np.empty(ns, np.int32), np.empty(nt, np.int32)
+        st = NavMatrixStats()
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        self._m._ck(self._m._L.fiesta_nav_matrix(self._h, lo.ctypes, hi.ctypes, src.ctypes, C.c_int64(ns), tgt.ctypes, C.c_int64(nt), r,
+                                                 flags, ss.ctypes, ts.ctypes, cost.ctypes, C.byref(st)), "NavField.matrix")
+        return cost, ss, ts, {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved_f"}
 
     def close(self):
         if self._h:

@@ -200,6 +200,38 @@ cudaError_t fb_nav_compute(const FbGeom &g, const uint32_t *cobs, const FbNavArg
 int fb_nav_relax_blocks(int device);
 cudaError_t fb_nav_paths(const FbGeom &g, const FbNavBox &b, const double *D, const double *w, const double *starts, long long n, int max_len,
                          int32_t *status, int32_t *len, double *cost, int32_t *vox, cudaStream_t s);
+// cost matrices (fb_navmatrix.cu): up to FB_NAVM_CH sources' fields relaxed together, one channel each
+#define FB_NAVM_CH 32
+struct FbNavMCtr {                 // per pass; zeroed before it
+  unsigned n[3], next[3];          // work-list lengths and fetch counters, rotating by generation as in FbNavCtr
+  unsigned long long mmin[FB_NAVM_CH][3];   // per channel: bits of the least value written in generation g, slot g % 3
+  unsigned queued[FB_NAVM_CH][3];           // per channel: work items queued for generation g, slot g % 3
+  unsigned retired[FB_NAVM_CH];             // the channel's targets are final: its work items are dropped
+};
+struct FbNavMTot {                 // summed over the passes of a call
+  unsigned long long generations, tile_visits, retired_early;
+};
+struct FbNavMArgs {
+  double *D;                       // [channel][box index] (fb_nav.h layout); +inf until reached
+  const uint32_t *M;               // per box voxel: fb_nav_move_bits
+  FbNavBox b;
+  int tn[3];                       // 8^3 tiles per box axis
+  unsigned nt;                     // tiles per channel; a work item is channel * nt + tile
+  long long nv;                    // box voxels
+  double w[3];
+  uint32_t *stamp;                 // per work item: stamp of the generation it is queued for (generation g has stamp g + 1)
+  uint32_t *list[2];               // work lists by generation parity
+  FbNavMCtr *ctr;
+  FbNavMTot *tot;
+  const long long *tgt;            // box indices of the status-0 targets
+  int n_tgt, nch;                  // status-0 targets, channels of this pass
+};
+int fb_navm_relax_blocks(int device);
+cudaError_t fb_navm_locate(const FbGeom &g, const uint32_t *cobs, const FbNavBox &b, double r, int unknown_blocks, uint32_t *M,
+                           const double *pts, long long n, int32_t *status, long long *idx, cudaStream_t s);
+cudaError_t fb_navm_pass(const FbNavMArgs &a, const long long *src_idx, int nblocks, cudaStream_t s);
+cudaError_t fb_navm_gather(const double *D, long long nv, const int32_t *rows, long long n_rows, const long long *tgt_idx, long long n_tgt,
+                           double *cost, cudaStream_t s);
 // frontier extraction (fb_frontier.cu)
 struct FbFrCtr {
   unsigned long long frontier;     // frontier voxels of the box

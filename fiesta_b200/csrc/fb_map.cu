@@ -9,8 +9,10 @@
 #include <stdlib.h>
 #include <string.h>
 #include <string>
+#include <algorithm>
 #include <memory>
 #include <new>
+#include <vector>
 #include "../../include/fiesta_b200.h"
 #include "fb_common.cuh"
 #include "fb_exact.h"
@@ -952,6 +954,16 @@ struct fiesta_nav_field {
   FbHostBuf<FbNavCtr> h_ctr;
   FbDevBuf<double> d_pd;            // fiesta_nav_paths: [starts 3n][cost n]
   FbDevBuf<int32_t> d_pi;           //                   [status n][len n][vox 3 n max_len]
+  // fiesta_nav_matrix: its own buffers, so that a matrix leaves the last field, export and paths as they were
+  int mblocks = 0;                  // co-resident CTAs of k_navm_relax
+  FbDevBuf<uint32_t> M;             // per box voxel: move mask
+  FbDevBuf<double> MD, m_pts, m_cost;   // [channel][box voxel] fields; points [sources 3 n_src][targets 3 n_tgt]; cost
+  FbDevBuf<uint32_t> m_stamp, m_list[2];  // per (channel, tile)
+  FbDevBuf<int32_t> m_st, m_rows;   // per point: status; rows: placed sources in index order, then the others
+  FbDevBuf<long long> m_idx, m_src, m_tgt;  // per point: box index or -1; placed sources' box indices; placed targets' box indices
+  FbDevBuf<FbNavMCtr> m_ctr;
+  FbDevBuf<FbNavMTot> m_tot;
+  FbHostBuf<FbNavMTot> h_mtot;
   cudaEvent_t ev[2] = {};
   FbNavBox box{};
   double w[3]{};
@@ -972,10 +984,14 @@ int fiesta_nav_create(fiesta_map *m, fiesta_nav_field **out) {
   if (!f) { fb_set_error("out of host memory"); return FIESTA_ERR_INVALID; }
   f->m = m;
   f->blocks = fb_nav_relax_blocks(m->device);
-  if (f->blocks <= 0) { fb_set_error("fiesta_nav_create: the relaxation kernel does not fit on this device"); return FIESTA_ERR_CUDA; }
+  f->mblocks = fb_navm_relax_blocks(m->device);
+  if (f->blocks <= 0 || f->mblocks <= 0) { fb_set_error("fiesta_nav_create: the relaxation kernel does not fit on this device"); return FIESTA_ERR_CUDA; }
   for (cudaEvent_t &e : f->ev) CK(cudaEventCreate(&e));
   CK(f->ctr.alloc(1));
   CK(f->h_ctr.alloc(1));
+  CK(f->m_ctr.alloc(1));
+  CK(f->m_tot.alloc(1));
+  CK(f->h_mtot.alloc(1));
   for (int k = 0; k < 3; ++k) f->w[k] = m->g.res * sqrt((double)(k + 1));
   *out = f.release();
   return FIESTA_OK;
@@ -1075,6 +1091,141 @@ int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, i
   CK(cudaMemcpyAsync(cost, d_cost, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
   CK(cudaMemcpyAsync(vox_xyz, d_vox, nv * 4, cudaMemcpyDeviceToHost, m->stream));
   CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+int fiesta_nav_matrix(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *sources_xyz, int64_t n_src,
+                      const double *targets_xyz, int64_t n_tgt, double clearance, int flags, int32_t *src_status, int32_t *tgt_status,
+                      double *cost, fiesta_nav_matrix_stats *stats) {
+  const char *fn = "fiesta_nav_matrix";
+  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (n_src < 0 || n_tgt < 0 || (n_src > 0 && !(sources_xyz && src_status)) || (n_tgt > 0 && !(targets_xyz && tgt_status)) ||
+      (n_src > 0 && n_tgt > 0 && !cost)) {
+    fb_set_error("%s: negative count or null buffer", fn);
+    return FIESTA_ERR_INVALID;
+  }
+  if (!segment_args_ok(fn, 0, clearance, flags, true)) return FIESTA_ERR_INVALID;
+  fiesta_map *m = f->m;
+  const int gs[3] = {m->g.gx, m->g.gy, m->g.gz};
+  FbNavMArgs a{};
+  for (int k = 0; k < 3; ++k) {
+    if (!(box_lo[k] >= 0 && box_lo[k] <= box_hi[k] && box_hi[k] < gs[k])) {
+      fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
+      return FIESTA_ERR_INVALID;
+    }
+    a.b.lo[k] = box_lo[k];
+    a.b.n[k] = box_hi[k] - box_lo[k] + 1;
+    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
+    a.w[k] = f->w[k];
+  }
+  if (n_src > 0 && n_tgt > 0 && n_src >= ((1ll << 31) + n_tgt - 1) / n_tgt) {
+    fb_set_error("%s: n_src * n_tgt must be below 2^31", fn);
+    return FIESTA_ERR_LIMIT;
+  }
+  const long long nv = (long long)a.b.n[0] * a.b.n[1] * a.b.n[2], nt = (long long)a.tn[0] * a.tn[1] * a.tn[2], np = n_src + n_tgt;
+  a.nv = nv;
+  a.nt = (unsigned)nt;
+  cudaStream_t s = m->stream;
+  CK(cudaSetDevice(m->device));
+  // (1) move masks, statuses and box indices of every point; the statuses and indices come back for the host to plan the passes
+  cudaError_t e = f->M.grow((size_t)nv, s);
+  if (e == cudaSuccess && np > 0) e = f->m_pts.grow((size_t)np * 3, s);
+  if (e == cudaSuccess && np > 0) e = f->m_st.grow((size_t)np, s);
+  if (e == cudaSuccess && np > 0) e = f->m_idx.grow((size_t)np, s);
+  if (e != cudaSuccess) {
+    cudaGetLastError();                                                   // not sticky: later calls must not see it
+    fb_set_error("%s: cannot allocate the move masks of %lld voxels: %s", fn, nv, cudaGetErrorString(e));
+    return FIESTA_ERR_CUDA;
+  }
+  CK(cudaEventRecord(f->ev[0], s));
+  if (n_src > 0) CK(cudaMemcpyAsync(f->m_pts, sources_xyz, (size_t)n_src * 24, cudaMemcpyHostToDevice, s));
+  if (n_tgt > 0) CK(cudaMemcpyAsync(f->m_pts + 3 * n_src, targets_xyz, (size_t)n_tgt * 24, cudaMemcpyHostToDevice, s));
+  CK(fb_navm_locate(m->g, m->cobs, a.b, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, f->M, f->m_pts, np, f->m_st, f->m_idx, s));
+  m->st.kernel_launches += np > 0 ? 3 : 2;
+  std::vector<int32_t> st((size_t)np);
+  std::vector<long long> idx((size_t)np);
+  if (np > 0) {
+    CK(cudaMemcpyAsync(st.data(), f->m_st, (size_t)np * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(idx.data(), f->m_idx, (size_t)np * 8, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  // rows: the placed sources in index order (channel k of the passes is placed source k), then the others (NaN rows)
+  std::vector<int32_t> rows;
+  std::vector<long long> src, tgt;
+  long long n_ps = 0;
+  for (long long i = 0; i < n_src; ++i) n_ps += st[i] == FB_NAVM_PLACED;
+  if (n_tgt > 0) {                                                         // then n_src < 2^31
+    for (long long i = 0; i < n_src; ++i)
+      if (st[i] == FB_NAVM_PLACED) { rows.push_back((int32_t)i); src.push_back(idx[i]); }
+    for (long long i = 0; i < n_src; ++i)
+      if (st[i] != FB_NAVM_PLACED) rows.push_back((int32_t)i);
+  }
+  for (long long j = n_src; j < np; ++j)
+    if (st[j] == FB_NAVM_PLACED) tgt.push_back(idx[j]);
+  const long long n_pt = (long long)tgt.size();
+  // (2) passes of C channels: C = min(32, sources left, max(1, floor(2^32 B / (8 B x box voxels))))
+  const long long per_pass = std::max(1ll, std::min((long long)FB_NAVM_CH, (1ll << 32) / (8 * nv)));
+  const long long C = std::min(per_pass, n_ps);
+  const bool work = n_ps > 0 && n_pt > 0;
+  if (work && C * nt >= (long long)0xffffffffu) {
+    fb_set_error("%s: the box has too many tiles", fn);
+    return FIESTA_ERR_LIMIT;
+  }
+  e = cudaSuccess;
+  if (n_src > 0 && n_tgt > 0) e = f->m_cost.grow((size_t)(n_src * n_tgt), s);
+  if (e == cudaSuccess && n_src > 0 && n_tgt > 0) e = f->m_rows.grow((size_t)n_src, s);
+  if (work) {
+    if (e == cudaSuccess) e = f->MD.grow((size_t)(C * nv), s);
+    for (FbDevBuf<uint32_t> *b : {&f->m_stamp, &f->m_list[0], &f->m_list[1]})
+      if (e == cudaSuccess) e = b->grow((size_t)(C * nt), s);
+    if (e == cudaSuccess) e = f->m_src.grow((size_t)n_ps, s);
+    if (e == cudaSuccess) e = f->m_tgt.grow((size_t)n_pt, s);
+  }
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    fb_set_error("%s: cannot allocate %lld fields of %lld voxels and the %lld x %lld matrix: %s", fn, C, nv, (long long)n_src,
+                 (long long)n_tgt, cudaGetErrorString(e));
+    return FIESTA_ERR_CUDA;
+  }
+  if (n_src > 0 && n_tgt > 0) CK(cudaMemcpyAsync(f->m_rows, rows.data(), (size_t)n_src * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(f->m_tot, 0, sizeof(FbNavMTot), s));
+  long long passes = 0;
+  if (work) {
+    CK(cudaMemcpyAsync(f->m_src, src.data(), (size_t)n_ps * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(f->m_tgt, tgt.data(), (size_t)n_pt * 8, cudaMemcpyHostToDevice, s));
+    a.D = f->MD; a.M = f->M; a.stamp = f->m_stamp; a.list[0] = f->m_list[0]; a.list[1] = f->m_list[1];
+    a.ctr = f->m_ctr; a.tot = f->m_tot; a.tgt = f->m_tgt; a.n_tgt = (int)n_pt;
+    for (long long p0 = 0; p0 < n_ps; p0 += C, ++passes) {
+      a.nch = (int)std::min(C, n_ps - p0);
+      CK(cudaMemsetAsync(f->m_stamp, 0, (size_t)(a.nch * nt) * 4, s));
+      CK(cudaMemsetAsync(f->m_ctr, 0, sizeof(FbNavMCtr), s));
+      CK(fb_navm_pass(a, f->m_src + p0, f->mblocks, s));
+      CK(fb_navm_gather(f->MD, nv, f->m_rows + p0, a.nch, f->m_idx + n_src, n_tgt, f->m_cost, s));
+      m->st.kernel_launches += 4;
+    }
+  }
+  // NaN rows: every source when no target is placed, else the sources not placed
+  const long long nan_from = work ? n_ps : 0;
+  if (n_src > nan_from && n_tgt > 0) {
+    CK(fb_navm_gather(nullptr, nv, f->m_rows + nan_from, n_src - nan_from, f->m_idx + n_src, n_tgt, f->m_cost, s));
+    m->st.kernel_launches++;
+  }
+  CK(cudaEventRecord(f->ev[1], s));
+  if (n_src > 0 && n_tgt > 0) CK(cudaMemcpyAsync(cost, f->m_cost, (size_t)(n_src * n_tgt) * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(f->h_mtot, f->m_tot, sizeof(FbNavMTot), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (n_src > 0) memcpy(src_status, st.data(), (size_t)n_src * 4);
+  if (n_tgt > 0) memcpy(tgt_status, st.data() + n_src, (size_t)n_tgt * 4);
+  if (stats) {
+    const FbNavMTot &t = *f->h_mtot;
+    *stats = fiesta_nav_matrix_stats{};
+    stats->sources_placed = n_ps;
+    stats->targets_placed = n_pt;
+    stats->passes = passes;
+    stats->generations = (int64_t)t.generations;
+    stats->tile_visits = (int64_t)t.tile_visits;
+    stats->sources_retired_early = (int64_t)t.retired_early;
+    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
+  }
   return FIESTA_OK;
 }
 

@@ -51,6 +51,25 @@ FB_HD bool fb_nav_move_ok(const FbNavBox &b, const double *D, const int *v, cons
   return true;
 }
 
+// Move mask of a voxel (cost matrices, fb_navmatrix.cu) from the traversability of its 3x3x3 neighbourhood, nb bit e = voxel +
+// fb_nav_dir(e) traversable (bit 13: the voxel itself).  Bit 13 of the result: the voxel is traversable; bit k != 13: the move from
+// neighbour k into the voxel is allowed, i.e. the box the two span is traversable.  0 for a blocked voxel.
+FB_HD unsigned fb_nav_move_bits(unsigned nb) {
+  if (!(nb & (1u << 13))) return 0;
+  unsigned out = 1u << 13;
+  for (int k = 0; k < 27; ++k) {
+    if (k == 13) continue;
+    int d[3];
+    fb_nav_dir(k, d);
+    unsigned need = 0;
+    for (int ex = d[0] < 0 ? -1 : 0; ex <= (d[0] > 0 ? 1 : 0); ++ex)
+      for (int ey = d[1] < 0 ? -1 : 0; ey <= (d[1] > 0 ? 1 : 0); ++ey)
+        for (int ez = d[2] < 0 ? -1 : 0; ez <= (d[2] > 0 ? 1 : 0); ++ez) need |= 1u << ((ex + 1) * 9 + (ey + 1) * 3 + ez + 1);
+    if ((nb & need) == need) out |= 1u << k;
+  }
+  return out;
+}
+
 // One step of the path rule: the first allowed neighbour u of v, in direction order, with fl(D(u) + w) == D(v).  False when there
 // is none (never at the fixpoint, for a reached voxel other than a goal).
 FB_HD bool fb_nav_step(const FbNavBox &b, const double *D, const double *w, int *v) {
@@ -91,4 +110,10 @@ FB_HD int fb_nav_path(const FbNavBox &b, const double *D, const double *w, int *
     if (!fb_nav_step(b, D, w, v)) return FB_NAV_TRUNCATED;   // no predecessor: only on a field that is not the fixpoint
   }
 }
+
+// Cost matrix (fiesta_nav_matrix, DESIGN.md §3.9): cost[i][j] = D_i(voxel of target j), D_i the field above with goals = {source i},
+// when both points have status 0; NaN otherwise.  The status of a source or a target:
+#define FB_NAVM_PLACED 0     // its voxel is a traversable box voxel
+#define FB_NAVM_BLOCKED 1    // its voxel is in the box but blocked
+#define FB_NAVM_OUTSIDE 2    // a NaN coordinate, fails PosInMap, or its voxel is outside the box
 #endif

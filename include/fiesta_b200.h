@@ -268,6 +268,38 @@ int fiesta_nav_export(const fiesta_nav_field *f, double *out);   /* box_voxels d
 int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, int32_t max_len, int32_t *status, int32_t *len,
                      double *cost, int32_t *vox_xyz /* n * max_len * 3 */);
 
+/* ---- cost matrices (tour planners, task allocation, roadmap edge costs): the geodesic cost from each of many sources to each of
+ * many targets through free space at a clearance, in one call.
+ *   box, clearance, flags   as fiesta_nav_compute (same rules, same errors).
+ *   status       per source and per target (positions in metres): 0 = its voxel (Pos2Vox) is a traversable box voxel, 1 = the voxel
+ *                is in the box but blocked, 2 = a NaN coordinate, outside the map (PosInMap) or the voxel is outside the box.
+ *   cost         cost[i * n_tgt + j] = D_i(voxel of target j) when source i and target j both have status 0, where D_i is the field
+ *                fiesta_nav_compute returns for the same box, clearance and flags with goals = {source i}: +inf when the target is
+ *                unreachable in the box, 0 when it lies in the source's voxel; NaN otherwise.  Bit for bit, so it also equals the
+ *                cost fiesta_nav_paths returns from target j on that field.  Duplicate points are allowed.  There is no symmetry:
+ *                cost[i][j] is the left fold of the weights from source i, so with the roles swapped the same pair of points can
+ *                differ in the last bits (fl-addition is not associative).
+ * The sources' fields are relaxed together, up to 32 per pass (fewer when 8 bytes per box voxel per source would pass 2^32 bytes),
+ * and a source stops as soon as all of its targets are provably final, so its time follows the distance to its farthest target
+ * rather than the box size.  The call owns separate buffers on the field object, which grow to the largest use: 4 bytes per box
+ * voxel (move masks), 8 bytes per box voxel and 12 bytes per 8^3 tile for each source of a pass (about 1.6 GB for 32 sources on a
+ * 160^3 box, 6.4 GB for 4 on a 512^3 box, with the 50 % growth headroom), and 8 bytes per matrix entry.  It does not change the
+ * field, export or paths of the last fiesta_nav_compute.  Synchronous, on the map's stream.  Errors, after which nothing has been
+ * written: FIESTA_ERR_INVALID for what fiesta_nav_compute rejects, negative counts, or null buffers where there is work (statuses
+ * for n > 0, cost when both counts are > 0); FIESTA_ERR_LIMIT when n_src * n_tgt >= 2^31; FIESTA_ERR_CUDA when the buffers
+ * cannot be allocated.  n_src == 0 or n_tgt == 0 is valid: the statuses are still written. */
+typedef struct fiesta_nav_matrix_stats {
+  int64_t sources_placed, targets_placed;  /* status-0 points */
+  int64_t passes;                          /* batches of sources resident together (0 when no source or no target is placed) */
+  int64_t generations, tile_visits;        /* summed over passes */
+  int64_t sources_retired_early;           /* sources stopped before their work list emptied */
+  float ms_compute;                        /* device time of the whole call */
+  float reserved_f[1];
+} fiesta_nav_matrix_stats;
+int fiesta_nav_matrix(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *sources_xyz, int64_t n_src,
+                      const double *targets_xyz, int64_t n_tgt, double clearance, int flags, int32_t *src_status, int32_t *tgt_status,
+                      double *cost /* n_src * n_tgt, row i = source i */, fiesta_nav_matrix_stats *stats /* nullable */);
+
 /* ---- frontier extraction (exploration planners: where does observed free space end?) ----
  * The free voxels of an inclusive voxel box [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis) that border never-observed
  * space, grouped into clusters, as a snapshot of the integrated records and log-odds at the time of the call (observations that

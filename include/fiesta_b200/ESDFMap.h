@@ -162,6 +162,16 @@ class ESDFMap {
     check(fiesta_nav_compute(f, box_lo, box_hi, goals_xyz, n_goals, clearance, flags, &st), "ComputeNavField");
     return st;
   }
+  // Cost matrix (fiesta_nav_matrix): cost[i * n_tgt + j] = the field of source i alone read at target j, NaN where either point is
+  // blocked or outside the box.  Leaves the last ComputeNavField result as it was.
+  fiesta_nav_matrix_stats NavCostMatrix(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *sources_xyz, long n_src,
+                                        const double *targets_xyz, long n_tgt, double clearance, int flags, int32_t *src_status,
+                                        int32_t *tgt_status, double *cost) {
+    fiesta_nav_matrix_stats st = {};
+    check(fiesta_nav_matrix(f, box_lo, box_hi, sources_xyz, n_src, targets_xyz, n_tgt, clearance, flags, src_status, tgt_status, cost, &st),
+          "NavCostMatrix");
+    return st;
+  }
   void ExportNavField(const fiesta_nav_field *f, double *out) { check(fiesta_nav_export(f, out), "ExportNavField"); }
   void NavPaths(fiesta_nav_field *f, const double *starts_xyz, long n, int max_len, int32_t *status, int32_t *len, double *cost,
                 int32_t *vox_xyz) {
