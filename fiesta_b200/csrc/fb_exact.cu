@@ -145,10 +145,12 @@ int fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t s) {
   CK(X->SUM.alloc(P)); CK(X->SUMg.alloc(P)); CK(cudaMemsetAsync(X->SUMg, 0, P * 4, s));
   CK(X->emask.alloc(P));
   CK(X->wstamp.alloc(P)); CK(cudaMemsetAsync(X->wstamp, 0, P * 4, s));
-  for (int k = 0; k < 3; ++k) { CK(X->W[k].alloc(P)); CK(X->F[k].alloc(P)); }
+  for (int k = 0; k < 3; ++k) { CK(X->W[k].alloc(P)); CK(X->F[k].alloc(P)); CK(cudaMemsetAsync(X->W[k], 0, P * 4, s)); }   // W doubles as the
+  // ring of k_x_relax's work queue, whose full slots carry bit 31: it never holds a stray one
   for (int k = 0; k < 2; ++k) CK(X->E[k].alloc(P));
   X->dense_min = 16384u;
   if (const char *e = getenv("FIESTA_X_DENSE")) { long v = atol(e); if (v >= 0 && v <= (1 << 24)) X->dense_min = (unsigned)v; }
+  if (const char *e = getenv("FIESTA_X_ASYNC")) X->async = atol(e) != 0;
   X->small_max = FB_X_SMALL_DEFAULT;
   if (const char *e = getenv("FIESTA_X_SMALL")) { long v = atol(e); if (v >= 0 && v <= 65536) X->small_max = (unsigned)v; }
   CK(X->slotc.alloc(((size_t)X->small_max + 1) * 32));
@@ -306,7 +308,16 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
     CK(cudaMemcpyAsync(h, X->d_ctl, sizeof(FbXCtl), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     *launches += 1;
-    if (h->err) { fb_set_error(h->err == 1u ? "exact mode: generation with more than 2^27 entries" : "exact mode: behaviour fixpoint did not converge"); return FIESTA_ERR_CUDA; }
+    if (h->err) {
+      if (h->err == 3u) {                                      // an abandoned work queue may leave marked ring slots and queue
+        for (int k = 0; k < 3; ++k) CK(cudaMemsetAsync(X->W[k], 0, P * 4, s));   // states above the saved clock behind
+        CK(cudaMemsetAsync(X->wstamp, 0, P * 4, s));
+        X->wclock = 0;
+      }
+      fb_set_error(h->err == 1u ? "exact mode: generation with more than 2^27 entries"
+                   : h->err == 3u ? "exact mode: a wait of the asynchronous work queue exceeded its bound" : "exact mode: behaviour fixpoint did not converge");
+      return FIESTA_ERR_CUDA;
+    }
     X->gen_id = h->gen_id; X->wclock = h->wclock; X->tclock = h->tclock; X->sclock = h->sclock;
     st->generations = h->generations; st->reseed_rounds = h->reseed_rounds; st->eval_rounds = h->rounds; st->dense_rounds = h->dense_rounds;
     st->voxels_changed = h->voxels_changed; st->expansions = h->expansions;
@@ -315,15 +326,27 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
       static double cyc_per_us = 0;                            // clock64 counts SM cycles: convert with this device's SM clock
       if (cyc_per_us == 0) { int dev = 0, khz = 0; CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev)); cyc_per_us = khz / 1000.0; }
       CK(cudaMemcpy(hd, X->d_dbg, sizeof(hd), cudaMemcpyDeviceToHost));
-      static const char *cat[14] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top", "empty-barrier", "reseed.rounds", "reseed.assemble"};
+      // phase categories of k_x_relax (14 and 15 are list-length counters, printed below)
+      static const char *cat[19] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top", "empty-barrier",
+                                    "reseed.rounds", "reseed.assemble", "", "", "async", "", "refresh"};
       fprintf(stderr, "[x] reseed rounds %u; phases (us, count):", st->reseed_rounds);
-      for (int c = 0; c < 14; ++c) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[3 * 1024 + 2 * c] / cyc_per_us, hd[3 * 1024 + 2 * c + 1]);
+      for (int c = 0; c < 19; ++c)
+        if (*cat[c]) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[FB_XDBG_PHASE + 2 * c] / cyc_per_us, hd[FB_XDBG_PHASE + 2 * c + 1]);
       fprintf(stderr, "\n");
-      { double wm = 0; for (int q = 0; q < 4096; ++q) wm += hd[3 * 1024 + 32 + 1024 + q] / cyc_per_us; fprintf(stderr, "[x] sum over rounds of the longest per-CTA work time: %.0f us (the rest of round1+rounds+dense+s.round1+s.rounds is barrier + skew)\n", wm); }
-      for (int gq = 0; gq < 2; ++gq) { fprintf(stderr, "[x] gen %d work lists:", gq); for (int r = 0; r < 512 && hd[3 * 1024 + 32 + gq * 512 + r]; ++r) fprintf(stderr, " %llu", hd[3 * 1024 + 32 + gq * 512 + r]); fprintf(stderr, "\n"); }
-      fprintf(stderr, "[x] work-list entries: evaluated %llu refreshed %llu reseeded %llu\n", hd[3 * 1024 + 2 * 14], hd[3 * 1024 + 2 * 14 + 1], hd[3 * 1024 + 2 * 15]);
+      fprintf(stderr, "[x] round work (summed longest CTA work time us / summed list length):");
+      for (int c : {1, 2, 3, 6, 7}) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[FB_XDBG_WORK + 2 * c] / cyc_per_us, hd[FB_XDBG_WORK + 2 * c + 1]);
+      fprintf(stderr, "\n");
+      for (int h = 0; h < 2; ++h) {
+        fprintf(stderr, "[x] list-length histogram %s (log2 bucket=rounds):", h ? "s.rounds" : "rounds");
+        for (int b = 0; b < 32; ++b) if (hd[FB_XDBG_NWH + 32 * h + b]) fprintf(stderr, " %d=%llu", b, hd[FB_XDBG_NWH + 32 * h + b]);
+        fprintf(stderr, "\n");
+      }
+      fprintf(stderr, "[x] async: evaluations %llu dirty %llu pushes %llu spin %.0f us\n", hd[FB_XDBG_Q + 0], hd[FB_XDBG_Q + 1], hd[FB_XDBG_Q + 2],
+              hd[FB_XDBG_Q + 3] / cyc_per_us);
+      for (int gq = 0; gq < 2; ++gq) { fprintf(stderr, "[x] gen %d work lists:", gq); for (int r = 0; r < 512 && hd[FB_XDBG_ROUNDS + gq * 512 + r]; ++r) fprintf(stderr, " %llu", hd[FB_XDBG_ROUNDS + gq * 512 + r]); fprintf(stderr, "\n"); }
+      fprintf(stderr, "[x] work-list entries: evaluated %llu refreshed %llu reseeded %llu\n", hd[FB_XDBG_PHASE + 2 * 14], hd[FB_XDBG_PHASE + 2 * 14 + 1], hd[FB_XDBG_PHASE + 2 * 15]);
       fprintf(stderr, "[x] gens %u rounds %u dense %u deps %u nE0 %u |", st->generations, st->eval_rounds, st->dense_rounds, st->dependants, nE);
-      for (unsigned q = 0; q < st->generations && q < 1024; ++q) fprintf(stderr, " %llu/%llu/%.1fus", hd[3 * q], hd[3 * q + 1], hd[3 * q + 2] / cyc_per_us);
+      for (unsigned q = 0; q < st->generations && q < FB_XDBG_GENS; ++q) fprintf(stderr, " %llu/%llu/%.1fus", hd[3 * q], hd[3 * q + 1], hd[3 * q + 2] / cyc_per_us);
       fprintf(stderr, "\n");
     }
   }

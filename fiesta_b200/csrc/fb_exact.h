@@ -5,7 +5,21 @@
 
 #define FB_X_MAX_BLOCKS 256
 #define FB_X_SMALL_DEFAULT 32768u   // (from a sweep on the 512^3 LIDAR frames; FIESTA_X_SMALL / FIESTA_X_DENSE override)
-#define FB_X_DBG_WORDS (3 * 1024 + 32 + 2 * 512 + 4096)
+// Trace layout of k_x_relax (FIESTA_DEBUG_X): [3 * FB_XDBG_GENS] per generation {nE, rounds, cycles}; FB_XDBG_NCAT x {cycles,
+// count} per phase category; 2 x 512 work-list sizes per round (first two generations); 4096 per-round slots for the longest
+// CTA work time of the round (cycles, reset once added up); FB_XDBG_NCAT x {summed longest CTA work time, summed list
+// length} per round category; 2 x 32 log2 histograms of the list lengths of BIG short-list rounds and SMALL later rounds;
+// FB_XDBG_NQ counters of the asynchronous schedule.
+#define FB_XDBG_GENS 1024
+#define FB_XDBG_NCAT 24
+#define FB_XDBG_NQ 8
+#define FB_XDBG_PHASE (3 * FB_XDBG_GENS)
+#define FB_XDBG_ROUNDS (FB_XDBG_PHASE + 2 * FB_XDBG_NCAT)
+#define FB_XDBG_WMAX (FB_XDBG_ROUNDS + 2 * 512)
+#define FB_XDBG_WORK (FB_XDBG_WMAX + 4096)
+#define FB_XDBG_NWH (FB_XDBG_WORK + 2 * FB_XDBG_NCAT)
+#define FB_XDBG_Q (FB_XDBG_NWH + 2 * 32)
+#define FB_X_DBG_WORDS (FB_XDBG_Q + FB_XDBG_NQ)
 
 struct FbExactStats {
   unsigned long long expansions;      // == the reference's "Expanding N nodes" (ESDFMap.cpp:347,394)
@@ -22,6 +36,10 @@ struct FbXCtl {
   unsigned generations, rounds, dense_rounds, reseed_rounds;
   unsigned long long tclock, expansions, voxels_changed;
   unsigned partial[FB_X_MAX_BLOCKS];  // winners per CTA range (ordered hand-over)
+  // work queue of the asynchronous schedule (one line each: the first two take every push / pop, the third is polled)
+  alignas(128) unsigned long long qtail;  // {outstanding items + warps still seeding : 32 | pushes so far : 32}
+  alignas(128) unsigned qhead;            // pops reserved so far
+  alignas(128) unsigned qdone;            // 1 once the outstanding count reached zero (or a wait exceeded its bound)
 };
 
 // Order-exact state of one map.  Zero until fb_exact_init; freed with the map.
@@ -46,6 +64,7 @@ struct FbExact {
   FbDevBuf<uint32_t> slotc;           // SMALL generations: codes of the owned slots
   unsigned dense_min = 0;             // work lists longer than this are evaluated through refreshed summaries (one wave of warps)
   unsigned small_max = 0;             // generations up to this many entries run without summaries
+  bool async = true;                  // short work lists resolved from a work queue instead of in rounds (FIESTA_X_ASYNC=0: rounds)
   FbDevBuf<FbXCtl> d_ctl;
   FbHostBuf<FbXCtl> h_ctl;
   FbDevBuf<unsigned long long> d_dbg;

@@ -18,7 +18,8 @@
 //    from a per-warp shared-memory stage filled by one round of loads (x_stage) while last round's flips refresh the
 //    summaries of their targets; long lists first refresh, then evaluate through the summaries.  Element i is right once all
 //    earlier ones are, so the fixpoint -- reached by a round without flips, which has only read final words -- is the
-//    sequential execution.
+//    sequential execution.  In BIG generations, once a list is short, the rest of the fixpoint runs without rounds from a
+//    work queue (x_async), followed by one summary refresh.
 //  * Hand-over: element i owns slot k iff the final state of its k-th target carries the timestamp 32*i + k; the owned slots in
 //    timestamp order (per-element masks, exclusive scan over CTA-contiguous ranges) are the next generation; old words are
 //    retired by compare-and-swap (a generation-parity bit tells old from new).
@@ -41,11 +42,11 @@
 #define X_MAX_ROUNDS 4000000u
 #define XGB 8                         // writer words loaded per batch by a gather (24 / XGB batches)
 #define XRC 8                         // directions listed per chunk after a re-seeding change (24 / XRC chunks)
-#define XDBG_GENS 1024                // trace layout (FIESTA_DEBUG_X): [3 * XDBG_GENS] per generation {nE, rounds, cycles},
-#define XDBG_PHASE (3 * XDBG_GENS)    // then 16 x {cycles, count} per phase category (14: summed work / flip list lengths, 15: summed
-                                      // re-seeding list lengths), then 2 x 512 work-list sizes per round
-#define XDBG_ROUNDS (XDBG_PHASE + 32)
-#define XDBG_WMAX (XDBG_ROUNDS + 1024)      // 4096 slots: per round of the fixpoint, the longest work time of any CTA (cycles)
+// trace layout (FIESTA_DEBUG_X): fb_exact.h.  Phase categories 14 and 15 hold summed work / flip list lengths and summed
+// re-seeding list lengths instead of times.
+#define XDBG_PHASE FB_XDBG_PHASE
+#define XDBG_ROUNDS FB_XDBG_ROUNDS
+#define XDBG_WMAX FB_XDBG_WMAX
 
 static __constant__ int x_dirs[24][3] = {
     {-1, 0, 0}, {1, 0, 0}, {0, -1, 0}, {0, 1, 0}, {0, 0, -1}, {0, 0, 1},
@@ -89,6 +90,7 @@ struct XShared {
   unsigned char self[32];             // index in off[] of target t itself (entry 24 = 0)
   unsigned red[XW], red2[XW];
   unsigned base, total;
+  unsigned qdone;                     // the work queue of the current asynchronous phase is done (copy of ctl->qdone)
 };
 
 __device__ __forceinline__ unsigned x_d2(int x, int y, int z, uint32_t c) {
@@ -219,6 +221,7 @@ struct XArgs {
   unsigned long long ls_deps;   // link time of dependant 0 (InsertIntoList order, :333)
   unsigned long long *dbg;  // optional per-generation trace {nE, rounds, ns} (FIESTA_DEBUG_X)
   unsigned div_pz_m, div_pz_s, div_gy_m, div_gy_s;   // n / d = umulhi(n, m) >> s for n < 2^31 (fb_div_make, fb_divmagic.h); m == 0: d == 1
+  unsigned async_on;        // resolve short work lists from the work queue (x_async) instead of in rounds
 };
 // voxel index -> coordinates: two divisions by run-time constants, as multiply-high + shift
 __device__ __forceinline__ unsigned x_div(unsigned n, unsigned m, unsigned s) { return m ? (__umulhi(n, m) >> s) : n; }
@@ -490,6 +493,181 @@ __device__ __forceinline__ unsigned x_warp_append_n(unsigned *counter, unsigned 
   return __shfl_sync(act, base, leader) + pre;
 }
 
+// ---- asynchronous schedule of the short work lists ------------------------------------------------------------------------
+// Rounds are a scheduling device: element i's behaviour depends only on the words of earlier elements, so the fixpoint is
+// unique and every fair schedule that re-evaluates an element after each change of its inputs reaches it (by induction on
+// i).  x_async runs such a schedule without grid barriers: every warp pops an element from a work queue, evaluates it from
+// its stage exactly as a round does, and on a flip pushes the later elements it can touch.
+//  * Element state, in wstamp with the phase's base A (stamps of earlier rounds and phases are all below A): RUNNING = A,
+//    MARKED = A + 1 (queued, or dirty while running), IDLE = anything below A.  A lister does atomicMax(MARKED) and pushes
+//    iff the element was IDLE; a running element that gets marked is dirty, and its worker evaluates it again before
+//    setting it IDLE (compare-and-swap RUNNING -> A - 1).  Hence an element is queued at most once and evaluated by one warp
+//    at a time.
+//  * No missed update.  The flipping warp stores its word, then fence.sc, then reads the state of each element it lists;
+//    a worker swaps the state to RUNNING, then fence.sc, then stages.  Of two such store-fence-load sequences at least one
+//    load sees the other's store.  So either the lister sees RUNNING / IDLE and marks the element (a worker will evaluate
+//    it again, after a swap that comes later), or the lister sees MARKED and the swap that follows it sees the flip.
+//    After the last flip of each input some evaluation sees it; an element whose inputs stop changing stops changing.
+//  * Ring: a buffer with one slot per element of the generation (at most nE elements are queued at once); pushes and pops
+//    reserve consecutive indices, slot = index mod nE.  A full slot carries bit 31 (work lists leave elements < 2^27 in the
+//    buffer, pops leave 0): a pusher waits for the slot to be free, a popper takes whatever element is in its slot (items
+//    may swap between poppers of one slot, which is harmless: each is taken once).  A pusher never waits forever: with
+//    at most nE distinct queued elements, every full slot has a reserved popper that has not taken an item yet.
+//  * Termination: qtail's high half counts the outstanding items (incremented with the push that creates one,
+//    decremented when its evaluation is over, after its own pushes) plus one token per warp until the warp has pushed its
+//    share of the seed list.  Zero is final (nothing runs that could push); whoever reaches it sets qdone.
+//  * Every wait is bounded (X_Q_WAIT_NS of no progress): the kernel then sets ctl->err = 3 and qdone, and every warp leaves.
+#define X_Q_FULL 0x80000000u
+#define X_Q_WAIT_NS 2000000000ull
+__device__ __forceinline__ unsigned x_ld_relaxed(const unsigned *p) {
+  unsigned v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ unsigned long long x_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ void x_q_abort(const XArgs &a) {
+  atomicCAS(&a.ctl->err, 0u, 3u);
+  atomicExch(&a.ctl->qdone, 1u);
+}
+// qtail += delta (one lane); sets qdone when the outstanding count reaches zero.  Returns the old push count.
+__device__ __forceinline__ unsigned x_q_count(const XArgs &a, unsigned long long delta) {
+  const unsigned long long old = atomicAdd(&a.ctl->qtail, delta);
+  if ((unsigned)((old + delta) >> 32) == 0u) atomicExch(&a.ctl->qdone, 1u);
+  return (unsigned)old;
+}
+// (qdone cannot be set while the pusher's own item is outstanding, unless the phase was abandoned: then it leaves at once)
+__device__ __forceinline__ void x_q_put(const XArgs &a, XShared &sh, uint32_t *ring, unsigned cap, unsigned idx, unsigned e) {
+  unsigned *slot = &ring[idx % cap];
+  const volatile unsigned *done = &sh.qdone;
+  unsigned cur = x_ld_relaxed(slot);
+  const unsigned long long t0 = x_globaltimer();
+  for (unsigned it = 0;; ++it) {
+    if (!(cur & X_Q_FULL)) {
+      const unsigned o = atomicCAS(slot, cur, e | X_Q_FULL);
+      if (o == cur) return;
+      cur = o;
+      continue;
+    }
+    if (*done) return;
+    if ((it & 15u) == 15u) {
+      if (x_ld_acquire(&a.ctl->qdone)) { sh.qdone = 1u; return; }
+      if (x_globaltimer() - t0 > X_Q_WAIT_NS) { x_q_abort(a); sh.qdone = 1u; return; }
+    }
+    __nanosleep(64);
+    cur = x_ld_relaxed(slot);
+  }
+}
+// One lane: the next element from the queue, or XNONE once the phase is over.  `h` keeps the reserved pop index between calls.
+__device__ __forceinline__ unsigned x_q_take(const XArgs &a, XShared &sh, uint32_t *ring, unsigned cap, unsigned &h) {
+  if (h == XNONE) h = atomicAdd(&a.ctl->qhead, 1u);
+  unsigned *slot = &ring[h % cap];
+  const volatile unsigned *done = &sh.qdone;
+  const long long c0 = a.dbg ? clock64() : 0;
+  unsigned long long t0 = 0;
+  unsigned ns = 32;
+  for (unsigned it = 0;; ++it) {
+    if (x_ld_relaxed(slot) & X_Q_FULL) {
+      const unsigned v = atomicExch(slot, 0u);
+      if (v & X_Q_FULL) { h = XNONE; if (a.dbg) atomicAdd(&a.dbg[FB_XDBG_Q + 3], (unsigned long long)(clock64() - c0)); return v & ~X_Q_FULL; }
+    }
+    if (*done) break;
+    if ((it & 15u) == 15u) {                                   // the global flag is polled by few warps at a time
+      if (x_ld_acquire(&a.ctl->qdone)) { sh.qdone = 1u; break; }
+      const unsigned long long t = x_globaltimer();
+      if (t0 == 0) t0 = t;
+      else if (t - t0 > X_Q_WAIT_NS) { x_q_abort(a); sh.qdone = 1u; break; }
+    }
+    __nanosleep(ns);
+    ns = ns < 256u ? 2u * ns : 256u;
+  }
+  if (a.dbg) atomicAdd(&a.dbg[FB_XDBG_Q + 3], (unsigned long long)(clock64() - c0));
+  return XNONE;
+}
+// Marks the later elements among the first `nof` staged offsets of element i and pushes those that were IDLE (one warp,
+// after the flip's word was stored and fenced).
+__device__ __forceinline__ unsigned x_q_list(const XArgs &a, XShared &sh, const XNb &nb, uint32_t *ring, unsigned cap, unsigned lane, unsigned i, unsigned nof, unsigned A) {
+  unsigned j[5], st[5];
+#pragma unroll
+  for (int t = 0; t < 5; ++t) {
+    const unsigned o = lane + 32u * (unsigned)t;
+    const unsigned long long w = o < nof ? nb.w[o] : XMB_NONE;
+    j[t] = w != XMB_NONE ? x_mb_idx(w) : 0u;
+    st[t] = (w != XMB_NONE && j[t] > i) ? x_ld_relaxed(&a.wstamp[j[t]]) : A + 1u;   // A + 1 = already marked or not a candidate
+  }
+  unsigned pm = 0;
+#pragma unroll
+  for (int t = 0; t < 5; ++t)
+    if (st[t] != A + 1u && atomicMax(&a.wstamp[j[t]], A + 1u) < A) pm |= 1u << t;
+  const unsigned cnt = (unsigned)__popc(pm);
+  unsigned incl = cnt;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const unsigned v = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane >= o) incl += v; }
+  const unsigned total = __shfl_sync(0xffffffffu, incl, 31);
+  if (total == 0u) return 0u;
+  unsigned base = 0;
+  if (lane == 0) base = x_q_count(a, (unsigned long long)total * 0x100000001ull);
+  base = __shfl_sync(0xffffffffu, base, 0) + incl - cnt;
+#pragma unroll
+  for (int t = 0; t < 5; ++t) if ((pm >> t) & 1u) x_q_put(a, sh, ring, cap, base++, j[t]);
+  return total;
+}
+// The asynchronous phase of one BIG generation (all warps of the grid): the nw elements of the work list `wl` seed the
+// queue, `ring` (nE slots) holds it; every flip is recorded in F[fout] for the summary refresh that follows.
+__device__ void x_async(const XArgs &a, XShared &sh, XNb &stg, unsigned lane, unsigned gwarp, unsigned gwarps, const uint32_t *E, unsigned nE,
+                        const uint32_t *wl, unsigned nw, uint32_t *ring, unsigned gen, unsigned A, unsigned fout) {
+  // seeds: this warp's chunks of 32, then its token
+  for (unsigned q0 = gwarp * 32u; q0 < nw; q0 += gwarps * 32u) {
+    const unsigned q = q0 + lane;
+    const unsigned e = q < nw ? __ldcg(&wl[q]) : 0u;
+    const bool push = q < nw && atomicMax(&a.wstamp[e], A + 1u) < A;
+    const unsigned pm = __ballot_sync(0xffffffffu, push), cnt = (unsigned)__popc(pm);
+    if (cnt == 0u) continue;
+    unsigned base = 0;
+    if (lane == 0) base = x_q_count(a, (unsigned long long)cnt * 0x100000001ull);
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (push) x_q_put(a, sh, ring, nE, base + (unsigned)__popc(pm & ((1u << lane) - 1u)), e);
+    if (a.dbg && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 2], (unsigned long long)cnt);
+  }
+  if (lane == 0) x_q_count(a, 0ull - (1ull << 32));
+  unsigned h = XNONE;
+  for (;;) {
+    unsigned i = 0;
+    if (lane == 0) i = x_q_take(a, sh, ring, nE, h);
+    i = __shfl_sync(0xffffffffu, i, 0);
+    if (i == XNONE) break;
+    const uint32_t p = __ldcg(&E[i]);
+    int x, y, z; x_coords(a, p, x, y, z);
+    for (;;) {
+      if (a.dbg && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 0], 1ull);
+      if (lane == 0) atomicExch(&a.wstamp[i], A);              // RUNNING (from MARKED: queued, or dirty)
+      __syncwarp();
+      __threadfence();
+      x_stage(a, sh, stg, lane, x, y, z);
+      const unsigned long long old = stg.w[0], nw2 = x_eval_nb(a, sh, stg, lane, gen, i, x, y, z);
+      if (nw2 != old) {                                        // flip
+        if (lane == 0) {
+          a.MB[p] = nw2;
+          const unsigned f = atomicAdd(&a.ctl->nF[fout], 1u);
+          if (f < (unsigned)a.g.ptotal) a.F[fout][f] = i;
+        }
+        __syncwarp();
+        __threadfence();
+        const unsigned np = x_q_list(a, sh, stg, ring, nE, lane, i, (x_mb_kind(old) == X_PUSH || x_mb_kind(nw2) == X_PUSH) ? (unsigned)X_NOFF : 25u, A);
+        if (a.dbg && lane == 0 && np) atomicAdd(&a.dbg[FB_XDBG_Q + 2], (unsigned long long)np);
+      }
+      unsigned again = 0;
+      if (lane == 0) again = atomicCAS(&a.wstamp[i], A, A - 1u) != A ? 1u : 0u;   // IDLE, unless marked dirty meanwhile
+      if (!__shfl_sync(0xffffffffu, again, 0)) break;
+      if (a.dbg && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 1], 1ull);
+    }
+    if (lane == 0) x_q_count(a, 0ull - (1ull << 32));
+  }
+}
+
 // One evaluation of the re-seeding rule: dependant i takes the closest obstacle of the FIRST neighbour in dirs_ order that
 // has a valid one (:308-321); dependants processed earlier expose their new value, later ones their (deleted) old one.
 __device__ __forceinline__ uint32_t x_reseed_eval(const XArgs &a, unsigned i, int x, int y, int z, unsigned &kc) {
@@ -524,6 +702,8 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
   const unsigned gwarp = gtid >> 5, gwarps = gthreads >> 5;
   for (unsigned k = tid; k < X_NOFF; k += XT) sh.off[k] = x_off_c[k];
   if (tid < 32) sh.self[tid] = 0;
+  if (tid == 0) sh.qdone = 0u;
+  if (gtid == 0) a.ctl->qtail = (unsigned long long)gwarps << 32;   // one seeding token per warp (x_async)
   if (tid < 32) sh.dir[tid] = tid < 24 ? ((x_dirs[tid][0] + 4) | ((x_dirs[tid][1] + 4) << 4) | ((x_dirs[tid][2] + 4) << 8)) : (4 | (4 << 4) | (4 << 8));
   __syncthreads();
   for (unsigned q = tid; q < 25u * 24u + 25u; q += XT) {         // where target t's k-th writer (and t itself) sits among the 129 offsets
@@ -703,6 +883,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
     const uint32_t *E = a.E[cur];
     // ---- behaviour fixpoint
     unsigned rounds = 0;
+    bool aborted = false;
     if (big) {
       ++sclock;
       for (unsigned i = gwarp; i < nE; i += gwarps) { int x, y, z; x_coords(a, __ldcg(&E[i]), x, y, z); x_claim_summaries(a, sh, lane, x, y, z, sclock); }
@@ -717,6 +898,36 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       if (r > 1u && nw == 0u && nf == 0u) break;
       if (r > X_MAX_ROUNDS) { if (gtid == 0) ctl->err = 2u; break; }   // cannot happen (element i is final after i+1 rounds at the latest); never spin forever on the GPU
       if (a.dbg && gtid == 0) { a.dbg[XDBG_PHASE + 2 * 14] += nw; a.dbg[XDBG_PHASE + 2 * 14 + 1] += nf; }
+      if (a.async_on && big && r > 1u && nw <= a.dense_min) {
+        // the rest of the fixpoint from the work queue, with W[out] as its ring; then the summaries of the targets of every
+        // flip since the last refresh: last round's (F[in]) and the queue's (F[out]).  (SMALL generations keep their rounds:
+        // their lists are a few entries long and the queue's start and end cost more than the barriers it saves, DESIGN §6.)  A summary's offer timestamps
+        // 32*i+k are fixed, so the refresh rule needs only the final word and the summary's first / best, however often the
+        // element flipped in between.
+        ++rounds; wclock += 3u;
+        const unsigned A = wclock - 1u;                        // RUNNING; MARKED = wclock; the stamps of the next rounds are above
+        x_async(a, sh, stg, lane, gwarp, gwarps, E, nE, a.W[in], nw, a.W[out], gen, A, out);
+        x_gsync(&ctl->bar, bar_target);
+        X_LAP(16);
+        if (tid == 0) sh.qdone = 0u;
+        if (gtid == 0) { ctl->qtail = (unsigned long long)gwarps << 32; ctl->qhead = 0u; ctl->qdone = 0u; }
+        if (__ldcg(&ctl->err)) { aborted = true; break; }
+        const unsigned nfa = __ldcg(&ctl->nF[out]);
+        if (nfa > (unsigned)g.ptotal) {                        // flip list overflowed: summarise every target again
+          ++sclock;
+          for (unsigned i = gwarp; i < nE; i += gwarps) { int x, y, z; x_coords(a, __ldcg(&E[i]), x, y, z); x_claim_summaries(a, sh, lane, x, y, z, sclock); }
+        } else {
+          for (unsigned q = gwarp; q < nf + nfa; q += gwarps) {
+            const unsigned i = q < nf ? __ldcg(&a.F[in][q]) : __ldcg(&a.F[out][q - nf]);
+            const uint32_t p = __ldcg(&E[i]);
+            int x, y, z; x_coords(a, p, x, y, z);
+            x_refresh_summaries(a, sh, lane, i, p, x, y, z);
+          }
+        }
+        x_gsync(&ctl->bar, bar_target);
+        X_LAP(18);
+        break;
+      }
       ++rounds; ++wclock;
       const bool dense = big && r > 1u && nw > a.dense_min;   // more than one wave of warps: evaluate through the summaries
       if (dense) {                                             // bring the summaries up to date first, then evaluate through them
@@ -777,10 +988,18 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       if (a.dbg) { __syncthreads(); if (tid == 0) atomicMax(&a.dbg[XDBG_WMAX + ((rounds_total + rounds) & 4095u)], (unsigned long long)(clock64() - t_w0)); }
       x_gsync(&ctl->bar, bar_target);
       X_LAP(big ? (r == 1u ? 1 : (dense ? 3 : 2)) : (r == 1u ? 6 : 7));
-      if (a.dbg && gtid == 0 && generations <= 2u && rounds <= 512u) a.dbg[XDBG_ROUNDS + (generations - 1u) * 512u + (rounds - 1u)] = nw;
+      if (a.dbg && gtid == 0) {
+        if (generations <= 2u && rounds <= 512u) a.dbg[XDBG_ROUNDS + (generations - 1u) * 512u + (rounds - 1u)] = nw;
+        // the round's longest CTA work time and list length, summed per category: the rest of the category's time is barrier
+        // and waiting for the slowest CTA
+        const unsigned cat = big ? (r == 1u ? 1u : (dense ? 3u : 2u)) : (r == 1u ? 6u : 7u);
+        unsigned long long *wm = &a.dbg[XDBG_WMAX + ((rounds_total + rounds) & 4095u)];
+        a.dbg[FB_XDBG_WORK + 2 * cat] += __ldcg(wm); a.dbg[FB_XDBG_WORK + 2 * cat + 1] += nw; *wm = 0;
+        if (cat == 2u || cat == 7u) a.dbg[FB_XDBG_NWH + (cat == 7u ? 32u : 0u) + (nw ? 32u - __clz(nw) : 0u)] += 1ull;
+      }
     }
     rounds_total += rounds;
-    if (rounds > X_MAX_ROUNDS) break;
+    if (rounds > X_MAX_ROUNDS || aborted) break;
 
     // ---- commit: per-element masks of owned slots, winner counts per CTA (CTA-contiguous ranges keep the order)
     const unsigned per = (nE + G - 1u) / G;
@@ -866,7 +1085,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       }
       run += ctot;
     }
-    if (a.dbg && gtid == 0 && generations <= 1024u) { a.dbg[3 * (generations - 1u)] = nE; a.dbg[3 * (generations - 1u) + 1] = rounds; a.dbg[3 * (generations - 1u) + 2] = (unsigned long long)(clock64() - t_gen); }
+    if (a.dbg && gtid == 0 && generations <= FB_XDBG_GENS) { a.dbg[3 * (generations - 1u)] = nE; a.dbg[3 * (generations - 1u) + 1] = rounds; a.dbg[3 * (generations - 1u) + 2] = (unsigned long long)(clock64() - t_gen); }
     tclock += (unsigned long long)nE * 32ull + 1ull;
     changed_total += n2;
     if (n2 >= (1u << 27)) { if (gtid == 0) ctl->err = 1u; break; }
@@ -925,6 +1144,7 @@ cudaError_t fb_xrelax_launch(FbExact *X, const FbGeom &g, uint32_t *cobs, unsign
   a.E[0] = X->E[0]; a.E[1] = X->E[1]; a.emask = X->emask;
   for (int k = 0; k < 3; ++k) { a.W[k] = X->W[k]; a.F[k] = X->F[k]; }
   a.wstamp = X->wstamp; a.slotc = X->slotc; a.ctl = X->d_ctl; a.nE0 = nE0; a.small_max = X->small_max; a.dense_min = X->dense_min; a.dbg = dbg;
+  a.async_on = X->async ? 1u : 0u;
   void *args[] = {(void *)&a};
   return cudaLaunchCooperativeKernel((void *)k_x_relax, dim3(X->relax_blocks), dim3(XT), args, sizeof(XNb) * XW, s);
 }

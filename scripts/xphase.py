@@ -7,7 +7,10 @@ clock64; the library converts cycles with the device's SM clock) and sums, over 
 the time of every phase, the evaluation rounds, the work-list entries evaluated and refreshed, and the re-seeding list
 entries.  It also prints, per frame, the (nE, rounds) list of every generation.  The numbers of generations and every nE
 are fixed by the sequential result; rounds and list lengths vary from run to run (a round reads words flipped in the same
-round).  The output is plain text, one item per line, so two runs can be diffed.  Needs a GPU.
+round).  For the evaluation-round categories it also splits the time into the summed longest CTA work time of every round
+and the rest (grid barrier plus waiting for the slowest CTA), with a log2 histogram of the list lengths of the short-list
+rounds, and it sums the counters of the asynchronous schedule (FIESTA_X_ASYNC).  The card, its power limit and the SM clock
+are printed first.  The output is plain text, one item per line, so two runs can be diffed.  Needs a GPU.
 """
 import argparse
 import os
@@ -17,7 +20,16 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PHASES = ["S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
-          "empty-barrier", "reseed.rounds", "reseed.assemble"]
+          "empty-barrier", "reseed.rounds", "reseed.assemble", "async", "refresh"]
+ROUND_CATS = ["round1", "rounds", "dense", "s.round1", "s.rounds"]
+
+
+def card():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    except OSError:
+        return "nvidia-smi not found"
 
 
 def child(wl, nframes):
@@ -69,6 +81,9 @@ def main():
     lo, hi = args.warmup, args.warmup + args.steps
     us = {k: 0.0 for k in PHASES}
     tot = dict(rounds=0, evaluated=0, refreshed=0, reseeded=0, reseed_rounds=0, generations=0, expansions=0)
+    work = {k: [0.0, 0] for k in ROUND_CATS}
+    hist = {"rounds": {}, "s.rounds": {}}
+    aq = dict(evaluations=0, dirty=0, pushes=0, spin_us=0.0)
     gens = {}
     f = -1
     for line in p.stderr.splitlines():
@@ -85,6 +100,17 @@ def main():
             tot["reseed_rounds"] += int(re.match(r"\[x\] reseed rounds (\d+)", line).group(1))
             for name, t, _ in re.findall(r" (\S+) ([\d.]+)/(\d+)", line.split(":", 1)[1]):
                 us[name] += float(t)
+        elif line.startswith("[x] round work"):
+            for name, t, n in re.findall(r" (\S+) ([\d.]+)/(\d+)", line.split(":", 1)[1]):
+                work[name][0] += float(t); work[name][1] += int(n)
+        elif line.startswith("[x] list-length histogram "):
+            name = line.split()[3]
+            for b, c in re.findall(r" (\d+)=(\d+)", line.split(":", 1)[1]):
+                hist[name][int(b)] = hist[name].get(int(b), 0) + int(c)
+        elif line.startswith("[x] async:"):
+            mm = re.search(r"evaluations (\d+) dirty (\d+) pushes (\d+) spin ([\d.]+)", line)
+            aq["evaluations"] += int(mm.group(1)); aq["dirty"] += int(mm.group(2)); aq["pushes"] += int(mm.group(3))
+            aq["spin_us"] += float(mm.group(4))
         elif line.startswith("[x] work-list entries:"):
             mm = re.search(r"evaluated (\d+) refreshed (\d+) reseeded (\d+)", line)
             tot["evaluated"] += int(mm.group(1)); tot["refreshed"] += int(mm.group(2)); tot["reseeded"] += int(mm.group(3))
@@ -92,12 +118,23 @@ def main():
             mm = re.match(r"\[x\] gens (\d+) rounds (\d+)", line)
             tot["generations"] += int(mm.group(1)); tot["rounds"] += int(mm.group(2))
             gens[f] = [tuple(int(v) for v in t.split("/")[:2]) for t in line.split("|", 1)[1].split()]
-    out = ["workload %s, frames %d-%d, phase totals of k_x_relax (ms):" % (args.workload, lo, hi - 1)]
+    out = ["card: " + card(), "FIESTA_X_ASYNC=%s" % os.environ.get("FIESTA_X_ASYNC", "(default)"),
+           "workload %s, frames %d-%d, phase totals of k_x_relax (ms):" % (args.workload, lo, hi - 1)]
     for k in PHASES:
         if k != "empty-barrier":
             out.append("  %-16s %9.2f" % (k, us[k] / 1000.0))
     out.append("  %-16s %9.2f" % ("sum", sum(v for k, v in us.items() if k != "empty-barrier") / 1000.0))
     out.append("  %-16s %9.2f us per empty grid barrier (mean over the frames)" % ("empty-barrier", us["empty-barrier"] / max(1, hi - lo)))
+    out.append("evaluation rounds (ms): wall = summed longest CTA work + barrier and idle; list entries")
+    for k in ROUND_CATS:
+        wall = us[k] / 1000.0
+        wmax = work[k][0] / 1000.0
+        out.append("  %-10s wall %9.2f work %9.2f barrier+idle %9.2f (%5.1f %%) entries %d" %
+                   (k, wall, wmax, wall - wmax, 100.0 * (wall - wmax) / wall if wall else 0.0, work[k][1]))
+    for name, h in hist.items():
+        out.append("list lengths of %s, rounds per log2 bucket [2^(b-1), 2^b): %s" % (name, " ".join("%d:%d" % kv for kv in sorted(h.items()))))
+    out.append("async: evaluations %d dirty re-runs %d pushes %d spin %.2f ms (summed over warps)" %
+               (aq["evaluations"], aq["dirty"], aq["pushes"], aq["spin_us"] / 1000.0))
     for k in ("generations", "rounds", "evaluated", "refreshed", "reseed_rounds", "reseeded", "expansions"):
         out.append("total %s %d" % (k, tot[k]))
     for fr in sorted(gens):
