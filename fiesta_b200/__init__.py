@@ -104,6 +104,7 @@ SYMBOLS = [
     "fiesta_frontiers_create", "fiesta_frontiers_destroy", "fiesta_frontiers_compute", "fiesta_frontiers_clusters",
     "fiesta_frontiers_voxels", "fiesta_frontiers_export", "fiesta_frontiers_score_viewpoints",
     "fiesta_inflate_boxes", "fiesta_corridors",
+    "fiesta_check_poses", "fiesta_check_poses_device", "fiesta_host_mirror_check_poses",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -155,6 +156,10 @@ def load_library():
         L.fiesta_check_segments.argtypes = seg
         L.fiesta_host_mirror_check_segments.argtypes = seg
         L.fiesta_check_segments_device.argtypes = seg + [C.c_void_p]
+        pose = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 3
+        L.fiesta_check_poses.argtypes = pose
+        L.fiesta_host_mirror_check_poses.argtypes = pose
+        L.fiesta_check_poses_device.argtypes = pose + [C.c_void_p]
         L.fiesta_nav_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
         L.fiesta_nav_destroy.argtypes = [C.c_void_p]
         L.fiesta_nav_destroy.restype = None
@@ -198,6 +203,24 @@ def _check_segments_host(fn, h, ab, clearance, unknown_blocks, ck):
     out = (np.empty(n, np.int32), np.empty(n, np.int64), np.empty(n), np.empty(n))
     r, flags = _segment_flags(clearance, unknown_blocks)
     ck(fn(h, ab.ctypes, C.c_int64(n), r, flags, *(o.ctypes for o in out)), "CheckSegments")
+    return out
+
+
+def _half_extents(h):
+    h = _f64(h)
+    if h.shape != (3,):
+        raise ValueError("CheckPoses: half_extents must be 3 numbers, got shape %s" % (h.shape,))
+    return h
+
+
+def _check_poses_host(fn, h, poses, half_extents, clearance, unknown_blocks, ck):
+    """fiesta_check_poses / fiesta_host_mirror_check_poses on host arrays: (status, n_blocked, hit_idx)."""
+    poses = _f64(poses).reshape(-1, 12)
+    n = len(poses)
+    he = _half_extents(half_extents)
+    out = (np.empty(n, np.int32), np.empty(n, np.int32), np.empty(n, np.int64))
+    r, flags = _segment_flags(clearance, unknown_blocks)
+    ck(fn(h, poses.ctypes, C.c_int64(n), he.ctypes, r, flags, *(o.ctypes for o in out)), "CheckPoses")
     return out
 
 
@@ -273,6 +296,12 @@ class HostMirror:
     def CheckSegments(self, ab, clearance, unknown_blocks=False):
         """Segment clearance from the pinned records (fiesta_host_mirror_check_segments): ab (n,6) -> (status, hit_idx, hit_t, min_dist)."""
         return _check_segments_host(self._m._L.fiesta_host_mirror_check_segments, self._h, ab, clearance, unknown_blocks, self._m._ck)
+
+    def CheckPoses(self, poses, half_extents, clearance, unknown_blocks=False):
+        """Robot-shaped collision checks from the pinned records (fiesta_host_mirror_check_poses): poses (n, 12) ->
+        (status, n_blocked, hit_idx)."""
+        return _check_poses_host(self._m._L.fiesta_host_mirror_check_poses, self._h, poses, half_extents, clearance, unknown_blocks,
+                                 self._m._ck)
 
     def close(self):
         if self._h:
@@ -564,6 +593,23 @@ class ESDFMap:
         r, flags = _segment_flags(clearance, unknown_blocks)
         self._ck(self._L.fiesta_check_segments_device(self._h, ab.data_ptr(), n, r, flags, *(o.data_ptr() for o in out), stream),
                  "CheckSegments(device)")
+        return out
+
+    def CheckPoses(self, poses, half_extents, clearance, unknown_blocks=False):
+        """Robot-shaped collision checks (fiesta_check_poses): an oriented box of half extents (h0, h1, h2) metres at n poses
+        {px, py, pz, R00 .. R22} (R world-to-body, row-major: its rows are the box axes) -> (status, n_blocked, hit_idx), status
+        0 clear / 1 blocked / 2 invalid pose / 3 the box leaves the map.  numpy in, numpy out; a CUDA float64 (n, 12) tensor on the
+        map's device runs fiesta_check_poses_device on the current torch stream and returns tensors without synchronising."""
+        if not _is_cuda_tensor(poses):
+            return _check_poses_host(self._L.fiesta_check_poses, self._h, poses, half_extents, clearance, unknown_blocks, self._ck)
+        torch, stream = self._device_tensor(poses, 12, "CheckPoses")
+        he = _half_extents(half_extents)
+        n = poses.shape[0]
+        out = (torch.empty(n, dtype=torch.int32, device=poses.device), torch.empty(n, dtype=torch.int32, device=poses.device),
+               torch.empty(n, dtype=torch.int64, device=poses.device))
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        self._ck(self._L.fiesta_check_poses_device(self._h, poses.data_ptr(), n, he.ctypes, r, flags, *(o.data_ptr() for o in out), stream),
+                 "CheckPoses(device)")
         return out
 
     def GetDistanceBatchDevice(self, pos):

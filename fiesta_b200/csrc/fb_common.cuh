@@ -299,6 +299,16 @@ cudaError_t fb_corr_launch_seeds(const int *L_lo, const int *L_hi, const int *ma
 cudaError_t fb_corr_launch_paths(const int *L_lo, const int *L_hi, const int *max_steps, const uint32_t *mask, const int32_t *P,
                                  const int64_t *off, long long n_paths, int32_t *status, int32_t *n_boxes, int32_t *blocked_at,
                                  int32_t *box_lo, int32_t *box_hi, int32_t *first, FbCorrCtr *ctr, cudaStream_t s);
+// robot-shaped collision checks (fb_pose.cu)
+struct FbPoseBufs {                // device buffers of fiesta_check_poses(_device), kept on the map
+  FbDevBuf<char> io;               // host form: [poses 12n][hit_idx n] 8-byte words, [status n][n_blocked n] int32
+  FbDevBuf<long long> work;        // [n + 1] chunk counts, scanned in place to each pose's first work item (work[n]: total)
+  FbDevBuf<char> tmp;              // CUB temporary storage
+};
+// Expects a validated call (fb_pose.h limits) with n >= 0; writes status / n_blocked / hit_idx, device pointers, on stream s.
+int fb_pose_check_batch(const FbGeom &g, const uint32_t *cobs, const double *poses, long long n, const double *h, double clearance,
+                        int unknown_blocks, int32_t *status, int32_t *n_blocked, int64_t *hit_idx, FbPoseBufs &B, cudaStream_t s,
+                        int *launches);
 struct FbDepthRel { double m[16]; };
 struct fiesta_depth_params;
 cudaError_t fb_depth_to_cloud(const uint16_t *d_img, const uint16_t *d_last, int rows, int cols, const fiesta_depth_params &p, int filter_on,

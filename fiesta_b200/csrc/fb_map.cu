@@ -3,6 +3,7 @@
 // Host code mirrors what the reference does on the caller's thread with pure arithmetic (index conversions,
 // update-range bookkeeping, sentinel returns: FIESTA src/ESDFMap.cpp:46-118, 401-421, 792-824) and hands every
 // per-voxel operation to the device.  There is NO CPU fallback: fiesta_create fails without an sm_90 device.
+#include <float.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -18,6 +19,7 @@
 #include "fb_exact.h"
 #include "fb_segment.h"
 #include "fb_corridor.h"
+#include "fb_pose.h"
 
 static thread_local std::string g_last_error;
 void fb_set_error(const char *fmt, ...) {
@@ -65,6 +67,7 @@ struct fiesta_map {
   FbDevBuf<double> d_qin, d_qout;
   FbDevBuf<char> d_seg;             // fiesta_check_segments: [ab 6n][hit_t n][min_dist n] doubles, [hit_idx n] int64, [status n] int32
   FbCorrBufs corr;                  // fiesta_inflate_boxes / fiesta_corridors
+  FbPoseBufs pose;                  // fiesta_check_poses / fiesta_check_poses_device
   cudaEvent_t ev[4] = {};
   cudaEvent_t ev_q[2] = {};         // device queries: map stream -> caller's stream, and back
   FbDevBuf<unsigned long long> d_dbg;
@@ -944,6 +947,61 @@ int fiesta_check_segments_device(fiesta_map *m, const double *d_ab, int64_t n, d
   return device_query_end(m, s);
 }
 
+// ---- robot-shaped collision checks (fb_pose.h, fb_pose.cu): oriented boxes at many poses
+static int pose_args(const fiesta_map *m, const char *fn, int64_t n, const double *h, double clearance, int flags, bool buffers) {
+  if (!h) { fb_set_error("%s: null half_extents", fn); return FIESTA_ERR_INVALID; }
+  for (int k = 0; k < 3; ++k)
+    if (!(h[k] >= 0.0 && h[k] <= DBL_MAX)) { fb_set_error("%s: half extents must be finite and >= 0", fn); return FIESTA_ERR_INVALID; }
+  if (!segment_args_ok(fn, n, clearance, flags, buffers)) return FIESTA_ERR_INVALID;
+  if ((h[0] + h[1]) + h[2] > FB_POSE_MAX_SPAN * m->g.res) {
+    fb_set_error("%s: h0 + h1 + h2 = %g m exceeds %d voxels", fn, (h[0] + h[1]) + h[2], FB_POSE_MAX_SPAN);
+    return FIESTA_ERR_LIMIT;
+  }
+  if (n >= INT32_MAX) { fb_set_error("%s: n = %lld poses, the limit is 2^31 - 2", fn, (long long)n); return FIESTA_ERR_LIMIT; }
+  return FIESTA_OK;
+}
+int fiesta_check_poses(fiesta_map *m, const double *poses, int64_t n, const double half_extents[3], double clearance, int flags,
+                       int32_t *status, int32_t *n_blocked, int64_t *hit_idx) {
+  const char *fn = "fiesta_check_poses";
+  if (!m) return FIESTA_ERR_INVALID;
+  int r;
+  if ((r = pose_args(m, fn, n, half_extents, clearance, flags, poses && status && n_blocked && hit_idx))) return r;
+  if (n == 0) return FIESTA_OK;
+  CK(cudaSetDevice(m->device));
+  CK(m->pose.io.grow((size_t)n * 112, m->stream));
+  double *d_poses = reinterpret_cast<double *>(m->pose.io.p);
+  int64_t *d_idx = reinterpret_cast<int64_t *>(d_poses + 12 * n);
+  int32_t *d_st = reinterpret_cast<int32_t *>(d_idx + n), *d_nb = d_st + n;
+  CK(cudaMemcpyAsync(d_poses, poses, (size_t)n * 96, cudaMemcpyHostToDevice, m->stream));
+  int launches = 0;
+  if ((r = fb_pose_check_batch(m->g, m->cobs, d_poses, n, half_extents, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, d_st, d_nb, d_idx,
+                               m->pose, m->stream, &launches)))
+    return r;
+  m->st.kernel_launches += launches;
+  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(n_blocked, d_nb, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(hit_idx, d_idx, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+int fiesta_check_poses_device(fiesta_map *m, const double *d_poses, int64_t n, const double half_extents[3], double clearance, int flags,
+                              int32_t *d_status, int32_t *d_n_blocked, int64_t *d_hit_idx, void *stream) {
+  const char *fn = "fiesta_check_poses_device";
+  if (!m) return FIESTA_ERR_INVALID;
+  int r;
+  if ((r = pose_args(m, fn, n, half_extents, clearance, flags, d_poses && d_status && d_n_blocked && d_hit_idx))) return r;
+  const cudaStream_t s = (cudaStream_t)stream;
+  if ((r = device_query_begin(m, fn, s))) return r;
+  if (n > 0) {
+    int launches = 0;
+    if ((r = fb_pose_check_batch(m->g, m->cobs, d_poses, n, half_extents, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, d_status,
+                                 d_n_blocked, d_hit_idx, m->pose, s, &launches)))
+      return r;
+    m->st.kernel_launches += launches;
+  }
+  return device_query_end(m, s);
+}
+
 // ---- cost-to-go field (fb_nav.h, fb_nav.cu): a box's geodesic distance to a goal set through free space at a clearance
 struct fiesta_nav_field {
   fiesta_map *m = nullptr;
@@ -1716,6 +1774,17 @@ int fiesta_host_mirror_check_segments(const fiesta_host_mirror *p, const double 
   const bool unknown_blocks = (flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS) != 0;
   for (int64_t i = 0; i < n; ++i)
     fb_seg_check(p->m->g, p->h_rec, ab + 6 * i, clearance, unknown_blocks, status + i, hit_idx + i, hit_t + i, min_dist + i);
+  return FIESTA_OK;
+}
+int fiesta_host_mirror_check_poses(const fiesta_host_mirror *p, const double *poses, int64_t n, const double half_extents[3],
+                                   double clearance, int flags, int32_t *status, int32_t *n_blocked, int64_t *hit_idx) {
+  if (!p) return FIESTA_ERR_INVALID;
+  int r;
+  if ((r = pose_args(p->m, "fiesta_host_mirror_check_poses", n, half_extents, clearance, flags, poses && status && n_blocked && hit_idx)))
+    return r;
+  const bool unknown_blocks = (flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS) != 0;
+  for (int64_t i = 0; i < n; ++i)
+    fb_pose_check(p->m->g, p->h_rec, poses + 12 * i, half_extents, clearance, unknown_blocks, status + i, n_blocked + i, hit_idx + i);
   return FIESTA_OK;
 }
 const uint32_t *fiesta_host_mirror_records(const fiesta_host_mirror *p) { return p ? p->h_rec.p : nullptr; }

@@ -227,6 +227,41 @@ int fiesta_check_segments(fiesta_map *m, const double *ab, int64_t n, double cle
 int fiesta_host_mirror_check_segments(const fiesta_host_mirror *p, const double *ab, int64_t n, double clearance, int flags,
                                       int32_t *status, int64_t *hit_idx, double *hit_t, double *min_dist);
 
+/* ---- robot-shaped collision checks (planners: hybrid A* / lattice motion primitives, MPPI rollouts, any robot that is not a sphere) ----
+ * Does an oriented box at a pose touch a voxel that blocks?  The half extents h[3] (metres, finite, >= 0; zeros give a plate, a
+ * segment or a point) are shared by the n poses of a call.  A pose is 12 doubles {px, py, pz, R00 .. R22}: p is the box centre in
+ * metres, R a row-major 3x3 world-to-body matrix whose rows u_0, u_1, u_2 are the box axes in world coordinates (the convention of
+ * the viewpoint orientations).  The rows are used exactly as given: no orthonormality check, no trigonometry; the result describes
+ * a box only when R is a rotation.
+ *   touched   voxel v (any integer triple, in the grid or not) with centre c_k = ((double)v_k + 0.5) * resolution + origin_k and
+ *             d_k = c_k - p_k is touched iff the closed cube of half-edge r = resolution / 2 and the closed box intersect, decided
+ *             by the separating-axis test over the world axes e_k, the box axes u_j and the nine products e_k x u_j: no L has
+ *             fabs(proj_L) > T_L, where, each fp64 operation rounded on its own,
+ *               proj_L = (L0*d0 + L1*d1) + L2*d2,  u_j.L = (u_j0*L0 + u_j1*L1) + u_j2*L2,
+ *               T_L = r * ((fabs(L0) + fabs(L1)) + fabs(L2)) + ((h0*fabs(u_0.L) + h1*fabs(u_1.L)) + h2*fabs(u_2.L)).
+ *             Touching faces count: a body whose face touches an obstacle's face collides.
+ *   blocking  a touched grid voxel blocks as in segment clearance: GetDistance(Vector3i) <= clearance (clearance 0: obstacle voxels
+ *             only) or, with FIESTA_SEGMENT_UNKNOWN_BLOCKS, never observed.
+ * Outputs per pose:
+ *   status    0 = no touched grid voxel blocks and the box stays in the grid; 1 = some touched grid voxel blocks; 2 = invalid pose:
+ *             p has a NaN or fails PosInMap, an R entry is non-finite or some |R_jk| > 1 + 2^-20; 3 = nothing blocks, but the box
+ *             touches a voxel outside the grid (it leaves the map).  1 takes precedence over 3.  Voxels outside the grid are never
+ *             read as records; a planner that wants the map's edge to block treats status 3 as blocked.
+ *   n_blocked the number of touched blocking grid voxels (0 unless status 1)
+ *   hit_idx   the least linear index x*Gy*Gz + y*Gz + z among them, else -1
+ * Every output is an integer decided by fixed fp64 expressions and the records: the same bits on every run and as the sequential
+ * definition (tests/poseref.py).  A union of boxes is the OR of the statuses of one call per box.  Errors, after which nothing is
+ * written: FIESTA_ERR_INVALID for a NaN, infinite or negative half extent, a clearance or flags that fiesta_check_segments
+ * rejects, n < 0, null half_extents, or null buffers with n > 0; FIESTA_ERR_LIMIT when h0 + h1 + h2 > 256 * resolution (at most
+ * 518 candidate voxels per axis) or n >= 2^31 - 1.  Memory on the map, grown as needed: 8 bytes per pose (work list) plus scan
+ * storage, and 112 bytes per pose for the host form's staging. */
+/* host pointers; synchronous like the other batch queries */
+int fiesta_check_poses(fiesta_map *m, const double *poses /* n * 12 */, int64_t n, const double half_extents[3], double clearance,
+                       int flags, int32_t *status, int32_t *n_blocked, int64_t *hit_idx);
+/* pure host code on the pinned records, as of the last refresh */
+int fiesta_host_mirror_check_poses(const fiesta_host_mirror *p, const double *poses, int64_t n, const double half_extents[3],
+                                   double clearance, int flags, int32_t *status, int32_t *n_blocked, int64_t *hit_idx);
+
 /* ---- cost-to-go field (planners: A* / hybrid-A* heuristics, guide paths for trajectory optimisers, cost to frontier goals) ----
  * How far is the nearest goal through free space, keeping a clearance, and which way leads there?  The field covers an inclusive
  * voxel box [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis) and is a snapshot of the records at the time of the call.
@@ -445,6 +480,10 @@ int fiesta_corridors(fiesta_map *m, const int box_lo[3], const int box_hi[3], co
  * stream is rejected with FIESTA_ERR_INVALID. */
 int fiesta_check_segments_device(fiesta_map *m, const double *d_ab, int64_t n, double clearance, int flags, int32_t *d_status,
                                  int64_t *d_hit_idx, double *d_hit_t, double *d_min_dist, void *stream);
+/* Robot-shaped collision checks on device poses (n * 12 doubles); half_extents is a HOST array.  The work list and scan storage
+ * are the map's own (queries are ordered through the map's stream, so two of them never share them at once). */
+int fiesta_check_poses_device(fiesta_map *m, const double *d_poses, int64_t n, const double half_extents[3] /* host */,
+                              double clearance, int flags, int32_t *d_status, int32_t *d_n_blocked, int64_t *d_hit_idx, void *stream);
 int fiesta_get_distance_batch_device(fiesta_map *m, const double *d_pos_xyz, int64_t n, double *d_dist, void *stream);
 int fiesta_get_dist_grad_trilinear_batch_device(fiesta_map *m, const double *d_pos_xyz, int64_t n, double *d_dist, double *d_grad_xyz,
                                                 void *stream);

@@ -149,6 +149,25 @@ class ESDFMap {
     check(fiesta_check_segments_device(h_, d_ab, n, clearance, flags, d_status, d_hit_idx, d_hit_t, d_min_dist, stream),
           "CheckSegmentsDevice");
   }
+  // Robot-shaped collision checks (fiesta_check_poses in fiesta_b200.h): an oriented box of half extents h (metres) at n poses
+  // {px, py, pz, R00 .. R22} (R world-to-body, rows = box axes); per pose status (0 clear, 1 blocked, 2 invalid pose, 3 leaves the
+  // map), the number of touched blocking voxels and the least linear index among them.  flags: FIESTA_SEGMENT_UNKNOWN_BLOCKS.
+  // Host pointers, synchronous.
+  void CheckPoses(const double *poses, long n, const double half_extents[3], double clearance, int flags, int32_t *status,
+                  int32_t *n_blocked, int64_t *hit_idx) {
+    check(fiesta_check_poses(h_, poses, n, half_extents, clearance, flags, status, n_blocked, hit_idx), "CheckPoses");
+  }
+  // The same on DEVICE poses and outputs (half_extents stays on the host), enqueued on `stream` without synchronising the host.
+  void CheckPosesDevice(const double *d_poses, long n, const double half_extents[3], double clearance, int flags, int32_t *d_status,
+                        int32_t *d_n_blocked, int64_t *d_hit_idx, void *stream) {
+    check(fiesta_check_poses_device(h_, d_poses, n, half_extents, clearance, flags, d_status, d_n_blocked, d_hit_idx, stream),
+          "CheckPosesDevice");
+  }
+  // The same from a host mirror's pinned records (pure host code, as of its last refresh).
+  void CheckPosesMirror(const fiesta_host_mirror *p, const double *poses, long n, const double half_extents[3], double clearance,
+                        int flags, int32_t *status, int32_t *n_blocked, int64_t *hit_idx) {
+    check(fiesta_host_mirror_check_poses(p, poses, n, half_extents, clearance, flags, status, n_blocked, hit_idx), "CheckPosesMirror");
+  }
   // Cost-to-go field for planners (fiesta_nav_* in fiesta_b200.h): geodesic distance from every voxel of a box to the nearest
   // goal through free space at a clearance, and paths down it.  Destroy the field with fiesta_nav_destroy before the map.
   fiesta_nav_field *MakeNavField() {
