@@ -135,6 +135,7 @@ struct FbEsdfArgs {
   FbCounters *ctr;
   double l_occ;
   int tile_x_lo, tile_x_hi;  // tile columns [lo, hi) this map relaxes (x-slab sharding; whole grid when unsharded)
+  int pull_all;              // every queued voxel pulls from all 24 neighbours (see `pulls` in k_wavefront)
   unsigned long long *dbg;   // optional per-generation trace: {nwork, nchanged, t_phase1_ns, t_phase2_ns} x 256 (FIESTA_DEBUG_WF=1)
 };
 

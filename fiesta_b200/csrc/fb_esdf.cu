@@ -260,11 +260,13 @@ k_wavefront(const __grid_constant__ CUtensorMap tmap, FbGeom g, FbEsdfArgs a) {
         // A voxel relaxes iff it has been observed (unknown voxels are barriers: distance_ = -10000 is never > tmp,
         // ESDFMap.cpp:382) and lies inside the update box (only in-box voxels are ever queued, ESDFMap.cpp:351,378).
         updatable[h] = (orig[h] & FB_CODE_MASK) != FB_UNKNOWN && fb_in_range(g, vx, vy, vz);
-        // With the whole grid in the update box every value a neighbour holds was offered to this voxel when it was set
-        // (the neighbour was in the queue then) and records only improve -- so the pull of a queued voxel (ESDFMap.cpp:
-        // 349-367) can only find something new if its own record was (re)set to "no obstacle": first observation or a
-        // deleted obstacle.  With a moving update box (VoxInRange, :351) that does not hold and every queued voxel pulls.
-        pulls[h] = !g.box_is_full || (orig[h] & FB_CODE_MASK) == FB_INF;
+        // While every relaxation of this map has covered the whole grid, every value a neighbour holds was offered to this
+        // voxel when it was set (the neighbour was in the queue then) and records only improve -- so the pull of a queued
+        // voxel (ESDFMap.cpp:349-367) can only find something new if its own record was (re)set to "no obstacle": first
+        // observation, local-map reset or a deleted obstacle.  Once a relaxation ran under a smaller box, VoxInRange(new_pos)
+        // (:351) withheld pushes to the voxels outside it, so that does not hold any more and every queued voxel pulls
+        // (a.pull_all, sticky per map).
+        pulls[h] = a.pull_all || (orig[h] & FB_CODE_MASK) == FB_INF;
         nmask[h] = 0xffffffu;
         if (!g.box_is_full) {                                 // VoxInRange(new_pos), ESDFMap.cpp:351
           nmask[h] = 0;

@@ -83,6 +83,9 @@ struct fiesta_map {
   int mode = FIESTA_MODE_EXACT;
   int shard_rank = 0, shard_world = 1, tile_x_lo = 0, tile_x_hi = 0;
   FbDevBuf<unsigned> d_halo_changed;
+  // FAST mode: some relaxation (UpdateESDF / shard_relax) ran under an update box that is not the whole grid, so voxels
+  // outside it may hold values their neighbours never offered them; from then on every queued voxel pulls (DESIGN 3.3)
+  bool local_box_seen = false;
   FbExact X;
   fiesta_stats st{};
   // pinned host mirror (next #3): union of the update boxes that were current while records could change
@@ -310,6 +313,7 @@ static void fill_esdf_args(fiesta_map *m, FbEsdfArgs &a) {
   a.cobs = m->cobs; a.cobs_b = m->cobs_b; a.occ = m->occ; a.occbits = m->occbits; a.tile_flag = m->tile_flag; a.nb_flag = m->nb_flag;
   for (int k = 0; k < 2; ++k) { a.list[k] = m->list[k]; a.changed[k] = m->changed[k]; a.changed_bbox[k] = m->changed_bbox[k]; }
   a.ctr = m->d_ctr; a.l_occ = m->l_occ; a.tile_x_lo = m->tile_x_lo; a.tile_x_hi = m->tile_x_hi; a.dbg = nullptr;
+  a.pull_all = (m->local_box_seen || !m->g.box_is_full) ? 1 : 0;
 }
 // FRESH flags the seed / delete scan / wavefront left in the ghost layers of a sharded map
 static int retire_halos(fiesta_map *m) {
@@ -756,6 +760,7 @@ int fiesta_update_esdf(fiesta_map *m) {
   }
   FbEsdfArgs a;
   fill_esdf_args(m, a);
+  if (!m->g.box_is_full) m->local_box_seen = true;                        // the box in force when the relaxation runs
   static const bool dbg_wf = getenv("FIESTA_DEBUG_WF") != nullptr;
   if (dbg_wf) { if (!m->d_dbg) CK(m->d_dbg.alloc(2048)); CK(cudaMemsetAsync(m->d_dbg, 0, 2048 * 8, m->stream)); a.dbg = m->d_dbg; }
   CK(cudaEventRecord(m->ev[0], m->stream));
@@ -1877,6 +1882,7 @@ int fiesta_shard_relax(fiesta_map *m, int64_t *changed) {
   CK(cudaSetDevice(m->device));
   mark_dirty(m);
   FbEsdfArgs a; fill_esdf_args(m, a);
+  if (!m->g.box_is_full) m->local_box_seen = true;
   k_reset_esdf_ctr<<<1, 1, 0, m->stream>>>(m->d_ctr);
   CK(fb_esdf_wavefront(m->g, a, m->tmap, m->wf_blocks, m->stream));
   int r;

@@ -15,6 +15,8 @@
  * Two switches exist to study variants offline: FM_FULL_PULL (every queued voxel pulls, the literal reading of
  * ESDFMap.cpp:349-367) and FM_EXIT_TEST (a visiting tile decides exactly whether its changes can improve a neighbour's
  * border before queueing it).  Both must leave the arrays unchanged.
+ * Also modelled: the local-map reset of UpdateOccupancy(false) (fm_local_reset) and the x-slab sharded UpdateESDF
+ * (fm_set_slab / fm_pack / fm_halo_ingest / fm_relax, tests/test_fast_model_boxes.py).
  */
 #include <math.h>
 #include <stdint.h>
@@ -39,6 +41,8 @@ typedef struct fm {
   uint32_t *tile_flag, *nb_flag;
   uint32_t *list[2], *changed, *changed_bb, *changed_need;
   unsigned n_list[2], n_changed, stamp;
+  int pull_all;                /* sticky: some UpdateESDF / relax ran under a box that is not the whole grid */
+  int slab_lo, slab_hi;        /* tile columns [lo, hi) this map relaxes (x-slab sharding; all of them when unsharded) */
 } fm;
 
 static const int KD[24][3] = {{-1, 0, 0}, {1, 0, 0}, {0, -1, 0}, {0, 1, 0}, {0, 0, -1}, {0, 0, 1},
@@ -83,6 +87,7 @@ fm *fm_create_tiled(int gx, int gy, int gz, int tile) {
   m->lo[0] = m->lo[1] = m->lo[2] = 0;
   m->hi[0] = gx - 1; m->hi[1] = gy - 1; m->hi[2] = gz - 1;
   m->stamp = 1;
+  m->slab_lo = 0; m->slab_hi = m->tx;
   return m;
 }
 fm *fm_create(int gx, int gy, int gz) { return fm_create_tiled(gx, gy, gz, 8); }
@@ -100,8 +105,11 @@ void fm_observe(fm *m, const uint32_t *idx, long long n) {
     if (m->code[idx[i]] == FM_UNKNOWN) m->code[idx[i]] = FM_INF;
 }
 
-/* fb_activate: queue tile t for the generation `stamp`; work = a neighbour / seed / reset asks for a full visit */
+/* fb_activate: queue tile t for the generation `stamp`; work = a neighbour / seed / reset asks for a full visit.
+ * Tiles outside this map's x-slab belong to another rank and are never queued here. */
 static void activate(fm *m, unsigned t, unsigned stamp, int which, int work) {
+  const int txc = (int)(t / ((unsigned)m->ty * (unsigned)m->tz));
+  if (txc < m->slab_lo || txc >= m->slab_hi) return;
   if (work) m->nb_flag[t] = stamp;
   if (m->tile_flag[t] != stamp) { m->tile_flag[t] = stamp; m->list[which][m->n_list[which]++] = t; }
 }
@@ -111,46 +119,24 @@ static void activate(fm *m, unsigned t, unsigned stamp, int which, int work) {
 #define BIDX(bx, by, bz) (((bx) * BOX + (by)) * BOX + (bz))
 #define VIDX(lx, ly, lz) (((lx) * T + (ly)) * T + (lz))
 
-/* stats: 0 generations, 1 full visits, 2 retire-only visits, 3 changed records, 4 reset records, 5 neighbour activations
- * asked for by the bounding-box rule, 6 of those suppressed by the exit test, 7 local iterations, 8 voxel evaluations
- * (listed voxels summed over the iterations), 9 candidate records compared */
-void fm_update(fm *m, const uint8_t *exist, const uint32_t *ins, long long n_ins, int have_del, int flags, long long *stats) {
-  const int full_box = box_is_full(m);
-  const int T = m->T, lg = m->lg, BOX = T + 4;
-  long long st[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+/* k_halo_retire: FRESH flags that E1 / E2 / E3 left in the ghost layers of a sharded map */
+static void retire_halos(fm *m) {
+  const long long per = (long long)m->gy * m->gz;
+  const int x0 = m->slab_lo * m->T, x1 = m->slab_hi * m->T < m->gx ? m->slab_hi * m->T : m->gx;
+  if (m->slab_lo > 0)
+    for (long long k = (long long)(x0 - 2) * per; k < (long long)x0 * per; ++k) m->code[k] &= FM_MASK;
+  if (m->slab_hi < m->tx)
+    for (long long k = (long long)x1 * per; k < (long long)(x1 + 2) * per; ++k) m->code[k] &= FM_MASK;
+}
+
+/* E3 (k_wavefront): generations over the tiles queued for generation m->stamp in list 0 */
+static void wavefront(fm *m, int flags, long long *st) {
+  const int T = m->T, BOX = T + 4;
   const unsigned stamp0 = m->stamp;
-  m->n_list[0] = m->n_list[1] = 0;
-  /* E1 (ESDFMap.cpp:278-291) */
-  for (long long i = 0; i < n_ins; ++i) {
-    const uint32_t ii = ins[i];
-    if (!exist[ii]) continue;
-    const int z = (int)(ii % (unsigned)m->gz), y = (int)((ii / (unsigned)m->gz) % (unsigned)m->gy), x = (int)(ii / ((unsigned)m->gz * (unsigned)m->gy));
-    m->code[ii] = pack(x, y, z) | FM_FRESH;
-    const int tx0 = (x - 2 > 0 ? x - 2 : 0) >> lg, tx1 = (x + 2 < m->gx - 1 ? x + 2 : m->gx - 1) >> lg;
-    const int ty0 = (y - 2 > 0 ? y - 2 : 0) >> lg, ty1 = (y + 2 < m->gy - 1 ? y + 2 : m->gy - 1) >> lg;
-    const int tz0 = (z - 2 > 0 ? z - 2 : 0) >> lg, tz1 = (z + 2 < m->gz - 1 ? z + 2 : m->gz - 1) >> lg;
-    for (int a = tx0; a <= tx1; ++a)
-      for (int b = ty0; b <= ty1; ++b)
-        for (int c = tz0; c <= tz1; ++c) activate(m, (unsigned)((a * m->ty + b) * m->tz + c), stamp0, 0, 1);
-  }
-  /* E2 (ESDFMap.cpp:292-337): dependants of deleted obstacles, found by a scan instead of the linked lists */
-  if (have_del)
-    for (int x = 0; x < m->gx; ++x)
-      for (int y = 0; y < m->gy; ++y)
-        for (int z = 0; z < m->gz; ++z) {
-          const long long ii = lin(m, x, y, z);
-          const uint32_t c = m->code[ii] & FM_MASK;
-          if (c >= 2u) {
-            int ox, oy, oz;
-            unpack(c, &ox, &oy, &oz);
-            if (!exist[lin(m, ox, oy, oz)]) {
-              m->code[ii] = FM_INF | FM_FRESH;
-              ++st[4];
-              activate(m, (unsigned)(((x >> lg) * m->ty + (y >> lg)) * m->tz + (z >> lg)), stamp0, 0, 1);
-            }
-          }
-        }
-  /* E3 */
+  /* A queued voxel may skip its pull only while every value a neighbour holds has been offered to it.  That holds for a
+   * map whose update box has always been the whole grid; once a relaxation ran under a smaller box, VoxInRange(new_pos)
+   * (ESDFMap.cpp:351) withheld pushes to the voxels outside it, and from then on every queued voxel pulls. */
+  const int pull_all = (flags & FM_FULL_PULL) || m->pull_all;
   unsigned cur = 0, gen = 0;
   static uint32_t V[MAXBOX * MAXBOX * MAXBOX], orig[MAXBOX * MAXBOX * MAXBOX], nv[MAXT * MAXT * MAXT];
   static unsigned char fresh[MAXBOX * MAXBOX * MAXBOX], upd[MAXT * MAXT * MAXT], pulls[MAXT * MAXT * MAXT], chg[MAXBOX * MAXBOX * MAXBOX];
@@ -186,7 +172,7 @@ void fm_update(fm *m, const uint8_t *exist, const uint32_t *ins, long long n_ins
             const uint32_t c = V[BIDX(lx + 2, ly + 2, lz + 2)];
             /* unknown voxels are barriers (distance_ = -10000 is never > tmp, ESDFMap.cpp:382); only in-box voxels are queued */
             upd[v] = (unsigned char)(c != FM_UNKNOWN && in_range(m, x0 + lx, y0 + ly, z0 + lz));
-            pulls[v] = (unsigned char)((flags & FM_FULL_PULL) || !full_box || c == FM_INF);
+            pulls[v] = (unsigned char)(pull_all || c == FM_INF);
           }
       for (;;) {                                          /* local Jacobi iterations */
         ++st[7];
@@ -333,6 +319,89 @@ void fm_update(fm *m, const uint8_t *exist, const uint32_t *ins, long long n_ins
   }
   st[0] = gen;
   m->stamp = stamp0 + gen + 1u;
+}
+
+/* stats: 0 generations, 1 full visits, 2 retire-only visits, 3 changed records, 4 reset records, 5 neighbour activations
+ * asked for by the bounding-box rule, 6 of those suppressed by the exit test, 7 local iterations, 8 voxel evaluations
+ * (listed voxels summed over the iterations), 9 candidate records compared */
+void fm_update(fm *m, const uint8_t *exist, const uint32_t *ins, long long n_ins, int have_del, int flags, long long *stats) {
+  const int lg = m->lg;
+  long long st[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const unsigned stamp0 = m->stamp;
+  m->n_list[0] = m->n_list[1] = 0;
+  if ((n_ins > 0 || have_del) && !box_is_full(m)) m->pull_all = 1;   /* the box in force when the relaxation runs */
+  /* E1 (ESDFMap.cpp:278-291) */
+  for (long long i = 0; i < n_ins; ++i) {
+    const uint32_t ii = ins[i];
+    if (!exist[ii]) continue;
+    const int z = (int)(ii % (unsigned)m->gz), y = (int)((ii / (unsigned)m->gz) % (unsigned)m->gy), x = (int)(ii / ((unsigned)m->gz * (unsigned)m->gy));
+    m->code[ii] = pack(x, y, z) | FM_FRESH;
+    const int tx0 = (x - 2 > 0 ? x - 2 : 0) >> lg, tx1 = (x + 2 < m->gx - 1 ? x + 2 : m->gx - 1) >> lg;
+    const int ty0 = (y - 2 > 0 ? y - 2 : 0) >> lg, ty1 = (y + 2 < m->gy - 1 ? y + 2 : m->gy - 1) >> lg;
+    const int tz0 = (z - 2 > 0 ? z - 2 : 0) >> lg, tz1 = (z + 2 < m->gz - 1 ? z + 2 : m->gz - 1) >> lg;
+    for (int a = tx0; a <= tx1; ++a)
+      for (int b = ty0; b <= ty1; ++b)
+        for (int c = tz0; c <= tz1; ++c) activate(m, (unsigned)((a * m->ty + b) * m->tz + c), stamp0, 0, 1);
+  }
+  /* E2 (ESDFMap.cpp:292-337): dependants of deleted obstacles, found by a scan instead of the linked lists */
+  if (have_del)
+    for (int x = 0; x < m->gx; ++x)
+      for (int y = 0; y < m->gy; ++y)
+        for (int z = 0; z < m->gz; ++z) {
+          const long long ii = lin(m, x, y, z);
+          const uint32_t c = m->code[ii] & FM_MASK;
+          if (c >= 2u) {
+            int ox, oy, oz;
+            unpack(c, &ox, &oy, &oz);
+            if (!exist[lin(m, ox, oy, oz)]) {
+              m->code[ii] = FM_INF | FM_FRESH;
+              ++st[4];
+              activate(m, (unsigned)(((x >> lg) * m->ty + (y >> lg)) * m->tz + (z >> lg)), stamp0, 0, 1);
+            }
+          }
+        }
+  wavefront(m, flags, st);
+  retire_halos(m);
+  if (stats) memcpy(stats, st, sizeof(st));
+}
+
+/* UpdateOccupancy(false) of a voxel outside the previous update box (ESDFMap.cpp:256-259, k_integrate<false>): distance_
+ * +infinity_, not queued */
+void fm_local_reset(fm *m, const uint32_t *idx, long long n) {
+  for (long long i = 0; i < n; ++i) m->code[idx[i]] = FM_INF;
+}
+
+/* ---- x-slab sharding (fiesta_set_shard / fiesta_shard_pack / fiesta_shard_ingest / fiesta_shard_relax).  Layers are
+ * gy*gz records in this model's own (unpadded) layout; only model instances exchange them. */
+void fm_set_slab(fm *m, int tile_x_lo, int tile_x_hi) { m->slab_lo = tile_x_lo; m->slab_hi = tile_x_hi; }
+void fm_pack(const fm *m, int x_first, int nlayers, uint32_t *out) {
+  memcpy(out, m->code + (long long)x_first * m->gy * m->gz, (size_t)nlayers * m->gy * m->gz * 4);
+}
+/* k_halo_ingest: a received ghost record that differs from the local copy is taken over, marked FRESH (it pushes into the
+ * slab next generation) and the own tiles of column own_tile_x within reach are queued.  Returns the changed records. */
+long long fm_halo_ingest(fm *m, const uint32_t *recv, int x_first, int nlayers, int own_tile_x) {
+  const long long per = (long long)m->gy * m->gz;
+  long long n = 0;
+  for (long long k = 0; k < per * nlayers; ++k) {
+    const int y = (int)((k % per) / m->gz), z = (int)(k % m->gz);
+    const long long ii = (long long)x_first * per + k;
+    const uint32_t nw = recv[k] & FM_MASK;
+    if (nw == (m->code[ii] & FM_MASK)) continue;
+    m->code[ii] = nw | FM_FRESH;
+    ++n;
+    const int ty0 = (y - 2 > 0 ? y - 2 : 0) >> m->lg, ty1 = (y + 2 < m->gy - 1 ? y + 2 : m->gy - 1) >> m->lg;
+    const int tz0 = (z - 2 > 0 ? z - 2 : 0) >> m->lg, tz1 = (z + 2 < m->gz - 1 ? z + 2 : m->gz - 1) >> m->lg;
+    for (int b = ty0; b <= ty1; ++b)
+      for (int c = tz0; c <= tz1; ++c) activate(m, (unsigned)((own_tile_x * m->ty + b) * m->tz + c), m->stamp, 0, 1);
+  }
+  return n;
+}
+/* fiesta_shard_relax: E3 over the tiles the ingests queued, then the ghost flags are retired */
+void fm_relax(fm *m, int flags, long long *stats) {
+  long long st[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  if (!box_is_full(m)) m->pull_all = 1;
+  wavefront(m, flags, st);
+  retire_halos(m);
   if (stats) memcpy(stats, st, sizeof(st));
 }
 
@@ -354,9 +423,12 @@ void fm_export(const fm *m, int32_t *cobs, double *dist, double res) {
         if (dist) dist[ii] = d;
       }
 }
-/* number of records still carrying the FRESH bit (must be 0 between updates) */
+/* number of records of the slab and its ghost layers still carrying the FRESH bit (must be 0 between updates; records
+ * further out are neither relaxed nor read by this map) */
 long long fm_fresh_left(const fm *m) {
+  const long long per = (long long)m->gy * m->gz;
+  const int x0 = m->slab_lo * m->T - 2, x1 = m->slab_hi * m->T + 2;
   long long n = 0;
-  for (long long i = 0; i < m->total; ++i) n += (m->code[i] >> 31);
+  for (long long i = (x0 > 0 ? x0 : 0) * per; i < (x1 < m->gx ? x1 : m->gx) * per; ++i) n += (m->code[i] >> 31);
   return n;
 }

@@ -267,6 +267,7 @@ class FastModel:
         self._L = C.CDLL(path)
         self._L.fm_create_tiled.restype = C.c_void_p
         self._L.fm_fresh_left.restype = C.c_longlong
+        self._L.fm_halo_ingest.restype = C.c_longlong
         self.grid_size = tuple(int(g) for g in grid_size)
         self.n = int(np.prod(self.grid_size))
         self.res = float(resolution)
@@ -289,21 +290,49 @@ class FastModel:
     def set_range(self, lo, hi):
         self._L.fm_set_range(self._h, I3(*[int(x) for x in lo]), I3(*[int(x) for x in hi]))
 
-    def update(self, dist, occ, flags=0):
-        """One UpdateESDF.  dist: distance_ (only `!= -10000` = observed is used), occ: occupancy log-odds."""
+    KEYS = ("generations", "full_visits", "retire_visits", "changed", "reset", "activations", "suppressed", "iterations",
+            "evaluations", "candidates")
+
+    def update(self, dist, occ, flags=0, reset=None):
+        """One UpdateESDF.  dist: distance_ (only `!= -10000` = observed is used), occ: occupancy log-odds, reset: linear
+        indices the local-map reset of UpdateOccupancy(false) set to +infinity (applied before the seeds and the delete scan)."""
         seen = np.asarray(dist) != -10000.0
         new = np.flatnonzero(seen & ~self._seen).astype(np.uint32)
         self._L.fm_observe(self._h, new.ctypes, C.c_longlong(len(new)))
         self._seen = seen
+        if reset is not None and len(reset):
+            r = np.ascontiguousarray(reset, dtype=np.uint32)
+            self._L.fm_local_reset(self._h, r.ctypes, C.c_longlong(len(r)))
         exist = (np.asarray(occ) > self.l_occ).astype(np.uint8)
         ins = np.flatnonzero((exist == 1) & (self._exist == 0)).astype(np.uint32)
         have_del = bool(np.any((exist == 0) & (self._exist == 1)))
         self._exist = exist
         st = (C.c_longlong * 10)()
         self._L.fm_update(self._h, exist.ctypes, ins.ctypes, C.c_longlong(len(ins)), C.c_int(int(have_del)), C.c_int(int(flags)), st)
-        keys = ("generations", "full_visits", "retire_visits", "changed", "reset", "activations", "suppressed", "iterations",
-                "evaluations", "candidates")
-        return dict(zip(keys, [int(x) for x in st]))
+        return dict(zip(self.KEYS, [int(x) for x in st]))
+
+    # --- x-slab sharding: mirrors ESDFMap.set_shard / shard_pack / shard_ingest / shard_relax on the model's own
+    # (unpadded) layout; a layer is gy*gz records and only model instances exchange them
+    def set_slab(self, tile_x_lo, tile_x_hi):
+        self._L.fm_set_slab(self._h, C.c_int(int(tile_x_lo)), C.c_int(int(tile_x_hi)))
+
+    def pack(self, x_first, nlayers):
+        out = np.empty(int(nlayers) * self.grid_size[1] * self.grid_size[2], np.uint32)
+        self._L.fm_pack(self._h, C.c_int(int(x_first)), C.c_int(int(nlayers)), out.ctypes)
+        return out
+
+    def halo_ingest(self, recv, x_first, nlayers, own_tile_x):
+        """Takes over the received ghost records that differ; returns how many did."""
+        recv = np.ascontiguousarray(recv, dtype=np.uint32)
+        assert len(recv) == int(nlayers) * self.grid_size[1] * self.grid_size[2]
+        return int(self._L.fm_halo_ingest(self._h, recv.ctypes, C.c_int(int(x_first)), C.c_int(int(nlayers)),
+                                          C.c_int(int(own_tile_x))))
+
+    def relax(self, flags=0):
+        """E3 over the tiles the ingests queued (shard_relax)."""
+        st = (C.c_longlong * 10)()
+        self._L.fm_relax(self._h, C.c_int(int(flags)), st)
+        return dict(zip(self.KEYS, [int(x) for x in st]))
 
     def export(self):
         cobs = np.empty((self.n, 3), np.int32)

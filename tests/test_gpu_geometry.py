@@ -9,7 +9,7 @@ is dyadic so that ceil(size / res) is exact."""
 import numpy as np
 import pytest
 
-from tests import frontierref, navref, scenes, segref
+from tests import fastbox, frontierref, navref, scenes, segref
 from tests.geometry import ORIGIN, RES, SHAPES, logit, random_voxels, shape_id, size_of, special_voxels, trilinear
 from tests.parity import compare, invariants
 
@@ -26,7 +26,7 @@ def same_counters(dev, ora):
 
 class Pair:
     """A device map and the reference driven with the same inputs; FAST maps also drive the CPU model from the device's
-    occupancy state (as tests/test_gpu_fast_model.py does) while the update box is the whole grid."""
+    occupancy state (as tests/test_gpu_fast_model.py does), under the device's update box and with its local-map resets."""
 
     def __init__(self, oracle_built, gs, mode, params=scenes.PARAMS_TOGGLE):
         import fiesta_b200
@@ -37,7 +37,8 @@ class Pair:
         for m in (self.dev, self.ora):
             m.SetParameters(*params)
         self.model = oracle_built.FastModel(gs, RES, logit(params[4])) if mode == "fast" else None
-        self.full_box = True
+        self.full = ((0, 0, 0), tuple(g - 1 for g in gs))
+        self.box = self.last_box = self.full           # min_vec_ .. max_vec_ and last_min_vec_ .. last_max_vec_
         self.updates = 0
         self.mirror = None                     # a Mirror, checked after every update when set
 
@@ -48,6 +49,20 @@ class Pair:
         a, b = self.both("SetOccupancyBatchVox", vox, occ)
         assert np.array_equal(a, b)
 
+    def set_box(self, lo, hi, new_vec=True):
+        self.both("SetUpdateRange", tuple(lo), tuple(hi), new_vec)
+        if new_vec:
+            self.last_box = self.box
+        self.box = fastbox.vox_box(ORIGIN, RES, size_of(self.gs), lo, hi)
+        if self.model is not None:
+            self.model.set_range(*self.box)
+
+    def original(self):
+        self.both("SetOriginalRange")
+        self.box = self.last_box = self.full
+        if self.model is not None:
+            self.model.set_range(*self.box)
+
     def update(self, tag, global_map=True):
         dev, ora = self.dev, self.ora
         assert same_counters(dev, ora), tag
@@ -55,10 +70,14 @@ class Pair:
         assert c == ora.CheckUpdate(), tag
         if not c:
             return False
+        reset = None
+        if self.model is not None and not global_map:
+            hit, tot = dev.export_counters()
+            reset = fastbox.reset_set(hit, tot, dev.export_occupancy(), self.last_box, self.gs, self.params)
         assert dev.UpdateOccupancy(global_map) == ora.UpdateOccupancy(global_map), tag
         st = None
-        if self.model is not None and self.full_box:
-            st = self.model.update(dev.export_distance(), dev.export_occupancy())
+        if self.model is not None:
+            st = self.model.update(dev.export_distance(), dev.export_occupancy(), 0, reset)
         dev.UpdateESDF(); ora.UpdateESDF()
         self.updates += 1
         self.check(tag, st)
@@ -75,7 +94,7 @@ class Pair:
             assert dev.stats()["expansions"] == ora.stats()["expansions"], tag
             return
         inv = invariants(dev, logit(self.params[4]))
-        if not self.full_box:                     # the wave stays inside the box: the 24-neighbour check does not apply
+        if self.box != self.full:                 # the wave stays inside the box: the 24-neighbour check does not apply
             inv.pop("closer_occupied_neighbour")
         assert not any(inv.values()), (tag, inv)
         if st is not None:
@@ -172,13 +191,12 @@ def box_phase(p, rng, tag):
     gs = p.gs
     lo, hi = np.asarray(ORIGIN), np.asarray(ORIGIN) + np.asarray(size_of(gs))
     mid = lo + (np.asarray(gs) // 2) * RES
-    p.full_box = False
     for k, (a, b) in enumerate([(lo, hi), (lo - 3.0, mid + 0.5 * RES), (mid - 0.25 * RES, hi + 7.0)]):
-        p.both("SetUpdateRange", tuple(a), tuple(b))
+        p.set_box(a, b)
         vox = np.concatenate([special_voxels(gs), random_voxels(rng, gs, 200)])
         p.events(vox, (rng.random(len(vox)) < 0.5).astype(np.uint8))
         p.update((tag, "box", k))
-    p.both("SetOriginalRange")
+    p.original()
 
 
 def local_map_loop(p, rng, tag):
@@ -190,13 +208,12 @@ def local_map_loop(p, rng, tag):
     p.events(allv[idx], np.ones(len(idx), np.uint8)); p.update((tag, "obstacles"))
     p.both("SetParameters", *scenes.PARAMS_DEFAULT)
     p.params = scenes.PARAMS_DEFAULT
-    p.full_box = False
     lo, size = np.asarray(ORIGIN), np.asarray(size_of(gs))
     seen_reset = 0
     for r in range(6):
         c = lo + size * (0.15 + 0.14 * r)
         half = size * 0.3
-        p.both("SetUpdateRange", tuple(c - half), tuple(c + half))
+        p.set_box(c - half, c + half)
         vox = random_voxels(rng, gs, 4000)
         p.events(vox, (rng.random(4000) < 0.4).astype(np.uint8))
         assert p.dev.UpdateOccupancy(False) == p.ora.UpdateOccupancy(False)
@@ -208,7 +225,7 @@ def local_map_loop(p, rng, tag):
         D, C = p.ora.export_distance(), p.ora.export_closest_obstacle()
         seen_reset += int(((D == 10000) & (C[:, 0] != -10000)).sum())       # FB_DINF records: infinity, obstacle kept
     assert seen_reset > 0
-    p.both("SetOriginalRange")
+    p.original()
 
 
 @pytest.mark.parametrize("mode", ["exact", "fast"])
