@@ -150,7 +150,8 @@ int fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t s) {
   for (int k = 0; k < 2; ++k) CK(X->E[k].alloc(P));
   X->dense_min = 16384u;
   if (const char *e = getenv("FIESTA_X_DENSE")) { long v = atol(e); if (v >= 0 && v <= (1 << 24)) X->dense_min = (unsigned)v; }
-  if (const char *e = getenv("FIESTA_X_ASYNC")) X->async = atol(e) != 0;
+  if (const char *e = getenv("FIESTA_X_ASYNC")) X->async = atol(e) != 0;                  // 0: no work queue anywhere
+  if (const char *e = getenv("FIESTA_X_SMALL_ASYNC")) X->small_async = atol(e) != 0;      // 1: SMALL generations from the queue
   X->small_max = FB_X_SMALL_DEFAULT;
   if (const char *e = getenv("FIESTA_X_SMALL")) { long v = atol(e); if (v >= 0 && v <= 65536) X->small_max = (unsigned)v; }
   CK(X->slotc.alloc(((size_t)X->small_max + 1) * 32));
@@ -327,10 +328,10 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
       if (cyc_per_us == 0) { int dev = 0, khz = 0; CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev)); cyc_per_us = khz / 1000.0; }
       CK(cudaMemcpy(hd, X->d_dbg, sizeof(hd), cudaMemcpyDeviceToHost));
       // phase categories of k_x_relax (14 and 15 are list-length counters, printed below)
-      static const char *cat[19] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top", "empty-barrier",
-                                    "reseed.rounds", "reseed.assemble", "", "", "async", "", "refresh"};
+      static const char *cat[20] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top", "empty-barrier",
+                                    "reseed.rounds", "reseed.assemble", "", "", "async", "", "refresh", "s.async"};
       fprintf(stderr, "[x] reseed rounds %u; phases (us, count):", st->reseed_rounds);
-      for (int c = 0; c < 19; ++c)
+      for (int c = 0; c < 20; ++c)
         if (*cat[c]) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[FB_XDBG_PHASE + 2 * c] / cyc_per_us, hd[FB_XDBG_PHASE + 2 * c + 1]);
       fprintf(stderr, "\n");
       fprintf(stderr, "[x] round work (summed longest CTA work time us / summed list length):");

@@ -65,6 +65,7 @@ struct FbExact {
   unsigned dense_min = 0;             // work lists longer than this are evaluated through refreshed summaries (one wave of warps)
   unsigned small_max = 0;             // generations up to this many entries run without summaries
   bool async = true;                  // short work lists resolved from a work queue instead of in rounds (FIESTA_X_ASYNC=0: rounds)
+  bool small_async = false;           // SMALL generations resolved from the queue, seeded with every element (FIESTA_X_SMALL_ASYNC=1)
   FbDevBuf<FbXCtl> d_ctl;
   FbHostBuf<FbXCtl> h_ctl;
   FbDevBuf<unsigned long long> d_dbg;

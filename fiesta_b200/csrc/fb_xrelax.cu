@@ -19,7 +19,8 @@
 //    summaries of their targets; long lists first refresh, then evaluate through the summaries.  Element i is right once all
 //    earlier ones are, so the fixpoint -- reached by a round without flips, which has only read final words -- is the
 //    sequential execution.  In BIG generations, once a list is short, the rest of the fixpoint runs without rounds from a
-//    work queue (x_async), followed by one summary refresh.
+//    work queue (x_async), followed by one summary refresh.  With FIESTA_X_SMALL_ASYNC=1, SMALL generations seed that
+//    queue with every element and run no rounds at all (slower on the measured workloads, DESIGN §6, so off by default).
 //  * Hand-over: element i owns slot k iff the final state of its k-th target carries the timestamp 32*i + k; the owned slots in
 //    timestamp order (per-element masks, exclusive scan over CTA-contiguous ranges) are the next generation; old words are
 //    retired by compare-and-swap (a generation-parity bit tells old from new).
@@ -222,6 +223,7 @@ struct XArgs {
   unsigned long long *dbg;  // optional per-generation trace {nE, rounds, ns} (FIESTA_DEBUG_X)
   unsigned div_pz_m, div_pz_s, div_gy_m, div_gy_s;   // n / d = umulhi(n, m) >> s for n < 2^31 (fb_div_make, fb_divmagic.h); m == 0: d == 1
   unsigned async_on;        // resolve short work lists from the work queue (x_async) instead of in rounds
+  unsigned small_async_on;  // SMALL generations: the whole fixpoint from the work queue, seeded with every element
 };
 // voxel index -> coordinates: two divisions by run-time constants, as multiply-high + shift
 __device__ __forceinline__ unsigned x_div(unsigned n, unsigned m, unsigned s) { return m ? (__umulhi(n, m) >> s) : n; }
@@ -533,10 +535,12 @@ __device__ __forceinline__ void x_q_abort(const XArgs &a) {
   atomicCAS(&a.ctl->err, 0u, 3u);
   atomicExch(&a.ctl->qdone, 1u);
 }
-// qtail += delta (one lane); sets qdone when the outstanding count reaches zero.  Returns the old push count.
-__device__ __forceinline__ unsigned x_q_count(const XArgs &a, unsigned long long delta) {
+// qtail += delta (one lane); sets qdone when the outstanding count reaches zero, and the CTA's copy with it, so that the
+// warp that ends the phase (often the only one left working) leaves at once instead of at its next poll of the global
+// flag.  Returns the old push count.
+__device__ __forceinline__ unsigned x_q_count(const XArgs &a, XShared &sh, unsigned long long delta) {
   const unsigned long long old = atomicAdd(&a.ctl->qtail, delta);
-  if ((unsigned)((old + delta) >> 32) == 0u) atomicExch(&a.ctl->qdone, 1u);
+  if ((unsigned)((old + delta) >> 32) == 0u) { atomicExch(&a.ctl->qdone, 1u); sh.qdone = 1u; }
   return (unsigned)old;
 }
 // (qdone cannot be set while the pusher's own item is outstanding, unless the phase was abandoned: then it leaves at once)
@@ -562,17 +566,18 @@ __device__ __forceinline__ void x_q_put(const XArgs &a, XShared &sh, uint32_t *r
   }
 }
 // One lane: the next element from the queue, or XNONE once the phase is over.  `h` keeps the reserved pop index between calls.
+template <bool DBG>
 __device__ __forceinline__ unsigned x_q_take(const XArgs &a, XShared &sh, uint32_t *ring, unsigned cap, unsigned &h) {
   if (h == XNONE) h = atomicAdd(&a.ctl->qhead, 1u);
   unsigned *slot = &ring[h % cap];
   const volatile unsigned *done = &sh.qdone;
-  const long long c0 = a.dbg ? clock64() : 0;
+  const long long c0 = DBG ? clock64() : 0;
   unsigned long long t0 = 0;
   unsigned ns = 32;
   for (unsigned it = 0;; ++it) {
     if (x_ld_relaxed(slot) & X_Q_FULL) {
       const unsigned v = atomicExch(slot, 0u);
-      if (v & X_Q_FULL) { h = XNONE; if (a.dbg) atomicAdd(&a.dbg[FB_XDBG_Q + 3], (unsigned long long)(clock64() - c0)); return v & ~X_Q_FULL; }
+      if (v & X_Q_FULL) { h = XNONE; if (DBG) atomicAdd(&a.dbg[FB_XDBG_Q + 3], (unsigned long long)(clock64() - c0)); return v & ~X_Q_FULL; }
     }
     if (*done) break;
     if ((it & 15u) == 15u) {                                   // the global flag is polled by few warps at a time
@@ -584,7 +589,7 @@ __device__ __forceinline__ unsigned x_q_take(const XArgs &a, XShared &sh, uint32
     __nanosleep(ns);
     ns = ns < 256u ? 2u * ns : 256u;
   }
-  if (a.dbg) atomicAdd(&a.dbg[FB_XDBG_Q + 3], (unsigned long long)(clock64() - c0));
+  if (DBG) atomicAdd(&a.dbg[FB_XDBG_Q + 3], (unsigned long long)(clock64() - c0));
   return XNONE;
 }
 // Marks the later elements among the first `nof` staged offsets of element i and pushes those that were IDLE (one warp,
@@ -609,14 +614,51 @@ __device__ __forceinline__ unsigned x_q_list(const XArgs &a, XShared &sh, const 
   const unsigned total = __shfl_sync(0xffffffffu, incl, 31);
   if (total == 0u) return 0u;
   unsigned base = 0;
-  if (lane == 0) base = x_q_count(a, (unsigned long long)total * 0x100000001ull);
+  if (lane == 0) base = x_q_count(a, sh, (unsigned long long)total * 0x100000001ull);
   base = __shfl_sync(0xffffffffu, base, 0) + incl - cnt;
 #pragma unroll
   for (int t = 0; t < 5; ++t) if ((pm >> t) & 1u) x_q_put(a, sh, ring, cap, base++, j[t]);
   return total;
 }
+// One element of an asynchronous phase, taken from the queue (RUNNING set here) or claimed by its owner (`claimed`: RUNNING
+// and fenced already): evaluated from its stage, its word stored on a flip (BIG: and recorded in F[fout]) and the later
+// elements it can touch listed; evaluated again while a lister marked it dirty meanwhile.
+template <bool BIG, bool DBG>
+__device__ __forceinline__ void x_q_run(const XArgs &a, XShared &sh, XNb &stg, unsigned lane, const uint32_t *E, unsigned nE, uint32_t *ring,
+                                        unsigned gen, unsigned A, unsigned fout, unsigned i, bool claimed) {
+  const uint32_t p = __ldcg(&E[i]);
+  int x, y, z; x_coords(a, p, x, y, z);
+  for (;; claimed = false) {
+    if (DBG && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 0], 1ull);
+    if (!claimed) {
+      if (lane == 0) atomicExch(&a.wstamp[i], A);              // RUNNING (from MARKED: queued, or dirty)
+      __syncwarp();
+      __threadfence();
+    }
+    x_stage(a, sh, stg, lane, x, y, z);
+    const unsigned long long old = stg.w[0], nw2 = x_eval_nb(a, sh, stg, lane, gen, i, x, y, z);
+    if (nw2 != old) {                                          // flip
+      if (lane == 0) {
+        a.MB[p] = nw2;
+        if (BIG) {
+          const unsigned f = atomicAdd(&a.ctl->nF[fout], 1u);
+          if (f < (unsigned)a.g.ptotal) a.F[fout][f] = i;
+        }
+      }
+      __syncwarp();
+      __threadfence();
+      const unsigned np = x_q_list(a, sh, stg, ring, nE, lane, i, (x_mb_kind(old) == X_PUSH || x_mb_kind(nw2) == X_PUSH) ? (unsigned)X_NOFF : 25u, A);
+      if (DBG && lane == 0 && np) atomicAdd(&a.dbg[FB_XDBG_Q + 2], (unsigned long long)np);
+    }
+    unsigned again = 0;
+    if (lane == 0) again = atomicCAS(&a.wstamp[i], A, A - 1u) != A ? 1u : 0u;   // IDLE, unless marked dirty meanwhile
+    if (!__shfl_sync(0xffffffffu, again, 0)) break;
+    if (DBG && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 1], 1ull);
+  }
+}
 // The asynchronous phase of one BIG generation (all warps of the grid): the nw elements of the work list `wl` seed the
 // queue, `ring` (nE slots) holds it; every flip is recorded in F[fout] for the summary refresh that follows.
+template <bool DBG>
 __device__ void x_async(const XArgs &a, XShared &sh, XNb &stg, unsigned lane, unsigned gwarp, unsigned gwarps, const uint32_t *E, unsigned nE,
                         const uint32_t *wl, unsigned nw, uint32_t *ring, unsigned gen, unsigned A, unsigned fout) {
   // seeds: this warp's chunks of 32, then its token
@@ -627,44 +669,54 @@ __device__ void x_async(const XArgs &a, XShared &sh, XNb &stg, unsigned lane, un
     const unsigned pm = __ballot_sync(0xffffffffu, push), cnt = (unsigned)__popc(pm);
     if (cnt == 0u) continue;
     unsigned base = 0;
-    if (lane == 0) base = x_q_count(a, (unsigned long long)cnt * 0x100000001ull);
+    if (lane == 0) base = x_q_count(a, sh, (unsigned long long)cnt * 0x100000001ull);
     base = __shfl_sync(0xffffffffu, base, 0);
     if (push) x_q_put(a, sh, ring, nE, base + (unsigned)__popc(pm & ((1u << lane) - 1u)), e);
-    if (a.dbg && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 2], (unsigned long long)cnt);
+    if (DBG && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 2], (unsigned long long)cnt);
   }
-  if (lane == 0) x_q_count(a, 0ull - (1ull << 32));
+  if (lane == 0) x_q_count(a, sh, 0ull - (1ull << 32));
   unsigned h = XNONE;
   for (;;) {
     unsigned i = 0;
-    if (lane == 0) i = x_q_take(a, sh, ring, nE, h);
+    if (lane == 0) i = x_q_take<DBG>(a, sh, ring, nE, h);
     i = __shfl_sync(0xffffffffu, i, 0);
     if (i == XNONE) break;
-    const uint32_t p = __ldcg(&E[i]);
-    int x, y, z; x_coords(a, p, x, y, z);
-    for (;;) {
-      if (a.dbg && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 0], 1ull);
-      if (lane == 0) atomicExch(&a.wstamp[i], A);              // RUNNING (from MARKED: queued, or dirty)
-      __syncwarp();
-      __threadfence();
-      x_stage(a, sh, stg, lane, x, y, z);
-      const unsigned long long old = stg.w[0], nw2 = x_eval_nb(a, sh, stg, lane, gen, i, x, y, z);
-      if (nw2 != old) {                                        // flip
-        if (lane == 0) {
-          a.MB[p] = nw2;
-          const unsigned f = atomicAdd(&a.ctl->nF[fout], 1u);
-          if (f < (unsigned)a.g.ptotal) a.F[fout][f] = i;
-        }
-        __syncwarp();
-        __threadfence();
-        const unsigned np = x_q_list(a, sh, stg, ring, nE, lane, i, (x_mb_kind(old) == X_PUSH || x_mb_kind(nw2) == X_PUSH) ? (unsigned)X_NOFF : 25u, A);
-        if (a.dbg && lane == 0 && np) atomicAdd(&a.dbg[FB_XDBG_Q + 2], (unsigned long long)np);
-      }
-      unsigned again = 0;
-      if (lane == 0) again = atomicCAS(&a.wstamp[i], A, A - 1u) != A ? 1u : 0u;   // IDLE, unless marked dirty meanwhile
-      if (!__shfl_sync(0xffffffffu, again, 0)) break;
-      if (a.dbg && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 1], 1ull);
+    x_q_run<true, DBG>(a, sh, stg, lane, E, nE, ring, gen, A, fout, i, false);
+    if (lane == 0) x_q_count(a, sh, 0ull - (1ull << 32));
+  }
+}
+// The asynchronous phase of one SMALL generation (FIESTA_X_SMALL_ASYNC=1): its whole behaviour fixpoint, seeded with every
+// element; no summaries, so nothing is recorded for a refresh (the commit re-stages the final words).  A seed's first
+// evaluation is round 1's, so seeds do not go through the ring: warp w takes the elements w, w + nwk, ... itself, 32 at a
+// time, IDLE -> RUNNING with one atomicMax each and one fence for the 32 (an element a lister marked first is already
+// queued and skipped here), and evaluates them in order under its seeding token, as if it had pushed and popped them.
+// Only the first nwk = min(warps, nE) warps take part (at most nE elements are ever queued): warp 0 drops the other
+// warps' tokens at once, and those warps leave, so a short generation does not pay for every warp's token and pop.
+template <bool DBG>
+__device__ void x_async_small(const XArgs &a, XShared &sh, XNb &stg, unsigned lane, unsigned gwarp, unsigned gwarps, const uint32_t *E, unsigned nE,
+                              uint32_t *ring, unsigned gen, unsigned A) {
+  const unsigned nwk = min(gwarps, nE);
+  if (gwarp >= nwk) return;
+  if (gwarp == 0u && lane == 0 && nwk < gwarps) x_q_count(a, sh, 0ull - ((unsigned long long)(gwarps - nwk) << 32));   // warp 0's own token stays
+  for (unsigned s0 = gwarp; s0 < nE; s0 += 32u * nwk) {
+    const unsigned e = s0 + lane * nwk;
+    unsigned om = __ballot_sync(0xffffffffu, e < nE && atomicMax(&a.wstamp[e], A) < A);   // IDLE -> RUNNING, else queued by a lister
+    __threadfence();                                           // RUNNING before any of their stages
+    while (om) {
+      const unsigned i = s0 + (unsigned)(__ffs(om) - 1) * nwk;
+      om &= om - 1u;
+      x_q_run<false, DBG>(a, sh, stg, lane, E, nE, ring, gen, A, 0u, i, true);
     }
-    if (lane == 0) x_q_count(a, 0ull - (1ull << 32));
+  }
+  if (lane == 0) x_q_count(a, sh, 0ull - (1ull << 32));
+  unsigned h = XNONE;
+  for (;;) {
+    unsigned i = 0;
+    if (lane == 0) i = x_q_take<DBG>(a, sh, ring, nE, h);
+    i = __shfl_sync(0xffffffffu, i, 0);
+    if (i == XNONE) break;
+    x_q_run<false, DBG>(a, sh, stg, lane, E, nE, ring, gen, A, 0u, i, false);
+    if (lane == 0) x_q_count(a, sh, 0ull - (1ull << 32));
   }
 }
 
@@ -692,6 +744,9 @@ __device__ __forceinline__ uint32_t x_reseed_eval(const XArgs &a, unsigned i, in
 
 extern __shared__ __align__(16) unsigned char x_dyn_smem[];
 
+// DBG: the FIESTA_DEBUG_X trace (a.dbg != nullptr).  The production instance carries none of its clocks and counters, which
+// would otherwise stay live across the generation loop and the queue phases (spills at the 64-register limit).
+template <bool DBG>
 __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
   __shared__ XShared sh;
   const FbGeom &g = a.g;
@@ -725,13 +780,13 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
   unsigned long long tclock = ctl->tclock;
   unsigned generations = 0, rounds_total = 0, dense_total = 0;
   unsigned long long changed_total = 0;
-  if (a.dbg) {                                                 // cost of an empty grid barrier
+  if (DBG) {                                                 // cost of an empty grid barrier
     const long long t0 = clock64();
     for (int q = 0; q < 32; ++q) x_gsync(&ctl->bar, bar_target);
     if (gtid == 0) a.dbg[XDBG_PHASE + 2 * 11] = (unsigned long long)(clock64() - t0) / 32ull;
   }
-  long long t_ph = a.dbg ? clock64() : 0;
-#define X_LAP(cat) do { if (a.dbg && gtid == 0) { const long long t_now = clock64(); a.dbg[XDBG_PHASE + 2 * (cat)] += (unsigned long long)(t_now - t_ph); a.dbg[XDBG_PHASE + 2 * (cat) + 1] += 1ull; t_ph = t_now; } } while (0)
+  long long t_ph = DBG ? clock64() : 0;
+#define X_LAP(cat) do { if (DBG && gtid == 0) { const long long t_now = clock64(); a.dbg[XDBG_PHASE + 2 * (cat)] += (unsigned long long)(t_now - t_ph); a.dbg[XDBG_PHASE + 2 * (cat) + 1] += 1ull; t_ph = t_now; } } while (0)
   // ---- E2, second half: re-seed the dependants of the deleted obstacles (fixpoint over work lists, in place), then append
   // the re-seeded ones, in list-walk order, to the insert seeds in E[0] (:301-334).
   unsigned reseed_rounds = 0;
@@ -741,7 +796,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       const unsigned nw = r == 1u ? a.ndep : __ldcg(&ctl->nW[in]);
       if (gtid == 0) ctl->nW[zz] = 0;
       if (r > 1u && nw == 0u) break;
-      if (a.dbg && gtid == 0) a.dbg[XDBG_PHASE + 2 * 15] += nw;
+      if (DBG && gtid == 0) a.dbg[XDBG_PHASE + 2 * 15] += nw;
       ++reseed_rounds; ++wclock;
       if (nw <= 2u * gwarps) {
         // short list: one WARP per dependant, lane k = neighbour k -- the 24 look-ups (position in deps, code, Exist bit) run side
@@ -877,7 +932,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
   x_gsync(&ctl->bar, bar_target);
 
   while (nE) {
-    const long long t_gen = a.dbg ? clock64() : 0;
+    const long long t_gen = DBG ? clock64() : 0;
     X_LAP(10);
     ++generations;
     const uint32_t *E = a.E[cur];
@@ -897,21 +952,24 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       if (gtid == 0) { ctl->nW[zz] = 0; ctl->nF[zz] = 0; }
       if (r > 1u && nw == 0u && nf == 0u) break;
       if (r > X_MAX_ROUNDS) { if (gtid == 0) ctl->err = 2u; break; }   // cannot happen (element i is final after i+1 rounds at the latest); never spin forever on the GPU
-      if (a.dbg && gtid == 0) { a.dbg[XDBG_PHASE + 2 * 14] += nw; a.dbg[XDBG_PHASE + 2 * 14 + 1] += nf; }
-      if (a.async_on && big && r > 1u && nw <= a.dense_min) {
-        // the rest of the fixpoint from the work queue, with W[out] as its ring; then the summaries of the targets of every
-        // flip since the last refresh: last round's (F[in]) and the queue's (F[out]).  (SMALL generations keep their rounds:
-        // their lists are a few entries long and the queue's start and end cost more than the barriers it saves, DESIGN §6.)  A summary's offer timestamps
+      if (DBG && gtid == 0) { a.dbg[XDBG_PHASE + 2 * 14] += nw; a.dbg[XDBG_PHASE + 2 * 14 + 1] += nf; }
+      if (a.async_on && (big ? r > 1u && nw <= a.dense_min : r == 1u && a.small_async_on)) {
+        // BIG: the rest of the fixpoint from the work queue, with W[out] as its ring; then the summaries of the targets of
+        // every flip since the last refresh: last round's (F[in]) and the queue's (F[out]).  A summary's offer timestamps
         // 32*i+k are fixed, so the refresh rule needs only the final word and the summary's first / best, however often the
-        // element flipped in between.
+        // element flipped in between.  SMALL: the whole fixpoint from the queue, seeded with every element instead of round
+        // 1 (the words start as "everybody pushes its snapshot code", as for round 1); no summaries, so no refresh: the
+        // commit follows the barrier, and the queue's reset below happens in the commit phase, behind the commit's barrier.
         ++rounds; wclock += 3u;
         const unsigned A = wclock - 1u;                        // RUNNING; MARKED = wclock; the stamps of the next rounds are above
-        x_async(a, sh, stg, lane, gwarp, gwarps, E, nE, a.W[in], nw, a.W[out], gen, A, out);
+        if (big) x_async<DBG>(a, sh, stg, lane, gwarp, gwarps, E, nE, a.W[in], nw, a.W[out], gen, A, out);
+        else x_async_small<DBG>(a, sh, stg, lane, gwarp, gwarps, E, nE, a.W[out], gen, A);
         x_gsync(&ctl->bar, bar_target);
-        X_LAP(16);
+        X_LAP(big ? 16 : 19);
         if (tid == 0) sh.qdone = 0u;
         if (gtid == 0) { ctl->qtail = (unsigned long long)gwarps << 32; ctl->qhead = 0u; ctl->qdone = 0u; }
         if (__ldcg(&ctl->err)) { aborted = true; break; }
+        if (!big) break;
         const unsigned nfa = __ldcg(&ctl->nF[out]);
         if (nfa > (unsigned)g.ptotal) {                        // flip list overflowed: summarise every target again
           ++sclock;
@@ -948,7 +1006,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       const bool use_sum = big && (r == 1u || dense);
       const unsigned nref = (big && !dense) ? nf : 0u;
       const uint32_t *wl = a.W[in];
-      const long long t_w0 = a.dbg ? clock64() : 0;
+      const long long t_w0 = DBG ? clock64() : 0;
       for (unsigned q = gwarp; q < nw + nref; q += gwarps) {
         if (q >= nw) {                                         // summaries of the targets of an element that flipped last round
           const unsigned i = __ldcg(&a.F[in][q - nw]);
@@ -985,10 +1043,10 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
         // element's offer to its own voxel, which only its 24 neighbours read (the table starts with 0 and dirs_)
         x_list_affected(a, sh, lane, i, x, y, z, (x_mb_kind(old) == X_PUSH || x_mb_kind(nb) == X_PUSH) ? (unsigned)X_NOFF : 25u, wclock, out);
       }
-      if (a.dbg) { __syncthreads(); if (tid == 0) atomicMax(&a.dbg[XDBG_WMAX + ((rounds_total + rounds) & 4095u)], (unsigned long long)(clock64() - t_w0)); }
+      if (DBG) { __syncthreads(); if (tid == 0) atomicMax(&a.dbg[XDBG_WMAX + ((rounds_total + rounds) & 4095u)], (unsigned long long)(clock64() - t_w0)); }
       x_gsync(&ctl->bar, bar_target);
       X_LAP(big ? (r == 1u ? 1 : (dense ? 3 : 2)) : (r == 1u ? 6 : 7));
-      if (a.dbg && gtid == 0) {
+      if (DBG && gtid == 0) {
         if (generations <= 2u && rounds <= 512u) a.dbg[XDBG_ROUNDS + (generations - 1u) * 512u + (rounds - 1u)] = nw;
         // the round's longest CTA work time and list length, summed per category: the rest of the category's time is barrier
         // and waiting for the slowest CTA
@@ -1085,7 +1143,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       }
       run += ctot;
     }
-    if (a.dbg && gtid == 0 && generations <= FB_XDBG_GENS) { a.dbg[3 * (generations - 1u)] = nE; a.dbg[3 * (generations - 1u) + 1] = rounds; a.dbg[3 * (generations - 1u) + 2] = (unsigned long long)(clock64() - t_gen); }
+    if (DBG && gtid == 0 && generations <= FB_XDBG_GENS) { a.dbg[3 * (generations - 1u)] = nE; a.dbg[3 * (generations - 1u) + 1] = rounds; a.dbg[3 * (generations - 1u) + 2] = (unsigned long long)(clock64() - t_gen); }
     tclock += (unsigned long long)nE * 32ull + 1ull;
     changed_total += n2;
     if (n2 >= (1u << 27)) { if (gtid == 0) ctl->err = 1u; break; }
@@ -1126,7 +1184,8 @@ cudaError_t fb_xrelax_init() {
 
 int fb_xrelax_blocks(int device) {
   int per_sm = 0, sms = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_x_relax, XT, sizeof(XNb) * XW) != cudaSuccess || per_sm < 1) return -1;
+  for (const void *k : {(const void *)k_x_relax<false>, (const void *)k_x_relax<true>})
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, XT, sizeof(XNb) * XW) != cudaSuccess || per_sm < 1) return -1;
   if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return -1;
   return sms;                                                  // one CTA per SM: the barrier is cheapest with few arrivals
 }
@@ -1145,6 +1204,7 @@ cudaError_t fb_xrelax_launch(FbExact *X, const FbGeom &g, uint32_t *cobs, unsign
   for (int k = 0; k < 3; ++k) { a.W[k] = X->W[k]; a.F[k] = X->F[k]; }
   a.wstamp = X->wstamp; a.slotc = X->slotc; a.ctl = X->d_ctl; a.nE0 = nE0; a.small_max = X->small_max; a.dense_min = X->dense_min; a.dbg = dbg;
   a.async_on = X->async ? 1u : 0u;
+  a.small_async_on = X->small_async ? 1u : 0u;
   void *args[] = {(void *)&a};
-  return cudaLaunchCooperativeKernel((void *)k_x_relax, dim3(X->relax_blocks), dim3(XT), args, sizeof(XNb) * XW, s);
+  return cudaLaunchCooperativeKernel(dbg ? (void *)k_x_relax<true> : (void *)k_x_relax<false>, dim3(X->relax_blocks), dim3(XT), args, sizeof(XNb) * XW, s);
 }

@@ -4,9 +4,14 @@
 //   gcc -O2 -ffp-contract=off -o /tmp/exact_async_model scripts/exact_async_model.c -lm
 //   /tmp/exact_async_model WORKERS SMALL_ASYNC G obs rounds nops seed [small [local [dense_min]]]
 // (the arguments after SMALL_ASYNC are exact_model.c's).  WORKERS = 0 runs exact_model.c's round schedule unchanged.
+// Built with -DNO_DIRTY_RULE, a running element that gets marked is not evaluated again (a mutation the replays must catch).
 //
-// In BIG generations the first work list of at most dense_min entries after round 1 (SMALL generations, with
-// SMALL_ASYNC = 1: the list after round 1) is not evaluated in rounds: it seeds a queue.  Each element is IDLE, PENDING
+// In BIG generations the first work list of at most dense_min entries after round 1 is not evaluated in rounds: it seeds a
+// queue.  SMALL generations: SMALL_ASYNC = 0 keeps their rounds, 1 seeds the queue with the list after round 1, 2 (what
+// k_x_relax does with FIESTA_X_SMALL_ASYNC=1) seeds it with every element of the generation instead of round 1: there,
+// worker w of nwk = min(WORKERS drawn, nE) owns the elements w, w + nwk, ...; it claims up to CLAIM of them at a time,
+// IDLE -> RUNNING (an element a lister already queued is skipped), evaluates them in order, and pops from the queue once
+// its own are done.  Each element is IDLE, PENDING
 // (queued), RUNNING or DIRTY (running, and an input flipped since it was marked running).  WORKERS simulated workers take
 // steps, one at a time, chosen at random:
 //   pop    take a random queued element, PENDING -> RUNNING;
@@ -35,12 +40,15 @@ static int WORKERS = 8, SMALL_ASYNC = 0;
 static long a_phases = 0, a_seeds = 0, a_evals = 0, a_dirty = 0, a_maxchain = 0, a_refreshed = 0;
 enum { A_IDLE = 0, A_PEND, A_RUN, A_DIRTY };
 static unsigned char *astate; static u32 *adepth; static u32 *bag; static long nbag;
-typedef struct { int step; u32 i, depth; u64 nb, old; } worker_t;
+typedef struct { int step; u32 i, depth; u64 nb, old; long next; int ncl, pcl; u32 cl[32]; } worker_t;
 #define MAXW 64
+#define CLAIM 4
 
 static void a_mark(u32 j) {
   if (astate[j] == A_IDLE) { astate[j] = A_PEND; bag[nbag++] = j; }
+#ifndef NO_DIRTY_RULE
   else if (astate[j] == A_RUN) astate[j] = A_DIRTY;
+#endif
 }
 // depth of an evaluation of element i from the current words: one more than the deepest earlier element it reads
 static u32 a_depth(u32 i) {
@@ -52,22 +60,34 @@ static u32 a_depth(u32 i) {
   }
   return d + 1;
 }
-// the rest of a generation's fixpoint from the nw elements of wl; BIG generations record every flip in F[fout]
+// the rest of a generation's fixpoint from the nw elements of wl (wl == NULL: the whole generation, owned by the workers);
+// BIG generations record every flip in F[fout]
 static void async_phase(u32 *wl, long nw, int big, int fout) {
   a_phases++; a_seeds += nw;
   memset(astate, 0, (size_t)nE); memset(adepth, 0, 4 * (size_t)nE); nbag = 0;
-  for (long q = 0; q < nw; q++) a_mark(wl[q]);
+  if (wl) for (long q = 0; q < nw; q++) a_mark(wl[q]);
   int nwk = 1 + rand() % WORKERS; worker_t wk[MAXW];
-  for (int k = 0; k < nwk; k++) wk[k].step = 0;
+  if (!wl && nwk > nw) nwk = (int)nw;
+  for (int k = 0; k < nwk; k++) { wk[k].step = 0; wk[k].next = wl ? nw : k; wk[k].ncl = wk[k].pcl = 0; }
   for (;;) {
     int en[MAXW], ne = 0;
-    for (int k = 0; k < nwk; k++) if (wk[k].step != 0 || nbag > 0) en[ne++] = k;
+    for (int k = 0; k < nwk; k++) if (wk[k].step != 0 || nbag > 0 || wk[k].pcl < wk[k].ncl || wk[k].next < nw) en[ne++] = k;
     if (!ne) break;                                            // queue empty and every worker waiting: quiescence
     worker_t *w = &wk[en[rand() % ne]];
     for (int t = 0; t < 8 && w->step == 2; t++) w = &wk[en[rand() % ne]];   // stores lag behind: more reads of stale words
     long p;
     switch (w->step) {
-      case 0: { long q = rand() % nbag; w->i = bag[q]; bag[q] = bag[--nbag]; astate[w->i] = A_RUN; w->step = 1; break; }
+      case 0:
+        if (w->pcl < w->ncl) { w->i = w->cl[w->pcl++]; w->step = 1; break; }            // next claimed own seed (RUNNING)
+        if (w->next < nw) {                                                             // claim own seeds: IDLE -> RUNNING
+          w->ncl = w->pcl = 0;
+          for (int c = 0; c < CLAIM && w->next < nw; c++, w->next += nwk)
+            if (astate[w->next] == A_IDLE) { astate[w->next] = A_RUN; w->cl[w->ncl++] = (u32)w->next; }
+          break;
+        }
+        if (nbag == 0) break;                                                           // waits for the queue
+        { long q = rand() % nbag; w->i = bag[q]; bag[q] = bag[--nbag]; astate[w->i] = A_RUN; w->step = 1; }
+        break;
       case 1: w->nb = eval(w->i, 0); w->depth = a_depth(w->i); a_evals++; totevals++; w->step = 2; break;
       case 2:
         p = E[cur][w->i]; w->old = MB[p];
@@ -107,8 +127,8 @@ static void relax_async(void) {
       long nf = (big && r > 1) ? nF[in] : 0;
       if (r > 1 && nw == 0 && nf == 0) break;
       rounds++;
-      if (r > 1 && (big ? nw <= DENSE_MIN : SMALL_ASYNC)) {
-        async_phase(wl, nw, big, out);
+      if (big ? r > 1 && nw <= DENSE_MIN : SMALL_ASYNC == 2 ? r == 1 : r > 1 && SMALL_ASYNC) {
+        async_phase(r == 1 ? NULL : wl, nw, big, out);
         if (big) {                                             // one refresh of every flip since the last one, in random order
           long nfa = nF[out];
           if (nfa > N) { sclock++; for (long i = 0; i < nE; i++) claim_summaries(i); }

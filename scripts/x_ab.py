@@ -1,6 +1,7 @@
-"""A/B of k_x_relax's two schedules of the short work lists: rounds (FIESTA_X_ASYNC=0) against the work queue (=1).
+"""A/B of two schedules of k_x_relax: a setting off (=0) against on (=1), by default FIESTA_X_ASYNC (rounds against the work
+queue for the short work lists); --var FIESTA_X_SMALL_ASYNC compares SMALL generations in rounds against the queue.
 
-    python scripts/x_ab.py --out DIR [--workload lidar512 ...] [--runs 3] [--steps 20] [--warmup 3] [--late-window 40]
+    python scripts/x_ab.py --out DIR [--var FIESTA_X_ASYNC] [--workload lidar512 ...] [--runs 3] [--steps 20] [--warmup 3] [--late-window 40]
 
 For every workload, runs `bench.py --no-cpu-baseline --other-frames 0 --no-host-mirror` alternately with each setting,
 `--runs` times per arm, in this one process tree (so both arms see the same card and the same neighbours).  The first run
@@ -36,11 +37,11 @@ def run(wl, arm, args, dump):
            "--workload", wl, "--no-cpu-baseline", "--other-frames", "0", "--no-host-mirror", "--late-window", str(args.late_window)]
     if dump:
         cmd += ["--dump-outputs", dump]
-    p = subprocess.run(cmd, env=dict(os.environ, FIESTA_X_ASYNC=arm), capture_output=True, text=True, cwd=ROOT)
+    p = subprocess.run(cmd, env=dict(os.environ, **{args.var: arm}), capture_output=True, text=True, cwd=ROOT)
     lines = [l for l in p.stdout.splitlines() if l.startswith("{")]
     if p.returncode or not lines:
         sys.stderr.write(p.stderr[-4000:])
-        raise SystemExit("bench.py failed (%s, FIESTA_X_ASYNC=%s): exit %d" % (wl, arm, p.returncode))
+        raise SystemExit("bench.py failed (%s, %s=%s): exit %d" % (wl, args.var, arm, p.returncode))
     return json.loads(lines[-1])
 
 
@@ -55,6 +56,7 @@ def same_arrays(d0, d1):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True)
+    ap.add_argument("--var", default="FIESTA_X_ASYNC", help="the setting the two arms differ in (0 / 1)")
     ap.add_argument("--workload", action="append")
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--steps", type=int, default=20)
@@ -71,19 +73,19 @@ def main():
             for arm in ("0", "1"):
                 dump = os.path.join(tmp, "dump_%s_async%s" % (wl, arm)) if k == 0 else None
                 line = run(wl, arm, args, dump)
-                line["FIESTA_X_ASYNC"] = arm
+                line[args.var] = arm
                 log.write(json.dumps(line) + "\n"); log.flush()
                 lw = line.get("late_window") or {}
                 res[arm].append((line["ms_per_step"], lw.get("ms_per_step"), line["expansions_equal_reference"], lw.get("expansions_equal_reference")))
-                print("%s run %d FIESTA_X_ASYNC=%s: %.3f ms/frame, late_window %s ms/frame, expansions_equal_reference %s / %s, clocks %s" %
-                      (wl, k, arm, line["ms_per_step"], "%.3f" % lw["ms_per_step"] if lw else "-", line["expansions_equal_reference"],
+                print("%s run %d %s=%s: %.3f ms/frame, late_window %s ms/frame, expansions_equal_reference %s / %s, clocks %s" %
+                      (wl, k, args.var, arm, line["ms_per_step"], "%.3f" % lw["ms_per_step"] if lw else "-", line["expansions_equal_reference"],
                        lw.get("expansions_equal_reference"), json.dumps(line.get("clocks"))), flush=True)
         eq, diff = same_arrays(os.path.join(tmp, "dump_%s_async0" % wl), os.path.join(tmp, "dump_%s_async1" % wl))
         for arm in ("0", "1"):
             ms = [r[0] for r in res[arm]]
             late = [r[1] for r in res[arm] if r[1] is not None]
-            print("%s FIESTA_X_ASYNC=%s: ms/frame min %.3f max %.3f; late_window min %s max %s; expansions equal %s" %
-                  (wl, arm, min(ms), max(ms), "%.3f" % min(late) if late else "-", "%.3f" % max(late) if late else "-",
+            print("%s %s=%s: ms/frame min %.3f max %.3f; late_window min %s max %s; expansions equal %s" %
+                  (wl, args.var, arm, min(ms), max(ms), "%.3f" % min(late) if late else "-", "%.3f" % max(late) if late else "-",
                    all(r[2] is not False and r[3] is not False for r in res[arm])), flush=True)
         print("%s dumped arrays bit-identical between the arms: %s%s" % (wl, eq, "" if eq else " (differ: %s)" % diff), flush=True)
     shutil.rmtree(tmp, ignore_errors=True)

@@ -9,8 +9,12 @@ entries.  It also prints, per frame, the (nE, rounds) list of every generation. 
 are fixed by the sequential result; rounds and list lengths vary from run to run (a round reads words flipped in the same
 round).  For the evaluation-round categories it also splits the time into the summed longest CTA work time of every round
 and the rest (grid barrier plus waiting for the slowest CTA), with a log2 histogram of the list lengths of the short-list
-rounds, and it sums the counters of the asynchronous schedule (FIESTA_X_ASYNC).  The card, its power limit and the SM clock
-are printed first.  The output is plain text, one item per line, so two runs can be diffed.  Needs a GPU.
+rounds, and it sums the counters of the asynchronous schedule (FIESTA_X_ASYNC; the queue of BIG generations is phase
+"async", the whole-generation queue of SMALL generations "s.async", FIESTA_X_SMALL_ASYNC).  SMALL generations (at most
+FIESTA_X_SMALL entries, default 32768) are summarised over the timed frames by log2 size bucket: count, rounds (a queue
+phase counts as one) and time per generation.  The card, its power limit and the SM clock are printed first.  The output is
+plain text, one item per line, so two runs can be diffed.  Needs a GPU, except with --from-trace FILE, which reads the
+library's stderr trace of an earlier child run (python scripts/xphase.py --child ... 2> FILE with FIESTA_DEBUG_X=1).
 """
 import argparse
 import os
@@ -20,7 +24,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PHASES = ["S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
-          "empty-barrier", "reseed.rounds", "reseed.assemble", "async", "refresh"]
+          "empty-barrier", "reseed.rounds", "reseed.assemble", "async", "refresh", "s.async"]
 ROUND_CATS = ["round1", "rounds", "dense", "s.round1", "s.rounds"]
 
 
@@ -67,18 +71,25 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--out", help="also write the report to this file")
+    ap.add_argument("--from-trace", help="summarise this saved trace instead of running the frames")
     ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.child:
         child(args.workload, args.warmup + args.steps)
         return
-    env = dict(os.environ, FIESTA_DEBUG_X="1")
-    cmd = [sys.executable, os.path.abspath(__file__), "--child", "--workload", args.workload, "--warmup", str(args.warmup), "--steps", str(args.steps)]
-    p = subprocess.run(cmd, env=env, stdout=subprocess.DEVNULL, stderr=subprocess.PIPE, text=True)
-    if p.returncode:
-        sys.stderr.write(p.stderr[-4000:])
-        raise SystemExit(p.returncode)
+    if args.from_trace:
+        trace = open(args.from_trace).read()
+    else:
+        env = dict(os.environ, FIESTA_DEBUG_X="1")
+        cmd = [sys.executable, os.path.abspath(__file__), "--child", "--workload", args.workload, "--warmup", str(args.warmup), "--steps", str(args.steps)]
+        p = subprocess.run(cmd, env=env, stdout=subprocess.DEVNULL, stderr=subprocess.PIPE, text=True)
+        if p.returncode:
+            sys.stderr.write(p.stderr[-4000:])
+            raise SystemExit(p.returncode)
+        trace = p.stderr
     lo, hi = args.warmup, args.warmup + args.steps
+    small_max = int(os.environ.get("FIESTA_X_SMALL", "32768"))
+    small = {}                                                 # log2 bucket of nE -> [generations, rounds, us]
     us = {k: 0.0 for k in PHASES}
     tot = dict(rounds=0, evaluated=0, refreshed=0, reseeded=0, reseed_rounds=0, generations=0, expansions=0)
     work = {k: [0.0, 0] for k in ROUND_CATS}
@@ -86,7 +97,7 @@ def main():
     aq = dict(evaluations=0, dirty=0, pushes=0, spin_us=0.0)
     gens = {}
     f = -1
-    for line in p.stderr.splitlines():
+    for line in trace.splitlines():
         if line.startswith("[frame] "):
             f = int(line.split()[1]); gens[f] = []
             continue
@@ -118,7 +129,13 @@ def main():
             mm = re.match(r"\[x\] gens (\d+) rounds (\d+)", line)
             tot["generations"] += int(mm.group(1)); tot["rounds"] += int(mm.group(2))
             gens[f] = [tuple(int(v) for v in t.split("/")[:2]) for t in line.split("|", 1)[1].split()]
-    out = ["card: " + card(), "FIESTA_X_ASYNC=%s" % os.environ.get("FIESTA_X_ASYNC", "(default)"),
+            for t in line.split("|", 1)[1].split():
+                n, r, t_us = t.split("/")
+                if int(n) <= small_max:
+                    b = small.setdefault(int(n).bit_length(), [0, 0, 0.0])
+                    b[0] += 1; b[1] += int(r); b[2] += float(t_us[:-2])
+    out = ["card: " + card() if not args.from_trace else "trace: " + args.from_trace,
+           "FIESTA_X_ASYNC=%s FIESTA_X_SMALL_ASYNC=%s" % (os.environ.get("FIESTA_X_ASYNC", "(default)"), os.environ.get("FIESTA_X_SMALL_ASYNC", "(default)")),
            "workload %s, frames %d-%d, phase totals of k_x_relax (ms):" % (args.workload, lo, hi - 1)]
     for k in PHASES:
         if k != "empty-barrier":
@@ -135,6 +152,12 @@ def main():
         out.append("list lengths of %s, rounds per log2 bucket [2^(b-1), 2^b): %s" % (name, " ".join("%d:%d" % kv for kv in sorted(h.items()))))
     out.append("async: evaluations %d dirty re-runs %d pushes %d spin %.2f ms (summed over warps)" %
                (aq["evaluations"], aq["dirty"], aq["pushes"], aq["spin_us"] / 1000.0))
+    out.append("SMALL generations (nE <= %d) per log2 bucket of nE [2^(b-1), 2^b): generations, rounds per generation, us per generation" % small_max)
+    for b in sorted(small):
+        g, r, t = small[b]
+        out.append("  b %2d: %6d gens %6.2f rounds %8.1f us" % (b, g, r / g, t / g))
+    g, r, t = (sum(v[k] for v in small.values()) for k in range(3))
+    out.append("  all : %6d gens %6.2f rounds %8.1f us (%.2f ms)" % (g, r / max(1, g), t / max(1, g), t / 1000.0))
     for k in ("generations", "rounds", "evaluated", "refreshed", "reseed_rounds", "reseeded", "expansions"):
         out.append("total %s %d" % (k, tot[k]))
     for fr in sorted(gens):
