@@ -47,6 +47,12 @@ class NavStats(C.Structure):
         ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
 
 
+class NavUpdateStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("box_voxels", "became_blocked", "became_free", "withdrawn", "goals_placed", "goals_new",
+                                         "seed_tiles", "withdraw_generations", "generations", "tile_visits", "blocked", "reached")] + [
+        ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
+
+
 class NavMatrixStats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("sources_placed", "targets_placed", "passes", "generations", "tile_visits",
                                          "sources_retired_early")] + [("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
@@ -100,7 +106,7 @@ SYMBOLS = [
     "fiesta_check_segments", "fiesta_check_segments_device", "fiesta_get_distance_batch_device",
     "fiesta_get_dist_grad_trilinear_batch_device", "fiesta_host_mirror_check_segments",
     "fiesta_nav_create", "fiesta_nav_destroy", "fiesta_nav_compute", "fiesta_nav_export", "fiesta_nav_paths",
-    "fiesta_nav_matrix",
+    "fiesta_nav_matrix", "fiesta_nav_update",
     "fiesta_frontiers_create", "fiesta_frontiers_destroy", "fiesta_frontiers_compute", "fiesta_frontiers_clusters",
     "fiesta_frontiers_voxels", "fiesta_frontiers_export", "fiesta_frontiers_score_viewpoints",
     "fiesta_inflate_boxes", "fiesta_corridors",
@@ -166,6 +172,7 @@ def load_library():
         L.fiesta_nav_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_int, C.c_void_p]
         L.fiesta_nav_export.argtypes = [C.c_void_p, C.c_void_p]
         L.fiesta_nav_paths.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 4
+        L.fiesta_nav_update.argtypes = [C.c_void_p, C.c_void_p]
         L.fiesta_nav_matrix.argtypes = [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_int64, C.c_double, C.c_int] + [C.c_void_p] * 4
         L.fiesta_frontiers_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
         L.fiesta_frontiers_destroy.argtypes = [C.c_void_p]
@@ -331,6 +338,13 @@ class NavField:
         self._m._ck(self._m._L.fiesta_nav_compute(self._h, lo.ctypes, hi.ctypes, goals.ctypes, C.c_int64(len(goals)), r, flags, C.byref(st)),
                     "NavField.compute")
         self.shape = tuple(int(b - a + 1) for a, b in zip(lo, hi))
+        return {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved_f"}
+
+    def update(self):
+        """Repair the field after map updates (fiesta_nav_update): afterwards it is bit for bit what compute() with the last box,
+        goals, clearance and flags would give on the current records -> stats dict."""
+        st = NavUpdateStats()
+        self._m._ck(self._m._L.fiesta_nav_update(self._h, C.byref(st)), "NavField.update")
         return {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved_f"}
 
     def export(self):

@@ -199,6 +199,15 @@ struct FbNavArgs {
 cudaError_t fb_nav_compute(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, const double *goals, long long n_goals, double r,
                            int unknown_blocks, int nblocks, cudaStream_t s);
 int fb_nav_relax_blocks(int device);
+// field update (fb_nav.cu, DESIGN.md §3.11)
+struct FbNavUCtr {
+  FbNavCtr wave;               // the withdrawal wave's work lists, generations and tile visits
+  unsigned long long became_blocked, became_free, withdrawn, goals_new;
+  unsigned seed_tiles, pad;
+};
+int fb_nav_withdraw_blocks(int device);
+cudaError_t fb_nav_update(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, uint8_t *flags, FbNavUCtr *u, const double *goals,
+                          long long n_goals, double r, int unknown_blocks, int nblocks, int wblocks, cudaStream_t s);
 cudaError_t fb_nav_paths(const FbGeom &g, const FbNavBox &b, const double *D, const double *w, const double *starts, long long n, int max_len,
                          int32_t *status, int32_t *len, double *cost, int32_t *vox, cudaStream_t s);
 // cost matrices (fb_navmatrix.cu): up to FB_NAVM_CH sources' fields relaxed together, one channel each

@@ -1011,12 +1011,16 @@ int fiesta_check_poses_device(fiesta_map *m, const double *d_poses, int64_t n, c
 struct fiesta_nav_field {
   fiesta_map *m = nullptr;
   int blocks = 0;                   // co-resident CTAs of k_nav_relax (cooperative launch)
+  int wblocks = 0;                  // co-resident CTAs of k_navu_withdraw
   FbDevBuf<double> D, d_goals;
   FbDevBuf<uint32_t> stamp, list[2];
   FbDevBuf<FbNavCtr> ctr;
   FbHostBuf<FbNavCtr> h_ctr;
   FbDevBuf<double> d_pd;            // fiesta_nav_paths: [starts 3n][cost n]
   FbDevBuf<int32_t> d_pi;           //                   [status n][len n][vox 3 n max_len]
+  FbDevBuf<uint8_t> u_flags;        // fiesta_nav_update: one scratch byte per box voxel
+  FbDevBuf<FbNavUCtr> u_ctr;
+  FbHostBuf<FbNavUCtr> h_uctr;
   // fiesta_nav_matrix: its own buffers, so that a matrix leaves the last field, export and paths as they were
   int mblocks = 0;                  // co-resident CTAs of k_navm_relax
   FbDevBuf<uint32_t> M;             // per box voxel: move mask
@@ -1031,6 +1035,9 @@ struct fiesta_nav_field {
   FbNavBox box{};
   double w[3]{};
   bool valid = false;               // D holds a field computed for `box`
+  long long n_goals = 0;            // goals (in d_goals), clearance and flags of the last compute: what fiesta_nav_update keeps
+  double clearance = 0.0;
+  int flags = 0;
 };
 void fiesta_nav_destroy(fiesta_nav_field *f) {
   if (!f) return;
@@ -1048,13 +1055,16 @@ int fiesta_nav_create(fiesta_map *m, fiesta_nav_field **out) {
   f->m = m;
   f->blocks = fb_nav_relax_blocks(m->device);
   f->mblocks = fb_navm_relax_blocks(m->device);
-  if (f->blocks <= 0 || f->mblocks <= 0) { fb_set_error("fiesta_nav_create: the relaxation kernel does not fit on this device"); return FIESTA_ERR_CUDA; }
+  f->wblocks = fb_nav_withdraw_blocks(m->device);
+  if (f->blocks <= 0 || f->mblocks <= 0 || f->wblocks <= 0) { fb_set_error("fiesta_nav_create: the relaxation kernel does not fit on this device"); return FIESTA_ERR_CUDA; }
   for (cudaEvent_t &e : f->ev) CK(cudaEventCreate(&e));
   CK(f->ctr.alloc(1));
   CK(f->h_ctr.alloc(1));
   CK(f->m_ctr.alloc(1));
   CK(f->m_tot.alloc(1));
   CK(f->h_mtot.alloc(1));
+  CK(f->u_ctr.alloc(1));
+  CK(f->h_uctr.alloc(1));
   for (int k = 0; k < 3; ++k) f->w[k] = m->g.res * sqrt((double)(k + 1));
   *out = f.release();
   return FIESTA_OK;
@@ -1102,6 +1112,9 @@ int fiesta_nav_compute(fiesta_nav_field *f, const int box_lo[3], const int box_h
   CK(cudaStreamSynchronize(m->stream));
   f->box = a.b;
   f->valid = true;
+  f->n_goals = n_goals;
+  f->clearance = clearance;
+  f->flags = flags;
   if (stats) {
     const FbNavCtr &c = *f->h_ctr;
     *stats = fiesta_nav_stats{};
@@ -1111,6 +1124,55 @@ int fiesta_nav_compute(fiesta_nav_field *f, const int box_lo[3], const int box_h
     stats->goals_placed = (int64_t)c.goals_placed;
     stats->generations = (int64_t)c.generations;
     stats->tile_visits = (int64_t)c.tile_visits;
+    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
+  }
+  return FIESTA_OK;
+}
+int fiesta_nav_update(fiesta_nav_field *f, fiesta_nav_update_stats *stats) {
+  const char *fn = "fiesta_nav_update";
+  if (!f) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (!f->valid) { fb_set_error("%s: no field has been computed", fn); return FIESTA_ERR_INVALID; }
+  fiesta_map *m = f->m;
+  FbNavArgs a{};
+  a.b = f->box;
+  for (int k = 0; k < 3; ++k) {
+    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
+    a.w[k] = f->w[k];
+  }
+  const size_t nv = (size_t)a.b.n[0] * a.b.n[1] * a.b.n[2];
+  CK(cudaSetDevice(m->device));
+  if (cudaError_t e = f->u_flags.grow(nv, m->stream)) {                  // before anything is written: the field stays valid
+    cudaGetLastError();
+    fb_set_error("%s: cannot allocate the scratch of %zu voxels: %s", fn, nv, cudaGetErrorString(e));
+    return FIESTA_ERR_CUDA;
+  }
+  a.D = f->D; a.stamp = f->stamp; a.list[0] = f->list[0]; a.list[1] = f->list[1]; a.ctr = f->ctr;
+  f->valid = false;                                                       // until the update has finished
+  CK(cudaEventRecord(f->ev[0], m->stream));
+  CK(fb_nav_update(m->g, m->cobs, a, f->u_flags, f->u_ctr, f->d_goals, f->n_goals, f->clearance, f->flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS,
+                   f->blocks, f->wblocks, m->stream));
+  m->st.kernel_launches += f->n_goals > 0 ? 6 : 5;
+  CK(cudaEventRecord(f->ev[1], m->stream));
+  CK(cudaMemcpyAsync(f->h_ctr, f->ctr, sizeof(FbNavCtr), cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(f->h_uctr, f->u_ctr, sizeof(FbNavUCtr), cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  f->valid = true;
+  if (stats) {
+    const FbNavCtr &c = *f->h_ctr;
+    const FbNavUCtr &u = *f->h_uctr;
+    *stats = fiesta_nav_update_stats{};
+    stats->box_voxels = (int64_t)nv;
+    stats->became_blocked = (int64_t)u.became_blocked;
+    stats->became_free = (int64_t)u.became_free;
+    stats->withdrawn = (int64_t)u.withdrawn;
+    stats->goals_placed = (int64_t)c.goals_placed;
+    stats->goals_new = (int64_t)u.goals_new;
+    stats->seed_tiles = (int64_t)u.seed_tiles;
+    stats->withdraw_generations = (int64_t)u.wave.generations;
+    stats->generations = (int64_t)c.generations;
+    stats->tile_visits = (int64_t)c.tile_visits;
+    stats->blocked = (int64_t)c.blocked;
+    stats->reached = (int64_t)c.reached;
     CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
   }
   return FIESTA_OK;

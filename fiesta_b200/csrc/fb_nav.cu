@@ -190,6 +190,215 @@ __global__ void k_nav_path(FbGeom g, FbNavBox b, const double *__restrict__ D, d
   status[i] = fb_nav_path(b, D, w, v, max_len, vox + 3 * (long long)max_len * i, &len[i], &cost[i]);
 }
 
+// ---------------------------------------------------------------- field update (DESIGN.md §3.11)
+// k_navu_scan     : the new traversability of every box voxel against the field's sign (the old one) into the scratch byte
+//                   (FB_NAVU_NEWT, FB_NAVU_CHG); counts the changes and queues for the withdrawal wave every tile holding a
+//                   26-neighbour of a newly blocked voxel (only those voxels can lose a move).
+// k_navu_withdraw : the withdrawal wave, persistent and cooperative with k_nav_relax's work list, stamps and rotating counters.  A
+//                   tile stages old costs and scratch bytes with a 1-voxel halo, and withdraws (FB_NAVU_WD) each candidate none of
+//                   whose tight supports is still kept through a still-allowed move, to a local fixpoint; the tiles across the
+//                   faces of a newly withdrawn boundary voxel are queued.  Withdrawals only accumulate and the support relation is
+//                   acyclic, so from all-kept every schedule ends at the unique solution.  The field itself is only read.
+// k_navu_apply    : the start state of the re-relaxation (-1 newly blocked, +inf withdrawn and newly free, everything else as it
+//                   was) and generation 0's tile list: the tile of a withdrawn voxel, every tile holding a newly free voxel or
+//                   one of its 26 neighbours (a newly placed goal is always newly free, so its tiles are among them).
+// k_navu_goals    : D := 0 on the stored goals that are traversable, as k_nav_goals does.
+// Then k_nav_relax and k_nav_count run unchanged.
+
+// Allowed moves into the centre voxel from the traversability of its 3x3x3 neighbourhood: fb_nav_move_bits without bit 13, unrolled
+// as in k_nav_relax.
+static __device__ __forceinline__ unsigned navu_allowed(unsigned nb) {
+  unsigned allowed = 0;
+  if (!(nb & (1u << 13))) return 0;
+#pragma unroll
+  for (int k = 0; k < 27; ++k) {
+    if (k == 13) continue;
+    const int dx = k / 9 - 1, dy = k / 3 % 3 - 1, dz = k % 3 - 1;
+    unsigned need = 0;
+#pragma unroll
+    for (int ex = (dx < 0 ? -1 : 0); ex <= (dx > 0 ? 1 : 0); ++ex)
+#pragma unroll
+      for (int ey = (dy < 0 ? -1 : 0); ey <= (dy > 0 ? 1 : 0); ++ey)
+#pragma unroll
+        for (int ez = (dz < 0 ? -1 : 0); ez <= (dz > 0 ? 1 : 0); ++ez) need |= 1u << ((ex + 1) * 9 + (ey + 1) * 3 + ez + 1);
+    if ((nb & need) == need) allowed |= 1u << k;
+  }
+  return allowed;
+}
+
+// Queue every tile that holds box voxel v or one of its 26 neighbours (own) or only those across its faces (!own) with `stamp`.
+static __device__ void navu_queue(const FbNavArgs &a, int x, int y, int z, bool own, unsigned stamp, uint32_t *list, unsigned *n) {
+  const int v[3] = {x, y, z};
+  for (int ox = ((v[0] & 7) == 0 ? -1 : 0); ox <= ((v[0] & 7) == FB_TILE - 1 ? 1 : 0); ++ox)
+    for (int oy = ((v[1] & 7) == 0 ? -1 : 0); oy <= ((v[1] & 7) == FB_TILE - 1 ? 1 : 0); ++oy)
+      for (int oz = ((v[2] & 7) == 0 ? -1 : 0); oz <= ((v[2] & 7) == FB_TILE - 1 ? 1 : 0); ++oz) {
+        if (!own && ox == 0 && oy == 0 && oz == 0) continue;
+        const int nx = (v[0] >> 3) + ox, ny = (v[1] >> 3) + oy, nz = (v[2] >> 3) + oz;
+        if (nx < 0 || nx >= a.tn[0] || ny < 0 || ny >= a.tn[1] || nz < 0 || nz >= a.tn[2]) continue;
+        const unsigned t = (unsigned)((nx * a.tn[1] + ny) * a.tn[2] + nz);
+        // the plain read spares the atomic on tiles already queued (a stamp, once set, stays for the rest of the kernel)
+        if (__ldcg(&a.stamp[t]) != stamp && atomicExch(&a.stamp[t], stamp) != stamp) list[atomicAdd(n, 1u)] = t;
+      }
+}
+
+__global__ void k_navu_scan(FbGeom g, const uint32_t *__restrict__ cobs, FbNavArgs w, uint8_t *__restrict__ flags, FbNavUCtr *u,
+                            double r, int unknown_blocks) {
+  const long long n = (long long)w.b.n[0] * w.b.n[1] * w.b.n[2];
+  unsigned nblk = 0, nfree = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int z = (int)(i % w.b.n[2]), y = (int)(i / w.b.n[2] % w.b.n[1]), x = (int)(i / ((long long)w.b.n[2] * w.b.n[1]));
+    const int v[3] = {w.b.lo[0] + x, w.b.lo[1] + y, w.b.lo[2] + z};
+    double d;
+    const bool newt = !fb_seg_blocks(g, cobs, v, r, unknown_blocks != 0, d), oldt = w.D[i] >= 0.0;
+    flags[i] = (uint8_t)((newt ? FB_NAVU_NEWT : 0u) | (newt != oldt ? FB_NAVU_CHG : 0u));
+    if (oldt && !newt) {
+      ++nblk;
+      navu_queue(w, x, y, z, true, 1u, w.list[0], &w.ctr->n[0]);          // generation 0 has stamp 1
+    }
+    nfree += newt && !oldt;
+  }
+  nblk = __reduce_add_sync(0xffffffffu, nblk);
+  nfree = __reduce_add_sync(0xffffffffu, nfree);
+  if ((threadIdx.x & 31) == 0) {
+    if (nblk) atomicAdd(&u->became_blocked, (unsigned long long)nblk);
+    if (nfree) atomicAdd(&u->became_free, (unsigned long long)nfree);
+  }
+}
+
+__global__ void __launch_bounds__(NAV_THREADS, 2) k_navu_withdraw(FbNavArgs a, uint8_t *flags) {
+  __shared__ double sD[NAV_H * NAV_H * NAV_H];
+  __shared__ uint8_t sF[NAV_H * NAV_H * NAV_H];
+  __shared__ unsigned s_tile, s_q;
+  cg::grid_group grid = cg::this_grid();
+  const int tid = threadIdx.x, lx = tid >> 6, ly = (tid >> 3) & 7, lz = tid & 7;
+  const int c = ((lx + 1) * NAV_H + ly + 1) * NAV_H + lz + 1;
+  unsigned long long visits = 0;
+  unsigned gen = 0;
+  for (;; ++gen) {                                                        // the generation loop of k_nav_relax
+    const unsigned cur = gen % 3u, nxt = (gen + 1u) % 3u;
+    const unsigned nwork = __ldcg(&a.ctr->n[cur]);
+    if (nwork == 0) break;
+    if (blockIdx.x == 0 && tid == 0) { a.ctr->n[(gen + 2u) % 3u] = 0; a.ctr->next[(gen + 2u) % 3u] = 0; }
+    const uint32_t *list = (gen & 1u) ? a.list[1] : a.list[0];
+    uint32_t *out = (gen & 1u) ? a.list[0] : a.list[1];
+    const unsigned stamp_next = gen + 2u;
+    for (;;) {
+      if (tid == 0) {
+        const unsigned k = atomicAdd(&a.ctr->next[cur], 1u);
+        s_tile = k < nwork ? __ldcg(&list[k]) : NAV_NONE;
+        s_q = 0;
+      }
+      __syncthreads();
+      const unsigned tile = s_tile;
+      if (tile == NAV_NONE) break;
+      if (tid == 0) ++visits;
+      const int tz = (int)(tile % (unsigned)a.tn[2]), ty = (int)(tile / (unsigned)a.tn[2] % (unsigned)a.tn[1]),
+                tx = (int)(tile / (unsigned)(a.tn[2] * a.tn[1]));
+      const int x0 = tx * FB_TILE - 1, y0 = ty * FB_TILE - 1, z0 = tz * FB_TILE - 1;
+      for (int i = tid; i < NAV_H * NAV_H * NAV_H; i += NAV_THREADS) {
+        const int x = x0 + i / (NAV_H * NAV_H), y = y0 + i / NAV_H % NAV_H, z = z0 + i % NAV_H;
+        const bool in = fb_nav_in_box(a.b, x, y, z);
+        const long long ii = in ? fb_nav_idx(a.b, x, y, z) : 0;
+        sD[i] = in ? __ldcg(&a.D[ii]) : FB_NAV_BLOCKED;
+        sF[i] = in ? __ldcg(&flags[ii]) : (uint8_t)0;
+      }
+      __syncthreads();
+      // candidates: still traversable, finite non-zero old cost, not yet withdrawn; sup = tight supports still allowed now
+      const double dv = sD[c];
+      const uint8_t f0 = sF[c];
+      bool cand = (f0 & FB_NAVU_NEWT) && !(f0 & FB_NAVU_WD) && dv > 0.0 && dv < (double)INFINITY;
+      unsigned sup = 0;
+      if (cand) {
+        unsigned nb = 0;
+#pragma unroll
+        for (int e = 0; e < 27; ++e) nb |= (sD[c + ((e / 9 - 1) * NAV_H + (e / 3 % 3 - 1)) * NAV_H + (e % 3 - 1)] >= 0.0 ? 1u : 0u) << e;
+        const unsigned old_bits = navu_allowed(nb);
+        for (unsigned m = old_bits; m; m &= m - 1u) {                      // the moves allowed before, one set bit at a time
+          const int k = __ffs(m) - 1, dx = k / 9 - 1, dy = k / 3 % 3 - 1, dz = k % 3 - 1, nz = (dx != 0) + (dy != 0) + (dz != 0);
+          if (fb_nav_is_support(true, sD[c + (dx * NAV_H + dy) * NAV_H + dz], nz == 1 ? a.w[0] : nz == 2 ? a.w[1] : a.w[2], dv)) sup |= 1u << k;
+        }
+        nb = 0;
+#pragma unroll
+        for (int e = 0; e < 27; ++e) nb |= ((sF[c + ((e / 9 - 1) * NAV_H + (e / 3 % 3 - 1)) * NAV_H + (e % 3 - 1)] & FB_NAVU_NEWT) ? 1u : 0u) << e;
+        sup &= navu_allowed(nb);
+      }
+      for (;;) {                                                          // local fixpoint: withdrawals only accumulate
+        bool ch = false;
+        if (cand) {
+          bool kept = false;
+          for (unsigned m = sup; m && !kept; m &= m - 1u) {                 // the supports, one set bit at a time
+            const int k = __ffs(m) - 1;
+            kept = !(sF[c + ((k / 9 - 1) * NAV_H + (k / 3 % 3 - 1)) * NAV_H + (k % 3 - 1)] & FB_NAVU_WD);
+          }
+          if (!kept) { sF[c] = (uint8_t)(f0 | FB_NAVU_WD); cand = false; ch = true; }
+        }
+        if (!__syncthreads_or(ch)) break;
+      }
+      if ((sF[c] & FB_NAVU_WD) && !(f0 & FB_NAVU_WD)) {
+        const int x = tx * FB_TILE + lx, y = ty * FB_TILE + ly, z = tz * FB_TILE + lz;
+        __stcg(&flags[fb_nav_idx(a.b, x, y, z)], sF[c]);
+        unsigned q = 0;
+        for (int ox = (lx == 0 ? -1 : 0); ox <= (lx == FB_TILE - 1 ? 1 : 0); ++ox)
+          for (int oy = (ly == 0 ? -1 : 0); oy <= (ly == FB_TILE - 1 ? 1 : 0); ++oy)
+            for (int oz = (lz == 0 ? -1 : 0); oz <= (lz == FB_TILE - 1 ? 1 : 0); ++oz) q |= 1u << ((ox + 1) * 9 + (oy + 1) * 3 + oz + 1);
+        q &= ~(1u << 13);
+        if (q) atomicOr(&s_q, q);
+      }
+      __syncthreads();
+      if (tid < 27 && ((s_q >> tid) & 1u)) {
+        const int nx = tx + tid / 9 - 1, ny = ty + tid / 3 % 3 - 1, nz = tz + tid % 3 - 1;
+        if (nx >= 0 && nx < a.tn[0] && ny >= 0 && ny < a.tn[1] && nz >= 0 && nz < a.tn[2]) {
+          const unsigned t = (unsigned)((nx * a.tn[1] + ny) * a.tn[2] + nz);
+          if (atomicExch(&a.stamp[t], stamp_next) != stamp_next) out[atomicAdd(&a.ctr->n[nxt], 1u)] = t;
+        }
+      }
+      __syncthreads();
+    }
+    grid.sync();
+  }
+  if (tid == 0) {
+    if (visits) atomicAdd(&a.ctr->tile_visits, visits);
+    if (blockIdx.x == 0) a.ctr->generations = gen;
+  }
+}
+
+__global__ void k_navu_apply(FbNavArgs a, const uint8_t *__restrict__ flags, FbNavUCtr *u) {
+  const long long n = (long long)a.b.n[0] * a.b.n[1] * a.b.n[2];
+  unsigned wd = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const unsigned f = flags[i];
+    if (!(f & FB_NAVU_NEWT)) {
+      if (f & FB_NAVU_CHG) a.D[i] = FB_NAV_BLOCKED;
+      continue;
+    }
+    if (!(f & (FB_NAVU_CHG | FB_NAVU_WD))) continue;                     // kept, or unreached before and after
+    a.D[i] = (double)INFINITY;
+    wd += (f & FB_NAVU_CHG) == 0;
+    const int z = (int)(i % a.b.n[2]), y = (int)(i / a.b.n[2] % a.b.n[1]), x = (int)(i / ((long long)a.b.n[2] * a.b.n[1]));
+    if (f & FB_NAVU_CHG) {
+      navu_queue(a, x, y, z, true, 1u, a.list[0], &a.ctr->n[0]);        // a freed voxel can allow a move between two others
+    } else {
+      const unsigned t = (unsigned)(((x >> 3) * a.tn[1] + (y >> 3)) * a.tn[2] + (z >> 3));
+      if (__ldcg(&a.stamp[t]) != 1u && atomicExch(&a.stamp[t], 1u) != 1u) a.list[0][atomicAdd(&a.ctr->n[0], 1u)] = t;
+    }
+  }
+  wd = __reduce_add_sync(0xffffffffu, wd);
+  if ((threadIdx.x & 31) == 0 && wd) atomicAdd(&u->withdrawn, (unsigned long long)wd);
+}
+
+__global__ void k_navu_goals(FbGeom g, FbNavArgs a, const uint8_t *__restrict__ flags, FbNavUCtr *u, const double *__restrict__ goals,
+                             long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int v[3];
+  if (!fb_nav_locate(g, a.b, goals + 3 * i, v)) return;
+  const long long ii = fb_nav_idx(a.b, v[0], v[1], v[2]);
+  if (!(a.D[ii] >= 0.0)) return;                                          // blocked goal
+  a.D[ii] = 0.0;
+  atomicAdd(&a.ctr->goals_placed, 1ull);
+  if (flags[ii] & FB_NAVU_CHG) atomicAdd(&u->goals_new, 1ull);           // newly free: its tiles are queued by k_navu_apply
+}
+
 // ---------------------------------------------------------------- host side
 static unsigned nav_blocks(long long n) {
   const long long want = (n + 255) / 256;
@@ -210,6 +419,40 @@ cudaError_t fb_nav_compute(const FbGeom &g, const uint32_t *cobs, const FbNavArg
   if (n_goals > 0) k_nav_goals<<<(unsigned)((n_goals + 127) / 128), 128, 0, s>>>(g, a, goals, n_goals);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
+  void *args[] = {(void *)&a};
+  if ((e = cudaLaunchCooperativeKernel((void *)k_nav_relax, dim3(nblocks), dim3(NAV_THREADS), args, 0, s)) != cudaSuccess) return e;
+  k_nav_count<<<nav_blocks(n), 256, 0, s>>>(a);
+  return cudaGetLastError();
+}
+
+int fb_nav_withdraw_blocks(int device) {
+  int per_sm = 0, sms = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_navu_withdraw, NAV_THREADS, 0) != cudaSuccess) return 0;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
+  return per_sm * sms;
+}
+
+// The whole update on stream s: 5 launches, 6 with goals.  a.D holds the old field; a.ctr and u are cleared here.
+cudaError_t fb_nav_update(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, uint8_t *flags, FbNavUCtr *u, const double *goals,
+                          long long n_goals, double r, int unknown_blocks, int nblocks, int wblocks, cudaStream_t s) {
+  const long long n = (long long)a.b.n[0] * a.b.n[1] * a.b.n[2];
+  const size_t nt = (size_t)a.tn[0] * a.tn[1] * a.tn[2];
+  FbNavArgs w = a;                                                        // the wave: same lists and stamps, its own counters
+  w.ctr = &u->wave;
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(u, 0, sizeof(FbNavUCtr), s)) != cudaSuccess) return e;
+  if ((e = cudaMemsetAsync(a.stamp, 0, nt * 4, s)) != cudaSuccess) return e;
+  k_navu_scan<<<nav_blocks(n), 256, 0, s>>>(g, cobs, w, flags, u, r, unknown_blocks);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  void *wargs[] = {(void *)&w, (void *)&flags};
+  if ((e = cudaLaunchCooperativeKernel((void *)k_navu_withdraw, dim3(wblocks), dim3(NAV_THREADS), wargs, 0, s)) != cudaSuccess) return e;
+  // old costs are read until here; the re-relaxation starts from clean stamps and counters, as in fb_nav_compute
+  if ((e = cudaMemsetAsync(a.stamp, 0, nt * 4, s)) != cudaSuccess) return e;
+  if ((e = cudaMemsetAsync(a.ctr, 0, sizeof(FbNavCtr), s)) != cudaSuccess) return e;
+  k_navu_apply<<<nav_blocks(n), 256, 0, s>>>(a, flags, u);
+  if (n_goals > 0) k_navu_goals<<<(unsigned)((n_goals + 127) / 128), 128, 0, s>>>(g, a, flags, u, goals, n_goals);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  if ((e = cudaMemcpyAsync(&u->seed_tiles, &a.ctr->n[0], 4, cudaMemcpyDeviceToDevice, s)) != cudaSuccess) return e;
   void *args[] = {(void *)&a};
   if ((e = cudaLaunchCooperativeKernel((void *)k_nav_relax, dim3(nblocks), dim3(NAV_THREADS), args, 0, s)) != cudaSuccess) return e;
   k_nav_count<<<nav_blocks(n), 256, 0, s>>>(a);

@@ -70,6 +70,33 @@ FB_HD unsigned fb_nav_move_bits(unsigned nb) {
   return out;
 }
 
+// Field update (fiesta_nav_update, DESIGN.md §3.11).  u = v + fb_nav_dir(k) is a tight support of v when the move u -> v was allowed
+// under the old traversability (fb_nav_move_bits of the old signs), D_old(u) is finite and fl(D_old(u) + w) == D_old(v).  Weights are positive, so a support always has the smaller cost and the relation is acyclic.
+FB_HD bool fb_nav_is_support(bool old_allowed, double du, double w, double dv) {
+  return old_allowed && du < (double)INFINITY && du + w == dv;
+}
+FB_HD double fb_nav_weight(int k, const double *w) {   // weight of a move in direction k != 13
+  int d[3];
+  fb_nav_dir(k, d);
+  const int nz = (d[0] != 0) + (d[1] != 0) + (d[2] != 0);
+  return nz == 1 ? w[0] : nz == 2 ? w[1] : w[2];
+}
+// All tight supports of a voxel from its 3x3x3 neighbourhood of old costs d27 (d27[13]: the voxel; -1 outside the box): bit k set
+// when neighbour k is one.  0 for a blocked voxel.
+FB_HD unsigned fb_nav_support_bits(const double *d27, const double *w) {
+  unsigned nb = 0;
+  for (int e = 0; e < 27; ++e) nb |= (d27[e] >= 0.0 ? 1u : 0u) << e;
+  const unsigned old_bits = fb_nav_move_bits(nb);
+  unsigned out = 0;
+  for (int k = 0; k < 27; ++k)
+    if (k != 13 && fb_nav_is_support((old_bits >> k) & 1u, d27[k], fb_nav_weight(k, w), d27[13])) out |= 1u << k;
+  return out;
+}
+// Per box voxel scratch byte of an update
+#define FB_NAVU_NEWT 1u      // traversable on the current records
+#define FB_NAVU_CHG 2u       // traversability changed since the field was last brought up to date
+#define FB_NAVU_WD 4u        // withdrawn: still traversable, finite old cost, no kept support
+
 // One step of the path rule: the first allowed neighbour u of v, in direction order, with fl(D(u) + w) == D(v).  False when there
 // is none (never at the fixpoint, for a reached voxel other than a goal).
 FB_HD bool fb_nav_step(const FbNavBox &b, const double *D, const double *w, int *v) {

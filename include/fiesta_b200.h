@@ -264,7 +264,8 @@ int fiesta_host_mirror_check_poses(const fiesta_host_mirror *p, const double *po
 
 /* ---- cost-to-go field (planners: A* / hybrid-A* heuristics, guide paths for trajectory optimisers, cost to frontier goals) ----
  * How far is the nearest goal through free space, keeping a clearance, and which way leads there?  The field covers an inclusive
- * voxel box [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis) and is a snapshot of the records at the time of the call.
+ * voxel box [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis) and is a snapshot of the records at the time of the call
+ * (fiesta_nav_update brings it up to date).
  *   traversable  a voxel of the box that does not block in the sense of segment clearance: GetDistance(Vector3i) > clearance,
  *                and, with FIESTA_SEGMENT_UNKNOWN_BLOCKS, observed.  Voxels outside the box count as blocked.
  *   moves        u -> u+d for the 26 offsets d in {-1,0,1}^3 \ {0}, allowed iff every voxel of the axis-aligned box spanned by u
@@ -302,6 +303,33 @@ int fiesta_nav_compute(fiesta_nav_field *f, const int box_lo[3], const int box_h
 int fiesta_nav_export(const fiesta_nav_field *f, double *out);   /* box_voxels doubles */
 int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, int32_t max_len, int32_t *status, int32_t *len,
                      double *cost, int32_t *vox_xyz /* n * max_len * 3 */);
+
+/* ---- cost-to-go fields that follow the map (replanning at sensor rate: D* Lite / LPA*-style users of a live field) ----
+ * fiesta_nav_update re-reads the map's records and repairs the field in place instead of recomputing it.  Afterwards the field,
+ * fiesta_nav_export and fiesta_nav_paths are bit for bit what fiesta_nav_compute would give now with the box, goals, clearance and
+ * flags of the last successful compute, in both map modes and after any sequence of frames, SetUpdateRange / local-map resets,
+ * SetParameters and chained updates.  A goal ignored because its voxel was blocked counts again once the voxel is traversable,
+ * and the reverse.  The old traversability is the field's own sign; voxels whose finite cost lost its support through a voxel
+ * that became blocked are withdrawn, then the relaxation of fiesta_nav_compute runs from the repaired start state over the tiles
+ * near the changes only (DESIGN.md §3.11), so a call with nothing changed does no relaxation (generations == tile_visits == 0).
+ * fiesta_nav_matrix keeps its own buffers: a matrix between a compute and an update changes neither.  Memory: 1 scratch byte per
+ * box voxel on the field object, grown like its other buffers (201 MB for a 512^3 box with the 50 % growth headroom).
+ * Synchronous, on the map's stream.  Errors: FIESTA_ERR_INVALID for a null field or before any successful compute (nothing
+ * changes); FIESTA_ERR_CUDA when the scratch cannot be allocated, in which case nothing has been written and the field is still
+ * valid. */
+typedef struct fiesta_nav_update_stats {
+  int64_t box_voxels;
+  int64_t became_blocked, became_free;   /* box voxels whose traversability changed since the field was last brought up to date */
+  int64_t withdrawn;                     /* traversable voxels whose finite cost lost its support (DESIGN.md §3.11) */
+  int64_t goals_placed, goals_new;       /* goals_placed as fiesta_nav_stats; goals_new: placed now, not placed before (duplicates
+                                            counted), i.e. goals on a voxel that became free */
+  int64_t seed_tiles;                    /* 8^3 tiles queued for the re-relaxation's generation 0 */
+  int64_t withdraw_generations, generations, tile_visits;   /* withdrawal wave; re-relaxation (as fiesta_nav_stats) */
+  int64_t blocked, reached;              /* of the repaired field, as fiesta_nav_stats */
+  float ms_compute;                      /* device time of the whole update */
+  float reserved_f[1];
+} fiesta_nav_update_stats;
+int fiesta_nav_update(fiesta_nav_field *f, fiesta_nav_update_stats *stats /* nullable */);
 
 /* ---- cost matrices (tour planners, task allocation, roadmap edge costs): the geodesic cost from each of many sources to each of
  * many targets through free space at a clearance, in one call.

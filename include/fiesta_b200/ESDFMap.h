@@ -181,6 +181,13 @@ class ESDFMap {
     check(fiesta_nav_compute(f, box_lo, box_hi, goals_xyz, n_goals, clearance, flags, &st), "ComputeNavField");
     return st;
   }
+  // Repair the field after map updates (fiesta_nav_update): the bits ComputeNavField would give now with the same box, goals,
+  // clearance and flags, at the cost of the region the changes affect.
+  fiesta_nav_update_stats UpdateNavField(fiesta_nav_field *f) {
+    fiesta_nav_update_stats st = {};
+    check(fiesta_nav_update(f, &st), "UpdateNavField");
+    return st;
+  }
   // Cost matrix (fiesta_nav_matrix): cost[i * n_tgt + j] = the field of source i alone read at target j, NaN where either point is
   // blocked or outside the box.  Leaves the last ComputeNavField result as it was.
   fiesta_nav_matrix_stats NavCostMatrix(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *sources_xyz, long n_src,
