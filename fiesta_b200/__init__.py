@@ -111,6 +111,7 @@ SYMBOLS = [
     "fiesta_frontiers_voxels", "fiesta_frontiers_export", "fiesta_frontiers_score_viewpoints",
     "fiesta_inflate_boxes", "fiesta_corridors",
     "fiesta_check_poses", "fiesta_check_poses_device", "fiesta_host_mirror_check_poses",
+    "fiesta_snapshot_save", "fiesta_snapshot_load", "fiesta_get_config",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -185,6 +186,9 @@ def load_library():
                                                         C.POINTER(SensorModel), C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.fiesta_inflate_boxes.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 4
         L.fiesta_corridors.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 7
+        L.fiesta_snapshot_save.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
+        L.fiesta_snapshot_load.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.POINTER(C.c_void_p)]
+        L.fiesta_get_config.argtypes = [C.c_void_p, C.POINTER(Config)]
         L.fiesta_get_distance_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
         L.fiesta_get_dist_grad_trilinear_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
@@ -485,13 +489,53 @@ class ESDFMap:
         if rc != 0:
             raise FiestaError("fiesta_create failed (%d): %s" % (rc, self._L.fiesta_last_error().decode()))
         self._h = h
+        self._describe()
+        self.mode = mode                                     # as requested (FIESTA_B200_MODE may override the map's own)
+
+    def _describe(self):
+        """grid_size, resolution, origin, mode and device of the map behind the handle (fiesta_get_config)."""
+        cfg = Config()
+        self._ck(self._L.fiesta_get_config(self._h, C.byref(cfg)), "fiesta_get_config")
         self.grid_total_size_ = int(self._L.fiesta_grid_total_size(self._h))
         g = I3()
         self._L.fiesta_grid_size(self._h, g)
         self.grid_size = tuple(int(x) for x in g)
-        self.resolution = float(resolution)
-        self.origin = tuple(float(x) for x in origin)
-        self.device = int(device)
+        self.resolution = float(cfg.resolution)
+        self.origin = tuple(float(x) for x in cfg.origin)
+        self.mode = ("exact", "fast")[cfg.mode]
+        self.device = int(cfg.device)
+
+    # --- map snapshots (fiesta_snapshot_save / fiesta_snapshot_load) ---
+    def save(self, path=None):
+        """Snapshot of the map (it must be quiescent: after UpdateESDF) as bytes, or written to the file `path`."""
+        n = C.c_int64(0)
+        self._ck(self._L.fiesta_snapshot_save(self._h, None, C.c_int64(0), C.byref(n)), "save")
+        buf = np.empty(n.value, np.uint8)
+        self._ck(self._L.fiesta_snapshot_save(self._h, buf.ctypes.data, C.c_int64(n.value), C.byref(n)), "save")
+        if path is None:
+            return buf.tobytes()
+        with open(path, "wb") as f:
+            f.write(buf.data)
+        return None
+
+    @classmethod
+    def load(cls, src, device=0):
+        """A new map from a snapshot: bytes-like data, or the path of a file holding one.  It continues bit for bit like the
+        saved map, in the snapshot's mode."""
+        if isinstance(src, (str, os.PathLike)):
+            with open(src, "rb") as f:
+                src = f.read()
+        buf = np.frombuffer(src, np.uint8)
+        self = cls.__new__(cls)
+        self._L = load_library()
+        h = C.c_void_p()
+        rc = self._L.fiesta_snapshot_load(buf.ctypes.data if len(buf) else None, C.c_int64(len(buf)), C.c_int32(int(device)), C.byref(h))
+        if rc != 0:
+            self._h = None
+            raise FiestaError("fiesta_snapshot_load failed (%d): %s" % (rc, self._L.fiesta_last_error().decode()))
+        self._h = h
+        self._describe()
+        return self
 
     def _ck(self, rc, what):
         if rc != 0:

@@ -19,6 +19,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <vector>
 #include "fb_host.h"     // FbDevBuf, CK
 #include "fb_record.h"   // FB_UNKNOWN / FB_INF / FB_DINF / FB_CODE_MASK, FbGeom, fb_pack / fb_unpack, fb_ii, the distance read
 #include "fb_nav.h"      // FbNavBox (cost-to-go field)
@@ -319,6 +320,29 @@ struct FbPoseBufs {                // device buffers of fiesta_check_poses(_devi
 int fb_pose_check_batch(const FbGeom &g, const uint32_t *cobs, const double *poses, long long n, const double *h, double clearance,
                         int unknown_blocks, int32_t *status, int32_t *n_blocked, int64_t *hit_idx, FbPoseBufs &B, cudaStream_t s,
                         int *launches);
+// map snapshots (fb_snapshot.cu; format in fb_snapshot.h)
+#define FB_SNAP_STAGE (16u << 20)  // bytes of each of the two device and two pinned staging buffers of a save or load
+struct FbSnapArrays {              // the per-voxel state a snapshot carries; LS is null in FAST mode
+  FbGeom g;
+  uint32_t *cobs;
+  double *occ;
+  unsigned long long *cnt, *LS;
+};
+struct FbSnapBufs {                // per-tile scratch of one save or load
+  FbDevBuf<uint8_t> flag;          // per grid tile: holds non-default state
+  FbDevBuf<uint32_t> list, d_n;    // stored tiles ascending; selection count, or {first bad tile, reasons} on load
+  FbDevBuf<unsigned long long> off;  // per stored tile: payload offset, and the end
+  FbHostBuf<uint32_t> h_n;
+  FbDevBuf<char> tmp;              // CUB temporary storage
+};
+// Lists the tiles with non-default state into B.list (ascending) and their count into *n.
+int fb_snap_list_tiles(const FbSnapArrays &A, FbSnapBufs &B, unsigned *n, cudaStream_t s);
+// Payload of the B.list tiles, whose offsets (and the end) are `off`, written to host memory dst + off[t].
+int fb_snap_pack(const FbSnapArrays &A, FbSnapBufs &B, const std::vector<unsigned long long> &off, uint8_t *dst, cudaStream_t s, int *launches);
+// Scatters the payload at src + off[t] of the h_list tiles into A; *bad_tile = the first tile position that failed validation
+// (0xffffffff: none), *reasons = the FB_SNAP_BAD_* bits.
+int fb_snap_unpack(const FbSnapArrays &A, FbSnapBufs &B, const uint32_t *h_list, const std::vector<unsigned long long> &off, const uint8_t *src,
+                   unsigned long long tclock, unsigned *bad_tile, unsigned *reasons, cudaStream_t s, int *launches);
 struct FbDepthRel { double m[16]; };
 struct fiesta_depth_params;
 cudaError_t fb_depth_to_cloud(const uint16_t *d_img, const uint16_t *d_last, int rows, int cols, const fiesta_depth_params &p, int filter_on,

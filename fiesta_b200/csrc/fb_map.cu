@@ -20,6 +20,7 @@
 #include "fb_segment.h"
 #include "fb_corridor.h"
 #include "fb_pose.h"
+#include "fb_snapshot.h"
 
 static thread_local std::string g_last_error;
 void fb_set_error(const char *fmt, ...) {
@@ -33,6 +34,7 @@ void fb_set_error(const char *fmt, ...) {
 
 struct fiesta_map {
   FbGeom g{};
+  fiesta_config cfg{};              // as given at create, with the device and the mode in force (fiesta_get_config, snapshots)
   int device = 0;
   cudaStream_t stream = nullptr;
   bool params_set = false;
@@ -377,7 +379,8 @@ void fiesta_destroy(fiesta_map *m) {
   delete m;                                                               // the buffers free themselves
 }
 
-int fiesta_create(const fiesta_config *cfg, fiesta_map **out) {
+// fiesta_create; a snapshot load passes honour_env = false, so that the mode it restores is not overridden by FIESTA_B200_MODE
+static int create_map(const fiesta_config *cfg, fiesta_map **out, bool honour_env) {
   if (!cfg || !out) { fb_set_error("fiesta_create: null argument"); return FIESTA_ERR_INVALID; }
   *out = nullptr;
   if (!(cfg->resolution > 0)) { fb_set_error("fiesta_create: resolution must be > 0"); return FIESTA_ERR_INVALID; }
@@ -393,11 +396,14 @@ int fiesta_create(const fiesta_config *cfg, fiesta_map **out) {
   if (!m) { fb_set_error("out of host memory"); return FIESTA_ERR_INVALID; }
   m->device = cfg->device;
   m->mode = cfg->mode == FIESTA_MODE_FAST ? FIESTA_MODE_FAST : FIESTA_MODE_EXACT;
-  if (const char *em = getenv("FIESTA_B200_MODE")) {                    // documented override (include/fiesta_b200.h)
+  const char *em = honour_env ? getenv("FIESTA_B200_MODE") : nullptr;
+  if (em) {                                                               // documented override (include/fiesta_b200.h)
     if (!strcmp(em, "fast")) m->mode = FIESTA_MODE_FAST; else if (!strcmp(em, "exact")) m->mode = FIESTA_MODE_EXACT;
   }
   FbGeom &g = m->g;
   int gs[3];
+  m->cfg = *cfg;
+  m->cfg.mode = m->mode;
   for (int i = 0; i < 3; ++i) {                                           // ctor, ESDFMap.cpp:171-186
     g.origin[i] = cfg->origin[i];
     gs[i] = (int)ceil(cfg->map_size[i] / cfg->resolution);
@@ -453,6 +459,12 @@ int fiesta_create(const fiesta_config *cfg, fiesta_map **out) {
   if (m->mode == FIESTA_MODE_EXACT && (r = fb_exact_init(&m->X, g, m->device, m->stream))) return r;
   CK(cudaStreamSynchronize(m->stream));
   *out = m.release();
+  return FIESTA_OK;
+}
+int fiesta_create(const fiesta_config *cfg, fiesta_map **out) { return create_map(cfg, out, true); }
+int fiesta_get_config(const fiesta_map *m, fiesta_config *out) {
+  if (!m || !out) return FIESTA_ERR_INVALID;
+  *out = m->cfg;
   return FIESTA_OK;
 }
 
@@ -632,18 +644,24 @@ int fiesta_raycast_frame(fiesta_map *m, const float *xyz, int64_t n, const doubl
   return fiesta_raycast_frame_device(m, m->d_xyz, n, T, p);
 }
 
+// the depth front end's buffers for images of N pixels, with no previous image or cloud
+static int alloc_depth(fiesta_map *m, size_t N) {
+  // d_img[0] is released first and allocated last, so its capacity is 0 until all six buffers hold N pixels: a call that
+  // fails part-way leaves the next call to reallocate them all
+  m->d_img[0] = FbDevBuf<uint16_t>();
+  m->image_cnt = 0; m->last_cloud_n = 0;
+  CK(m->d_img[1].alloc(N)); CK(m->d_dpts.alloc(N * 3)); CK(m->d_dcloud.alloc(N * 3)); CK(m->d_dflags.alloc(N)); CK(m->d_dsel.alloc(N));
+  CK(m->d_img[0].alloc(N));
+  return FIESTA_OK;
+}
 int fiesta_depth_frame(fiesta_map *m, const uint16_t *depth, int rows, int cols, const fiesta_depth_params *dp, const double T[16],
                        const double m_rel[16], const fiesta_raycast_params *rp, int64_t *n_points) {
   if (!m || !depth || !dp || !T || !rp || rows <= 0 || cols <= 0) { fb_set_error("fiesta_depth_frame: bad argument"); return FIESTA_ERR_INVALID; }
   CK(cudaSetDevice(m->device));
   const size_t N = (size_t)rows * cols;
   if (N > m->d_img[0].cap) {                                               // larger images: new buffers, and no previous image or cloud
-    // d_img[0] is released first and allocated last, so its capacity is 0 until all six buffers hold N pixels: a call that
-    // fails part-way leaves the next call to reallocate them all
-    m->d_img[0] = FbDevBuf<uint16_t>();
-    m->image_cnt = 0; m->last_cloud_n = 0;
-    CK(m->d_img[1].alloc(N)); CK(m->d_dpts.alloc(N * 3)); CK(m->d_dcloud.alloc(N * 3)); CK(m->d_dflags.alloc(N)); CK(m->d_dsel.alloc(N));
-    CK(m->d_img[0].alloc(N));
+    int r = alloc_depth(m, N);
+    if (r) return r;
   }
   if (!m->d_dcount) CK(m->d_dcount.alloc(4));
   ++m->image_cnt;                                                          // Fiesta.h:321-323: img_[image_cnt_ & 1] is the current image
@@ -1974,6 +1992,142 @@ int fiesta_get_slice_marker(fiesta_map *m, int slice, double max_dist, double *x
   if ((r = fb_vis_slice(m->g, m->cobs, slice, max_dist, xyz, rgba, cap, &c, m->stream))) return r;
   m->st.kernel_launches += 3;
   *count = c;
+  return FIESTA_OK;
+}
+
+// ---- map snapshots (format: fb_snapshot.h; kernels: fb_snapshot.cu; DESIGN.md §3.12)
+static FbSnapArrays snap_arrays(fiesta_map *m) {
+  return FbSnapArrays{m->g, m->cobs, m->occ, m->cnt, m->mode == FIESTA_MODE_EXACT ? m->X.LS.p : nullptr};
+}
+// the fiesta_stats counters in snapshot order: every one but kernel_launches (raycast_rounds' slot is not used)
+static int64_t *snap_stat(fiesta_stats &st, int i) {
+  int64_t *f[FB_SNAP_NSTATS] = {&st.occupancy_updates, &st.inserts, &st.deletes, &st.voxels_changed, &st.expansions, &st.voxels_reset,
+                                &st.tile_visits, &st.generations, &st.rays_cast, &st.rays_dropped, &st.ray_voxels, &st.raycast_rounds,
+                                &st.touched_voxels};
+  return f[i];
+}
+static std::vector<unsigned long long> snap_offsets(const FbGeom &g, int exact, const uint32_t *list, size_t n) {
+  std::vector<unsigned long long> off(n + 1);
+  off[0] = 0;
+  for (size_t t = 0; t < n; ++t) off[t + 1] = off[t] + fb_snap_tile_bytes(g.gx, g.gy, g.gz, exact, list[t]);
+  return off;
+}
+int fiesta_snapshot_save(fiesta_map *m, void *buf, int64_t cap, int64_t *size) {
+  const char *fn = "fiesta_snapshot_save";
+  if (!m || !size || cap < 0 || (cap > 0 && !buf)) { fb_set_error("%s: bad argument", fn); return FIESTA_ERR_INVALID; }
+  *size = 0;
+  if (m->n_ev > 0) { fb_set_error("%s: SetOccupancy events are staged (UpdateOccupancy has not run)", fn); return FIESTA_ERR_INVALID; }
+  if (m->n_touch_tiles > 0) { fb_set_error("%s: the occupancy queue is not empty (UpdateOccupancy has not run)", fn); return FIESTA_ERR_INVALID; }
+  if (m->n_ins > 0 || m->n_del > 0) { fb_set_error("%s: inserts or deletes are pending (UpdateESDF has not run)", fn); return FIESTA_ERR_INVALID; }
+  if (m->shard_world > 1) { fb_set_error("%s: an x-slab shard cannot be saved", fn); return FIESTA_ERR_INVALID; }
+  CK(cudaSetDevice(m->device));
+  const FbSnapArrays A = snap_arrays(m);
+  const int exact = m->mode == FIESTA_MODE_EXACT;
+  FbSnapBufs B;
+  unsigned n = 0;
+  int r;
+  if ((r = fb_snap_list_tiles(A, B, &n, m->stream))) return r;
+  m->st.kernel_launches += 2;
+  std::vector<uint32_t> list(n);
+  if (n) {
+    CK(cudaMemcpyAsync(list.data(), B.list, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaStreamSynchronize(m->stream));
+  }
+  const std::vector<unsigned long long> off = snap_offsets(m->g, exact, list.data(), n);
+  const int64_t depth_pixels = m->image_cnt ? (int64_t)m->d_img[0].cap : 0;
+  FbSnapLayout L;
+  fb_snap_layout(n, off[n], depth_pixels, &L);
+  *size = (int64_t)L.total;
+  if (!buf) return FIESTA_OK;                                             // size query
+  if (cap < *size) { fb_set_error("%s: the buffer holds %lld bytes, the snapshot needs %lld", fn, (long long)cap, (long long)*size); return FIESTA_ERR_LIMIT; }
+  uint8_t *p = static_cast<uint8_t *>(buf);
+  int launches = 0;
+  if ((r = fb_snap_pack(A, B, off, p + L.payload_off, m->stream, &launches))) return r;
+  m->st.kernel_launches += launches;
+  memset(p + L.list_off, 0, L.payload_off - L.list_off);
+  for (unsigned t = 0; t < n; ++t) fb_snap_st32(p + L.list_off + 4 * t, list[t]);
+  memset(p + L.depth_off, 0, L.depth_bytes);
+  if (depth_pixels) {
+    CK(cudaMemcpyAsync(p + L.depth_off, m->d_img[m->image_cnt & 1], (size_t)depth_pixels * 2, cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaStreamSynchronize(m->stream));
+  }
+  FbSnapHeader h{};
+  h.version = FB_SNAP_VERSION; h.mode = (uint32_t)m->mode;
+  for (int i = 0; i < 3; ++i) {
+    h.origin[i] = m->cfg.origin[i]; h.map_size[i] = m->cfg.map_size[i];
+    h.min_vec[i] = m->g.min_vec[i]; h.max_vec[i] = m->g.max_vec[i]; h.last_min_vec[i] = m->g.last_min_vec[i]; h.last_max_vec[i] = m->g.last_max_vec[i];
+  }
+  h.resolution = m->cfg.resolution;
+  h.grid[0] = m->g.gx; h.grid[1] = m->g.gy; h.grid[2] = m->g.gz;
+  h.params_set = m->params_set ? 1 : 0;
+  h.l_hit = m->l_hit; h.l_miss = m->l_miss; h.l_min = m->l_min; h.l_max = m->l_max; h.l_occ = m->l_occ;
+  h.flags = m->local_box_seen ? FB_SNAP_LOCAL_BOX_SEEN : 0u;
+  h.image_cnt = m->image_cnt;
+  h.tclock = exact ? m->X.tclock : 0; h.key_base = exact ? m->X.key_base : 0;
+  for (int i = 0; i < FB_SNAP_NSTATS; ++i) h.stats[i] = i == FB_SNAP_STAT_ROUNDS ? 0 : *snap_stat(m->st, i);
+  h.depth_pixels = depth_pixels;
+  h.n_tiles = n;
+  h.list_sum = fb_snap_checksum(p + L.list_off, (L.payload_off - L.list_off) / 8);
+  h.depth_sum = fb_snap_checksum(p + L.depth_off, L.depth_bytes / 8);
+  fb_snap_encode(h, p);
+  return FIESTA_OK;
+}
+int fiesta_snapshot_load(const void *buf, int64_t size, int32_t device, fiesta_map **out) {
+  const char *fn = "fiesta_snapshot_load";
+  if (!out) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  *out = nullptr;
+  if (!buf || size < 0) { fb_set_error("%s: bad argument", fn); return FIESTA_ERR_INVALID; }
+  const uint8_t *p = static_cast<const uint8_t *>(buf);
+  FbSnapHeader h;
+  FbSnapLayout L;
+  char err[256];
+  if (fb_snap_parse(p, size, &h, &L, err, (int)sizeof(err))) { fb_set_error("%s: %s", fn, err); return FIESTA_ERR_INVALID; }
+  fiesta_config cfg{};
+  for (int i = 0; i < 3; ++i) { cfg.origin[i] = h.origin[i]; cfg.map_size[i] = h.map_size[i]; }
+  cfg.resolution = h.resolution; cfg.device = device; cfg.mode = (int32_t)h.mode;
+  fiesta_map *raw = nullptr;
+  int r;
+  if ((r = create_map(&cfg, &raw, false))) return r;                     // the mode is the snapshot's, whatever FIESTA_B200_MODE says
+  std::unique_ptr<fiesta_map, void (*)(fiesta_map *)> m(raw, fiesta_destroy);   // destroyed on any failure below
+  FbGeom &g = m->g;
+  if (g.gx != h.grid[0] || g.gy != h.grid[1] || g.gz != h.grid[2]) { fb_set_error("%s: the rebuilt grid differs from the stored one", fn); return FIESTA_ERR_INVALID; }
+  m->params_set = h.params_set != 0;
+  m->l_hit = h.l_hit; m->l_miss = h.l_miss; m->l_min = h.l_min; m->l_max = h.l_max; m->l_occ = h.l_occ;
+  for (int i = 0; i < 3; ++i) {
+    g.min_vec[i] = h.min_vec[i]; g.max_vec[i] = h.max_vec[i]; g.last_min_vec[i] = h.last_min_vec[i]; g.last_max_vec[i] = h.last_max_vec[i];
+  }
+  set_box_flag(g);
+  m->local_box_seen = (h.flags & FB_SNAP_LOCAL_BOX_SEEN) != 0;
+  if (m->mode == FIESTA_MODE_EXACT) { m->X.tclock = h.tclock; m->X.key_base = h.key_base; }
+  for (int i = 0; i < FB_SNAP_NSTATS; ++i) if (i != FB_SNAP_STAT_ROUNDS) *snap_stat(m->st, i) = h.stats[i];
+  std::vector<uint32_t> list((size_t)h.n_tiles);
+  for (size_t t = 0; t < list.size(); ++t) list[t] = fb_snap_ld32(p + L.list_off + 4 * t);
+  const std::vector<unsigned long long> off = snap_offsets(g, m->mode == FIESTA_MODE_EXACT, list.data(), list.size());
+  FbSnapBufs B;
+  unsigned bad = 0, why = 0;
+  int launches = 0;
+  if ((r = fb_snap_unpack(snap_arrays(m.get()), B, list.data(), off, p + L.payload_off, h.tclock, &bad, &why, m->stream, &launches))) return r;
+  m->st.kernel_launches += launches;
+  if (why) {
+    fb_set_error("%s: stored tile %u (grid tile %u) is malformed:%s%s%s%s%s%s", fn, bad, list[bad], (why & FB_SNAP_BAD_SUM) ? " checksum mismatch;" : "",
+                 (why & FB_SNAP_BAD_COBS) ? " closest-obstacle record outside the grid;" : "", (why & FB_SNAP_BAD_BIT31) ? " bad bit 31 of a record;" : "",
+                 (why & FB_SNAP_BAD_OCC) ? " log-odds not finite;" : "", (why & FB_SNAP_BAD_LS) ? " relink time not below the relink clock;" : "",
+                 (why & FB_SNAP_BAD_CNT) ? " more hits than observations;" : "");
+    return FIESTA_ERR_INVALID;
+  }
+  // rebuilt, not stored: the Exist() bitmap, and FAST mode's staging copy of the records
+  const size_t words = ((size_t)g.ptotal + 31) / 32;
+  k_rebuild_occbits<<<(unsigned)((words + 255) / 256), 256, 0, m->stream>>>(m->occ, g.ptotal, m->l_occ, m->occbits);
+  m->st.kernel_launches++;
+  CK(cudaGetLastError());
+  if (m->mode == FIESTA_MODE_FAST) CK(cudaMemcpyAsync(m->cobs_b, m->cobs, (size_t)g.ptotal * 4, cudaMemcpyDeviceToDevice, m->stream));
+  if (h.depth_pixels > 0) {
+    if ((r = alloc_depth(m.get(), (size_t)h.depth_pixels))) return r;
+    CK(cudaMemcpyAsync(m->d_img[h.image_cnt & 1], p + L.depth_off, (size_t)h.depth_pixels * 2, cudaMemcpyHostToDevice, m->stream));
+  }
+  m->image_cnt = h.image_cnt;
+  CK(cudaStreamSynchronize(m->stream));
+  *out = m.release();
   return FIESTA_OK;
 }
 

@@ -522,6 +522,38 @@ int fiesta_export_closest_obstacle(fiesta_map *m, int *out_xyz);    /* closest_o
 int fiesta_export_occupancy(fiesta_map *m, double *out);            /* occupancy_buffer_ log-odds */
 int fiesta_export_counters(fiesta_map *m, int *num_hit, int *num_total); /* num_hit_, num_miss_ (all observations) */
 
+/* ---- map snapshots: save a map to bytes and load it into a new map that continues bit for bit (DESIGN.md §3.12) ----
+ * fiesta_snapshot_save serialises the map into a self-describing, versioned little-endian byte stream; fiesta_snapshot_load
+ * creates a NEW map from one on `device`.  Continuation guarantee: feed the saved map A and the loaded map B the same calls
+ * afterwards (frames, update boxes, UpdateOccupancy, UpdateESDF, SetParameters, filtered depth frames) and after every call
+ * the exports, every query, GetPointCloud / GetSliceMarker and every fiesta_stats field except kernel_launches, the ms_*
+ * timings and raycast_rounds are equal bit for bit, in both modes (raycast_rounds counts stamp-resolution rounds, which depend
+ * on the order in which concurrent rays claim voxels: two maps fed the same frames can differ in it, so it is not stored); an EXACT map therefore stays bit-identical to the reference.  The stream
+ * carries the mode, and load creates the map in that mode: FIESTA_B200_MODE is ignored by load.  Objects attached to a map
+ * (host mirror, nav fields, frontiers, query plans, shard settings) are not saved; create them again on the loaded map.  The
+ * stream depends only on the map's state: saving a loaded map gives the same bytes.
+ *
+ * Save.  Only a quiescent map can be saved, as it stands after UpdateESDF in the per-frame driver: FIESTA_ERR_INVALID, with
+ * nothing written, while SetOccupancy events are staged, while the occupancy queue is not empty (fiesta_check_update() == 1),
+ * while inserts or deletes are pending (UpdateOccupancy returned 1 and UpdateESDF has not run), and for an x-slab shard
+ * (fiesta_set_shard with world > 1).  *size always receives the stream size when the map can be saved; buf == NULL with cap == 0
+ * only queries it; cap < *size returns FIESTA_ERR_LIMIT and writes nothing.  The source map is not changed.
+ * Load.  FIESTA_ERR_INVALID for anything malformed: a truncated or oversized stream, a bad magic, version or checksum, a
+ * config whose grid differs from the stored one, an update box outside the grid, tiles not strictly ascending or past the grid,
+ * or a voxel word that is not a valid state (a closest-obstacle record outside the grid, bit 31 in a FAST snapshot, a non-finite
+ * log-odds, a relink time not below the stored relink clock); every word is checked on the device before any other kernel can
+ * read it.  FIESTA_ERR_NO_DEVICE / FIESTA_ERR_LIMIT as fiesta_create.  On any failure the new map is destroyed, *out is NULL
+ * and fiesta_last_error() names the reason.
+ * Size.  Only the 8^3 tiles holding anything but the never-observed state are stored: per voxel 20 bytes (FAST) or 28 bytes
+ * (EXACT) plus 8 bytes per stored tile; a map that has seen little of its volume is small, a fully observed 512^3 grid is about
+ * 2.7 GB (FAST) or 3.8 GB (EXACT).
+ * Memory.  Both run through two 16 MB device and two 16 MB pinned staging buffers whatever the grid size, plus per-tile arrays
+ * of at most 8 bytes per 8^3 tile of the grid; neither needs a copy of the grid.  Synchronous. */
+int fiesta_snapshot_save(fiesta_map *m, void *buf, int64_t cap, int64_t *size);
+int fiesta_snapshot_load(const void *buf, int64_t size, int32_t device, fiesta_map **out);
+/* The configuration the map was created with: origin, resolution and map_size as given, the device, and the mode in force. */
+int fiesta_get_config(const fiesta_map *m, fiesta_config *out);
+
 /* ---- multi-GPU: x-slab sharding of UpdateESDF (one process per GPU; the caller moves the ghost layers, e.g. with NCCL) ----
  * Every rank holds the whole grid and integrates every frame identically (ray casting and UpdateOccupancy are replicated),
  * but relaxes only the tile columns of its own x-slab.  dirs_ reaches 2 voxels (parameters.h:66-68), so the ghost layer is 2

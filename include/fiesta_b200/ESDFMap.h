@@ -18,6 +18,8 @@
 
 #include <Eigen/Eigen>
 #include <cmath>
+#include <cstdint>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -40,6 +42,17 @@ class ESDFMap {
 
   static void check(int rc, const char *what) {
     if (rc != FIESTA_OK) throw std::runtime_error(std::string(what) + ": " + fiesta_last_error());
+  }
+  // a map the library created (Load): the geometry comes from the map itself
+  explicit ESDFMap(fiesta_map *h) : h_(h) {
+    fiesta_config cfg;
+    check(fiesta_get_config(h_, &cfg), "fiesta_get_config");
+    resolution_ = cfg.resolution;
+    origin_ = Eigen::Vector3d(cfg.origin[0], cfg.origin[1], cfg.origin[2]);
+    grid_total_size_ = fiesta_grid_total_size(h_);
+    int gs[3];
+    fiesta_grid_size(h_, gs);
+    grid_size_ = Eigen::Vector3i(gs[0], gs[1], gs[2]);
   }
   void Pos2VoxHost(const Eigen::Vector3d &pos, Eigen::Vector3i &vox) const {   // ESDFMap.cpp:74-77
     for (int i = 0; i < 3; ++i) vox(i) = (int)std::floor((pos(i) - origin_(i)) / resolution_);
@@ -69,6 +82,21 @@ class ESDFMap {
   ESDFMap(const ESDFMap &) = delete;
   ESDFMap &operator=(const ESDFMap &) = delete;
   fiesta_map *handle() { return h_; }
+
+  // Map snapshots (fiesta_snapshot_save / fiesta_snapshot_load): a loaded map continues bit for bit like the saved one.  Save
+  // needs a quiescent map (after UpdateESDF in the per-frame driver); Load creates the map in the snapshot's mode.
+  std::vector<uint8_t> Save() {
+    int64_t size = 0;
+    check(fiesta_snapshot_save(h_, nullptr, 0, &size), "Save");
+    std::vector<uint8_t> out((size_t)size);
+    check(fiesta_snapshot_save(h_, out.data(), size, &size), "Save");
+    return out;
+  }
+  static std::unique_ptr<ESDFMap> Load(const void *data, size_t size, int device = 0) {
+    fiesta_map *h = nullptr;
+    check(fiesta_snapshot_load(data, (int64_t)size, device, &h), "Load");
+    return std::unique_ptr<ESDFMap>(new ESDFMap(h));
+  }
 
   // ESDFMap.h:124
   void SetParameters(double p_hit, double p_miss, double p_min, double p_max, double p_occ) {
