@@ -19,10 +19,8 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <vector>
 #include "fb_host.h"     // FbDevBuf, CK
 #include "fb_record.h"   // FB_UNKNOWN / FB_INF / FB_DINF / FB_CODE_MASK, FbGeom, fb_pack / fb_unpack, fb_ii, the distance read
-#include "fb_nav.h"      // FbNavBox (cost-to-go field)
 
 // SMs of an H100 SXM: fixed-size grid-stride launches are sized to a multiple of it.
 #define FB_SMS 132
@@ -178,171 +176,7 @@ cudaError_t fb_esdf_halo_retire(const FbGeom &g, uint32_t *cobs, int x_first, in
 cudaError_t fb_ray_frame(const FbGeom &g, const FbRayArgs &a, int nblocks_resolve, cudaStream_t s, int *launches);
 int fb_ray_resolve_blocks(int device);
 int fb_vis_point_cloud(const FbGeom &g, const double *occ, double l_occ, int zlo, int zhi, float *h_out, long long cap, long long *count, cudaStream_t s);
-cudaError_t fb_segment_clearance(const FbGeom &g, const uint32_t *cobs, const double *ab, long long n, double r, int unknown_blocks,
-                                 int32_t *status, int64_t *hit_idx, double *hit_t, double *min_dist, cudaStream_t s);
 int fb_vis_slice(const FbGeom &g, const uint32_t *cobs, int slice, double max_dist, double *h_xyz, float *h_rgba, long long cap, long long *count, cudaStream_t s);
-// cost-to-go field (fb_nav.cu)
-struct FbNavCtr {
-  unsigned n[3];               // tile work-list lengths, rotating by generation (k_nav_relax)
-  unsigned next[3];            // dynamic tile fetch counters, rotating the same way
-  unsigned generations, pad;
-  unsigned long long goals_placed, blocked, reached, tile_visits;
-};
-struct FbNavArgs {
-  double *D;                   // the field, box layout (fb_nav.h)
-  FbNavBox b;
-  int tn[3];                   // 8^3 tiles per box axis
-  double w[3];                 // res * sqrt(1), res * sqrt(2), res * sqrt(3)
-  uint32_t *stamp;             // per tile: stamp of the generation it is queued for (generation g has stamp g + 1)
-  uint32_t *list[2];           // tile work lists by generation parity
-  FbNavCtr *ctr;
-};
-cudaError_t fb_nav_compute(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, const double *goals, long long n_goals, double r,
-                           int unknown_blocks, int nblocks, cudaStream_t s);
-int fb_nav_relax_blocks(int device);
-// field update (fb_nav.cu, DESIGN.md §3.11)
-struct FbNavUCtr {
-  FbNavCtr wave;               // the withdrawal wave's work lists, generations and tile visits
-  unsigned long long became_blocked, became_free, withdrawn, goals_new;
-  unsigned seed_tiles, pad;
-};
-int fb_nav_withdraw_blocks(int device);
-cudaError_t fb_nav_update(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, uint8_t *flags, FbNavUCtr *u, const double *goals,
-                          long long n_goals, double r, int unknown_blocks, int nblocks, int wblocks, cudaStream_t s);
-cudaError_t fb_nav_paths(const FbGeom &g, const FbNavBox &b, const double *D, const double *w, const double *starts, long long n, int max_len,
-                         int32_t *status, int32_t *len, double *cost, int32_t *vox, cudaStream_t s);
-// cost matrices (fb_navmatrix.cu): up to FB_NAVM_CH sources' fields relaxed together, one channel each
-#define FB_NAVM_CH 32
-struct FbNavMCtr {                 // per pass; zeroed before it
-  unsigned n[3], next[3];          // work-list lengths and fetch counters, rotating by generation as in FbNavCtr
-  unsigned long long mmin[FB_NAVM_CH][3];   // per channel: bits of the least value written in generation g, slot g % 3
-  unsigned queued[FB_NAVM_CH][3];           // per channel: work items queued for generation g, slot g % 3
-  unsigned retired[FB_NAVM_CH];             // the channel's targets are final: its work items are dropped
-};
-struct FbNavMTot {                 // summed over the passes of a call
-  unsigned long long generations, tile_visits, retired_early;
-};
-struct FbNavMArgs {
-  double *D;                       // [channel][box index] (fb_nav.h layout); +inf until reached
-  const uint32_t *M;               // per box voxel: fb_nav_move_bits
-  FbNavBox b;
-  int tn[3];                       // 8^3 tiles per box axis
-  unsigned nt;                     // tiles per channel; a work item is channel * nt + tile
-  long long nv;                    // box voxels
-  double w[3];
-  uint32_t *stamp;                 // per work item: stamp of the generation it is queued for (generation g has stamp g + 1)
-  uint32_t *list[2];               // work lists by generation parity
-  FbNavMCtr *ctr;
-  FbNavMTot *tot;
-  const long long *tgt;            // box indices of the status-0 targets
-  int n_tgt, nch;                  // status-0 targets, channels of this pass
-};
-int fb_navm_relax_blocks(int device);
-cudaError_t fb_navm_locate(const FbGeom &g, const uint32_t *cobs, const FbNavBox &b, double r, int unknown_blocks, uint32_t *M,
-                           const double *pts, long long n, int32_t *status, long long *idx, cudaStream_t s);
-cudaError_t fb_navm_pass(const FbNavMArgs &a, const long long *src_idx, int nblocks, cudaStream_t s);
-cudaError_t fb_navm_gather(const double *D, long long nv, const int32_t *rows, long long n_rows, const long long *tgt_idx, long long n_tgt,
-                           double *cost, cudaStream_t s);
-// frontier extraction (fb_frontier.cu)
-struct FbFrCtr {
-  unsigned long long frontier;     // frontier voxels of the box
-  unsigned long long roots;        // clusters before the size filter
-  unsigned long long kept_voxels;  // members of the kept clusters
-  unsigned sel[3];                 // CUB selection counts: roots, kept clusters, kept members
-  unsigned pad;
-};
-struct FbFrBufs {                  // device buffers of one fiesta_frontiers object, grown by fb_frontier_compute
-  FbDevBuf<uint32_t> P;            // box: union-find parent words (FR_NONE off the frontier)
-  FbDevBuf<int32_t> L;             // box: cluster label, -1 elsewhere (fiesta_frontiers_export)
-  // per cluster before the size filter (C of them): root box index, size, kept ids in order, pre-filter id -> kept id or -1,
-  // grid-coordinate sums [3C], bounding boxes [lo 3C][hi 3C]
-  FbDevBuf<uint32_t> roots, size, kept;
-  FbDevBuf<int32_t> newid, box;
-  FbDevBuf<unsigned long long> sum;
-  // outputs per kept cluster, at pre-filter capacity C: size, [rep 3C][bbox lo 3C][bbox hi 3C], centroid [3C]
-  FbDevBuf<int64_t> o_size;
-  FbDevBuf<int32_t> o_i32;
-  FbDevBuf<double> o_cen;
-  // per member: sort keys and box indices (double-buffered), then the grid xyz of the sorted members
-  FbDevBuf<uint32_t> mkey[2], mval[2];
-  FbDevBuf<int32_t> m_xyz;
-  FbDevBuf<char> tmp;              // CUB temporary storage
-  FbDevBuf<FbFrCtr> ctr;
-  FbHostBuf<FbFrCtr> h_ctr;
-  unsigned C = 0;                  // pre-filter clusters of the last compute: the stride of o_i32
-};
-int fb_frontier_compute(const FbGeom &g, const uint32_t *cobs, const double *occ, double l_occ, const FbNavBox &b, double r,
-                        long long min_size, FbFrBufs &B, cudaStream_t s, int *launches);
-// viewpoint coverage of frontier clusters (fb_view.cu)
-struct FbViewCtr {
-  unsigned long long scored, walked, visible;   // status-0 candidates, pairs in range and view, walked pairs with a clear line of sight
-};
-struct FbViewBufs {                // device buffers of fiesta_frontiers_score_viewpoints, kept on the frontier object
-  FbDevBuf<double> pos;            // per candidate: position [3n]
-  FbDevBuf<int32_t> cl, status;    //                cluster id, status
-  FbDevBuf<long long> work;        //                [n + 1] chunk counts, scanned in place to each one's first chunk (work[n]: total)
-  FbDevBuf<int32_t> score;         //                [n * n_orient]
-  FbDevBuf<long long> moff;        // per kept cluster: its first member in the member list
-  FbDevBuf<double> orient;         // [9 * n_orient]
-  FbDevBuf<FbViewCtr> ctr;
-  FbHostBuf<FbViewCtr> h_ctr;
-};
-// Expects V.pos / cl / orient filled for n >= 1 candidates and V.score / ctr zeroed; size / m_xyz are the frontier result's.
-int fb_view_score(const FbGeom &g, const uint32_t *cobs, const int64_t *size, const int32_t *m_xyz, unsigned K, FbViewBufs &V,
-                  FbDevBuf<char> &tmp, long long n, int n_orient, const fiesta_sensor_model &sm, double clearance, int unknown_blocks,
-                  cudaStream_t s, int *launches);
-// safe flight corridors (fb_corridor.cu); L_lo / L_hi: the limit box, inclusive grid voxels
-struct FbCorrCtr {
-  unsigned long long boxes, tested, grown;   // boxes written (seeds inflated), layer tests, grown layers
-};
-struct FbCorrBufs {                // device buffers of fiesta_inflate_boxes / fiesta_corridors, kept on the map
-  FbDevBuf<uint32_t> mask;         // the limit box's traversable bits, z-rows then y-rows (fb_corridor.h)
-  FbDevBuf<int32_t> in;            // seeds [lo 3n][hi 3n], or path voxels [3 total]
-  FbDevBuf<int64_t> off;           // path offsets [n_paths + 1]
-  FbDevBuf<int32_t> out;           // seeds: [status n][lo 3n][hi 3n]; paths: [status][n_boxes][blocked_at] x n_paths, [lo 3T][hi 3T][first T]
-  FbDevBuf<FbCorrCtr> ctr;
-  FbHostBuf<FbCorrCtr> h_ctr;
-};
-cudaError_t fb_corr_launch_mask(const FbGeom &g, const uint32_t *cobs, const int *L_lo, const int *L_hi, double r, int unknown_blocks,
-                                uint32_t *mask, cudaStream_t s);
-cudaError_t fb_corr_launch_seeds(const int *L_lo, const int *L_hi, const int *max_steps, const uint32_t *mask, const int32_t *seeds,
-                                 long long n, int32_t *status, int32_t *out_lo, int32_t *out_hi, FbCorrCtr *ctr, cudaStream_t s);
-cudaError_t fb_corr_launch_paths(const int *L_lo, const int *L_hi, const int *max_steps, const uint32_t *mask, const int32_t *P,
-                                 const int64_t *off, long long n_paths, int32_t *status, int32_t *n_boxes, int32_t *blocked_at,
-                                 int32_t *box_lo, int32_t *box_hi, int32_t *first, FbCorrCtr *ctr, cudaStream_t s);
-// robot-shaped collision checks (fb_pose.cu)
-struct FbPoseBufs {                // device buffers of fiesta_check_poses(_device), kept on the map
-  FbDevBuf<char> io;               // host form: [poses 12n][hit_idx n] 8-byte words, [status n][n_blocked n] int32
-  FbDevBuf<long long> work;        // [n + 1] chunk counts, scanned in place to each pose's first work item (work[n]: total)
-  FbDevBuf<char> tmp;              // CUB temporary storage
-};
-// Expects a validated call (fb_pose.h limits) with n >= 0; writes status / n_blocked / hit_idx, device pointers, on stream s.
-int fb_pose_check_batch(const FbGeom &g, const uint32_t *cobs, const double *poses, long long n, const double *h, double clearance,
-                        int unknown_blocks, int32_t *status, int32_t *n_blocked, int64_t *hit_idx, FbPoseBufs &B, cudaStream_t s,
-                        int *launches);
-// map snapshots (fb_snapshot.cu; format in fb_snapshot.h)
-#define FB_SNAP_STAGE (16u << 20)  // bytes of each of the two device and two pinned staging buffers of a save or load
-struct FbSnapArrays {              // the per-voxel state a snapshot carries; LS is null in FAST mode
-  FbGeom g;
-  uint32_t *cobs;
-  double *occ;
-  unsigned long long *cnt, *LS;
-};
-struct FbSnapBufs {                // per-tile scratch of one save or load
-  FbDevBuf<uint8_t> flag;          // per grid tile: holds non-default state
-  FbDevBuf<uint32_t> list, d_n;    // stored tiles ascending; selection count, or {first bad tile, reasons} on load
-  FbDevBuf<unsigned long long> off;  // per stored tile: payload offset, and the end
-  FbHostBuf<uint32_t> h_n;
-  FbDevBuf<char> tmp;              // CUB temporary storage
-};
-// Lists the tiles with non-default state into B.list (ascending) and their count into *n.
-int fb_snap_list_tiles(const FbSnapArrays &A, FbSnapBufs &B, unsigned *n, cudaStream_t s);
-// Payload of the B.list tiles, whose offsets (and the end) are `off`, written to host memory dst + off[t].
-int fb_snap_pack(const FbSnapArrays &A, FbSnapBufs &B, const std::vector<unsigned long long> &off, uint8_t *dst, cudaStream_t s, int *launches);
-// Scatters the payload at src + off[t] of the h_list tiles into A; *bad_tile = the first tile position that failed validation
-// (0xffffffff: none), *reasons = the FB_SNAP_BAD_* bits.
-int fb_snap_unpack(const FbSnapArrays &A, FbSnapBufs &B, const uint32_t *h_list, const std::vector<unsigned long long> &off, const uint8_t *src,
-                   unsigned long long tclock, unsigned *bad_tile, unsigned *reasons, cudaStream_t s, int *launches);
 struct FbDepthRel { double m[16]; };
 struct fiesta_depth_params;
 cudaError_t fb_depth_to_cloud(const uint16_t *d_img, const uint16_t *d_last, int rows, int cols, const fiesta_depth_params &p, int filter_on,

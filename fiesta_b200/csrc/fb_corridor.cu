@@ -13,11 +13,15 @@
 // Every output is a function of the masks and the sequential rule, and the statistics are integer sums: nothing depends on the
 // schedule.
 #include <algorithm>
-#include "fb_common.cuh"
+#include "fb_map.h"
 #include "fb_corridor.h"
 
 #define CORR_WARPS 8
 #define CORR_BATCH 4
+
+struct FbCorrCtr {
+  unsigned long long boxes, tested, grown;   // boxes written (seeds inflated), layer tests, grown layers
+};
 
 __global__ void k_corr_mask(FbGeom g, const uint32_t *__restrict__ cobs, FbCorrMask M, double r, int unknown_blocks, uint32_t *mask) {
   const int lane = threadIdx.x & 31;
@@ -166,32 +170,121 @@ __global__ void __launch_bounds__(32 * CORR_WARPS) k_corr_chain(FbCorrMask M, co
   corr_count(ctr, acc.lane, (unsigned long long)nb, c);
 }
 
-// ---------------------------------------------------------------- host side
-cudaError_t fb_corr_launch_mask(const FbGeom &g, const uint32_t *cobs, const int *L_lo, const int *L_hi, double r, int unknown_blocks,
-                                uint32_t *mask, cudaStream_t s) {
-  const FbCorrMask M = fb_corr_mask_geom(L_lo, L_hi);
+// ---------------------------------------------------------------- entry points (include/fiesta_b200.h)
+static bool corridor_args_ok(const char *fn, const fiesta_map *m, const int *box_lo, const int *box_hi, const int32_t *max_steps,
+                             int64_t n, double clearance, int flags, bool buffers) {
+  if (!m || !box_lo || !box_hi || !max_steps) { fb_set_error("%s: null argument", fn); return false; }
+  if (!count_buffers_ok(fn, n, buffers) || !clearance_flags_ok(fn, clearance, flags)) return false;
+  for (int k = 0; k < 3; ++k) {                                           // per axis: the box, then its max_steps
+    if (!box_axis_ok(fn, m->g, box_lo, box_hi, k)) return false;
+    if (max_steps[k] < 0) { fb_set_error("%s: max_steps must be >= 0", fn); return false; }
+  }
+  return true;
+}
+// Grow the buffers, then record the start event and build the limit box's masks (2 launches).
+static int corridor_begin(fiesta_map *m, const char *fn, const int *box_lo, const int *box_hi, double clearance, int flags,
+                          size_t in_words, size_t off_words, size_t out_words) {
+  FbCorrBufs &B = m->corr;
+  const FbCorrMask M = fb_corr_mask_geom(box_lo, box_hi);
+  const cudaStream_t s = m->stream;
+  CK(cudaSetDevice(m->device));
+  cudaError_t e = B.mask.grow((size_t)fb_corr_mask_words(M), s);
+  if (e == cudaSuccess) e = B.in.grow(in_words, s);
+  if (e == cudaSuccess && off_words) e = B.off.grow(off_words, s);
+  if (e == cudaSuccess) e = B.out.grow(out_words, s);
+  if (e == cudaSuccess) e = B.ctr.grow(1, s);
+  if (e == cudaSuccess && !B.h_ctr) e = B.h_ctr.alloc(1);
+  if (e != cudaSuccess) return alloc_failed(e, "%s: cannot allocate the buffers", fn);
+  CK(cudaEventRecord(m->ev[0], s));
+  CK(cudaMemsetAsync(B.ctr, 0, sizeof(FbCorrCtr), s));
   const long long ywords = fb_corr_mask_words(M) - M.zwords;
   const long long cap = (long long)FB_SMS * 64;                          // blocks of 8 warps, grid-stride beyond
-  k_corr_mask<<<(unsigned)std::min((M.zwords + 7) / 8, cap), 256, 0, s>>>(g, cobs, M, r, unknown_blocks, mask);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  k_corr_transpose<<<(unsigned)std::min((ywords + 7) / 8, cap), 256, 0, s>>>(M, mask);
-  return cudaGetLastError();
+  k_corr_mask<<<(unsigned)std::min((M.zwords + 7) / 8, cap), 256, 0, s>>>(m->g, m->cobs, M, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS,
+                                                                           B.mask);
+  CK(cudaGetLastError());
+  k_corr_transpose<<<(unsigned)std::min((ywords + 7) / 8, cap), 256, 0, s>>>(M, B.mask);
+  CK(cudaGetLastError());
+  m->st.kernel_launches += 2;
+  return FIESTA_OK;
 }
-
-cudaError_t fb_corr_launch_seeds(const int *L_lo, const int *L_hi, const int *max_steps, const uint32_t *mask, const int32_t *seeds,
-                                 long long n, int32_t *status, int32_t *out_lo, int32_t *out_hi, FbCorrCtr *ctr, cudaStream_t s) {
-  const FbCorrMask M = fb_corr_mask_geom(L_lo, L_hi);
+// After the copies out have been enqueued: synchronise and fill the statistics.
+static int corridor_end(fiesta_map *m, const int *box_lo, const int *box_hi, fiesta_corridor_stats *stats) {
+  FbCorrBufs &B = m->corr;
+  CK(cudaEventRecord(m->ev[1], m->stream));
+  CK(cudaMemcpyAsync(B.h_ctr, B.ctr, sizeof(FbCorrCtr), cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  if (stats) {
+    *stats = fiesta_corridor_stats{};
+    stats->boxes = (int64_t)B.h_ctr->boxes;
+    stats->layers_tested = (int64_t)B.h_ctr->tested;
+    stats->layers_grown = (int64_t)B.h_ctr->grown;
+    stats->mask_voxels = 1;
+    for (int k = 0; k < 3; ++k) stats->mask_voxels *= (int64_t)(box_hi[k] - box_lo[k] + 1);
+    CK(cudaEventElapsedTime(&stats->ms_compute, m->ev[0], m->ev[1]));
+  }
+  return FIESTA_OK;
+}
+int fiesta_inflate_boxes(fiesta_map *m, const int box_lo[3], const int box_hi[3], const int32_t *seed_lo_xyz, const int32_t *seed_hi_xyz,
+                         int64_t n, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *out_lo_xyz,
+                         int32_t *out_hi_xyz, fiesta_corridor_stats *stats) {
+  const char *fn = "fiesta_inflate_boxes";
+  if (!corridor_args_ok(fn, m, box_lo, box_hi, max_steps, n, clearance, flags, seed_lo_xyz && seed_hi_xyz && status && out_lo_xyz && out_hi_xyz))
+    return FIESTA_ERR_INVALID;
+  if (n >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 seeds per call", fn); return FIESTA_ERR_LIMIT; }
+  if (stats) *stats = fiesta_corridor_stats{};
+  if (n == 0) return FIESTA_OK;
+  int r;
+  if ((r = corridor_begin(m, fn, box_lo, box_hi, clearance, flags, (size_t)n * 6, 0, (size_t)n * 7))) return r;
+  FbCorrBufs &B = m->corr;
+  const cudaStream_t s = m->stream;
+  int32_t *d_st = B.out, *d_lo = d_st + n, *d_hi = d_lo + 3 * n;
+  CK(cudaMemcpyAsync(B.in, seed_lo_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(B.in + 3 * n, seed_hi_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, s));
   k_corr_inflate<<<(unsigned)((n + CORR_WARPS - 1) / CORR_WARPS), 32 * CORR_WARPS, 0, s>>>(
-      M, mask, make_int3(max_steps[0], max_steps[1], max_steps[2]), seeds, n, status, out_lo, out_hi, ctr);
-  return cudaGetLastError();
+      fb_corr_mask_geom(box_lo, box_hi), B.mask, make_int3(max_steps[0], max_steps[1], max_steps[2]), B.in, n, d_st, d_lo, d_hi, B.ctr);
+  CK(cudaGetLastError());
+  m->st.kernel_launches++;
+  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out_lo_xyz, d_lo, (size_t)n * 12, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out_hi_xyz, d_hi, (size_t)n * 12, cudaMemcpyDeviceToHost, s));
+  return corridor_end(m, box_lo, box_hi, stats);
 }
-
-cudaError_t fb_corr_launch_paths(const int *L_lo, const int *L_hi, const int *max_steps, const uint32_t *mask, const int32_t *P,
-                                 const int64_t *off, long long n_paths, int32_t *status, int32_t *n_boxes, int32_t *blocked_at,
-                                 int32_t *box_lo, int32_t *box_hi, int32_t *first, FbCorrCtr *ctr, cudaStream_t s) {
-  const FbCorrMask M = fb_corr_mask_geom(L_lo, L_hi);
+int fiesta_corridors(fiesta_map *m, const int box_lo[3], const int box_hi[3], const int32_t *path_vox_xyz, const int64_t *path_off,
+                     int64_t n_paths, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *n_boxes,
+                     int32_t *blocked_at, int32_t *box_lo_xyz, int32_t *box_hi_xyz, int32_t *first, fiesta_corridor_stats *stats) {
+  const char *fn = "fiesta_corridors";
+  if (!corridor_args_ok(fn, m, box_lo, box_hi, max_steps, n_paths, clearance, flags, path_off && status && n_boxes && blocked_at))
+    return FIESTA_ERR_INVALID;
+  if (n_paths > 0 && path_off[0] != 0) { fb_set_error("%s: path_off[0] must be 0", fn); return FIESTA_ERR_INVALID; }
+  for (int64_t p = 0; p < n_paths; ++p)
+    if (path_off[p + 1] < path_off[p]) { fb_set_error("%s: path_off decreases at %lld", fn, (long long)p); return FIESTA_ERR_INVALID; }
+  const int64_t total = n_paths > 0 ? path_off[n_paths] : 0;
+  if (total > 0 && !(path_vox_xyz && box_lo_xyz && box_hi_xyz && first)) { fb_set_error("%s: null buffer", fn); return FIESTA_ERR_INVALID; }
+  if (total >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 path voxels per call", fn); return FIESTA_ERR_LIMIT; }
+  if (stats) *stats = fiesta_corridor_stats{};
+  if (total == 0) {                                                       // only empty paths: status 0, no boxes
+    for (int64_t p = 0; p < n_paths; ++p) { status[p] = FB_CORR_OK; n_boxes[p] = 0; blocked_at[p] = -1; }
+    return FIESTA_OK;
+  }
+  const size_t T = (size_t)total, np = (size_t)n_paths;
+  int r;
+  if ((r = corridor_begin(m, fn, box_lo, box_hi, clearance, flags, T * 3, np + 1, np * 3 + T * 7))) return r;
+  FbCorrBufs &B = m->corr;
+  const cudaStream_t s = m->stream;
+  int32_t *d_st = B.out, *d_nb = d_st + np, *d_bl = d_nb + np, *d_lo = d_bl + np, *d_hi = d_lo + 3 * T, *d_first = d_hi + 3 * T;
+  CK(cudaMemcpyAsync(B.in, path_vox_xyz, T * 12, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(B.off, path_off, (np + 1) * 8, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(d_lo, 0xff, T * 28, s));                            // -1 in every slot no box is written to
   k_corr_chain<<<(unsigned)((n_paths + CORR_WARPS - 1) / CORR_WARPS), 32 * CORR_WARPS, 0, s>>>(
-      M, mask, make_int3(max_steps[0], max_steps[1], max_steps[2]), P, off, n_paths, status, n_boxes, blocked_at, box_lo, box_hi, first, ctr);
-  return cudaGetLastError();
+      fb_corr_mask_geom(box_lo, box_hi), B.mask, make_int3(max_steps[0], max_steps[1], max_steps[2]), B.in, B.off, n_paths, d_st, d_nb, d_bl,
+      d_lo, d_hi, d_first, B.ctr);
+  CK(cudaGetLastError());
+  m->st.kernel_launches++;
+  CK(cudaMemcpyAsync(status, d_st, np * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(n_boxes, d_nb, np * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(blocked_at, d_bl, np * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(box_lo_xyz, d_lo, T * 12, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(box_hi_xyz, d_hi, T * 12, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(first, d_first, T * 4, cudaMemcpyDeviceToHost, s));
+  return corridor_end(m, box_lo, box_hi, stats);
 }

@@ -19,7 +19,7 @@
 // in.  Everything after that is ordered compaction, integer atomics and a stable sort, and the centroid is one fp64 expression.
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
-#include "fb_common.cuh"
+#include "fb_frontier.cuh"
 #include "fb_frontier.h"
 
 #define FR_THREADS 512          // one thread per voxel of an 8^3 tile
@@ -248,11 +248,7 @@ static unsigned fr_grid(unsigned long long n) { return (unsigned)((n + 255) / 25
 #define FR_GROW(buf, n)                                                                                                  \
   do {                                                                                                                 \
     const cudaError_t e_ = (buf).grow((size_t)(n), s);                                                                 \
-    if (e_ != cudaSuccess) {                                                                                           \
-      cudaGetLastError();                                   /* not sticky: later calls must not see it */                \
-      fb_set_error("fiesta_frontiers_compute: cannot allocate %zu elements: %s", (size_t)(n), cudaGetErrorString(e_)); \
-      return FIESTA_ERR_CUDA;                                                                                          \
-    }                                                                                                                  \
+    if (e_ != cudaSuccess) return alloc_failed(e_, "fiesta_frontiers_compute: cannot allocate %zu elements", (size_t)(n));     \
   } while (0)
 
 // One CUB call with temporary storage from B.tmp (grown as needed).
@@ -272,8 +268,8 @@ static int fr_read_ctr(FbFrBufs &B, cudaStream_t s) {
   return FIESTA_OK;
 }
 
-int fb_frontier_compute(const FbGeom &g, const uint32_t *cobs, const double *occ, double l_occ, const FbNavBox &b, double r,
-                        long long min_size, FbFrBufs &B, cudaStream_t s, int *launches) {
+static int frontier_compute(const FbGeom &g, const uint32_t *cobs, const double *occ, double l_occ, const FbNavBox &b, double r,
+                            long long min_size, FbFrBufs &B, cudaStream_t s, int *launches) {
   const long long nv = fr_total(b);
   const int tn[3] = {(b.n[0] + FB_TILE - 1) / FB_TILE, (b.n[1] + FB_TILE - 1) / FB_TILE, (b.n[2] + FB_TILE - 1) / FB_TILE};
   const unsigned nt = (unsigned)(tn[0] * tn[1] * tn[2]);
@@ -338,5 +334,93 @@ int fb_frontier_compute(const FbGeom &g, const uint32_t *cobs, const double *occ
   k_fr_members<<<fr_grid(M), 256, 0, s>>>(b, B.mval[1], (unsigned)M, B.m_xyz);
   CK(cudaGetLastError());
   *launches += 5;
+  return FIESTA_OK;
+}
+
+// ---------------------------------------------------------------- entry points (include/fiesta_b200.h)
+void fiesta_frontiers_destroy(fiesta_frontiers *f) { handle_destroy(f); }
+int fiesta_frontiers_create(fiesta_map *m, fiesta_frontiers **out) {
+  if (!m || !out) { fb_set_error("fiesta_frontiers_create: null argument"); return FIESTA_ERR_INVALID; }
+  *out = nullptr;
+  FbHandle<fiesta_frontiers> f;
+  int r;
+  if ((r = handle_new(m, f))) return r;
+  if (!f) { fb_set_error("out of host memory"); return FIESTA_ERR_INVALID; }
+  for (cudaEvent_t &e : f->ev) CK(cudaEventCreate(&e));
+  CK(f->B.ctr.alloc(1));
+  CK(f->B.h_ctr.alloc(1));
+  *out = f.release();
+  return FIESTA_OK;
+}
+int fiesta_frontiers_compute(fiesta_frontiers *f, const int box_lo[3], const int box_hi[3], double clearance, int64_t min_cluster_size,
+                             fiesta_frontier_stats *stats) {
+  const char *fn = "fiesta_frontiers_compute";
+  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (!clearance_flags_ok(fn, clearance, 0)) return FIESTA_ERR_INVALID;
+  if (min_cluster_size < 1) { fb_set_error("%s: min_cluster_size must be >= 1", fn); return FIESTA_ERR_INVALID; }
+  fiesta_map *m = f->m;
+  FbNavBox b{};
+  if (!box_arg(fn, m->g, box_lo, box_hi, &b)) return FIESTA_ERR_INVALID;
+  CK(cudaSetDevice(m->device));
+  f->valid = false;
+  int launches = 0;
+  CK(cudaEventRecord(f->ev[0], m->stream));
+  const int r = frontier_compute(m->g, m->cobs, m->occ, m->l_occ, b, clearance, (long long)min_cluster_size, f->B, m->stream, &launches);
+  m->st.kernel_launches += launches;
+  if (r != FIESTA_OK) return r;
+  CK(cudaEventRecord(f->ev[1], m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  const FbFrCtr &c = *f->B.h_ctr;
+  f->st = fiesta_frontier_stats{};
+  f->st.box_voxels = (int64_t)b.n[0] * b.n[1] * b.n[2];
+  f->st.frontier_voxels = (int64_t)c.frontier;
+  f->st.clusters = (int64_t)c.roots;
+  f->st.kept_clusters = (int64_t)c.sel[1];
+  f->st.kept_voxels = (int64_t)c.kept_voxels;
+  CK(cudaEventElapsedTime(&f->st.ms_compute, f->ev[0], f->ev[1]));
+  f->box = b;
+  f->valid = true;
+  if (stats) *stats = f->st;
+  return FIESTA_OK;
+}
+int fiesta_frontiers_clusters(const fiesta_frontiers *f, int64_t cap, int64_t *size, int32_t *rep_xyz, int32_t *bbox_lo_xyz,
+                              int32_t *bbox_hi_xyz, double *centroid_xyz) {
+  const char *fn = "fiesta_frontiers_clusters";
+  if (!f || cap < 0 || (cap > 0 && !(size && rep_xyz && bbox_lo_xyz && bbox_hi_xyz && centroid_xyz))) {
+    fb_set_error("%s: null buffer or negative capacity", fn);
+    return FIESTA_ERR_INVALID;
+  }
+  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
+  const size_t n = (size_t)(cap < f->st.kept_clusters ? cap : f->st.kept_clusters), C = f->B.C;
+  if (n == 0) return FIESTA_OK;
+  const fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  CK(cudaMemcpyAsync(size, f->B.o_size, n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(rep_xyz, f->B.o_i32, n * 12, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(bbox_lo_xyz, f->B.o_i32 + 3 * C, n * 12, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(bbox_hi_xyz, f->B.o_i32 + 6 * C, n * 12, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(centroid_xyz, f->B.o_cen, n * 24, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+int fiesta_frontiers_voxels(const fiesta_frontiers *f, int64_t cap, int32_t *vox_xyz) {
+  const char *fn = "fiesta_frontiers_voxels";
+  if (!f || cap < 0 || (cap > 0 && !vox_xyz)) { fb_set_error("%s: null buffer or negative capacity", fn); return FIESTA_ERR_INVALID; }
+  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
+  const size_t n = (size_t)(cap < f->st.kept_voxels ? cap : f->st.kept_voxels);
+  if (n == 0) return FIESTA_OK;
+  const fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  CK(cudaMemcpyAsync(vox_xyz, f->B.m_xyz, n * 12, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+int fiesta_frontiers_export(const fiesta_frontiers *f, int32_t *labels) {
+  if (!f || !labels) { fb_set_error("fiesta_frontiers_export: null argument"); return FIESTA_ERR_INVALID; }
+  if (!f->valid) { fb_set_error("fiesta_frontiers_export: no frontiers have been computed"); return FIESTA_ERR_INVALID; }
+  const fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  CK(cudaMemcpyAsync(labels, f->B.L, (size_t)f->st.box_voxels * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
   return FIESTA_OK;
 }

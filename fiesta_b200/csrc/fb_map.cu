@@ -10,17 +10,12 @@
 #include <stdlib.h>
 #include <string.h>
 #include <string>
-#include <algorithm>
 #include <memory>
 #include <new>
-#include <vector>
-#include "../../include/fiesta_b200.h"
-#include "fb_common.cuh"
-#include "fb_exact.h"
+#include "fb_map.h"
+#include "fb_nav.h"
 #include "fb_segment.h"
-#include "fb_corridor.h"
 #include "fb_pose.h"
-#include "fb_snapshot.h"
 
 static thread_local std::string g_last_error;
 void fb_set_error(const char *fmt, ...) {
@@ -32,69 +27,6 @@ void fb_set_error(const char *fmt, ...) {
   g_last_error = buf;
 }
 
-struct fiesta_map {
-  FbGeom g{};
-  fiesta_config cfg{};              // as given at create, with the device and the mode in force (fiesta_get_config, snapshots)
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  bool params_set = false;
-  double l_hit = 0, l_miss = 0, l_min = 0, l_max = 0, l_occ = 0;
-  double l_cornor[3]{}, r_cornor[3]{};
-  // per-voxel state
-  FbDevBuf<uint32_t> cobs, cobs_b, stamp[2], occbits;
-  FbDevBuf<double> occ;
-  FbDevBuf<unsigned long long> cnt;
-  // tiles
-  FbDevBuf<uint32_t> tile_flag, nb_flag, list[2], changed[2], changed_bbox[2];
-  CUtensorMap tmap{};
-  int wf_blocks = 0, rr_blocks = 0;
-  // queues
-  FbDevBuf<uint32_t> touch_flag, touch_list;
-  unsigned touch_epoch = 0;
-  FbDevBuf<uint32_t> ins, del;
-  unsigned n_touch_tiles = 0, n_ins = 0, n_del = 0;  // host view (valid after the last sync)
-  FbDevBuf<FbCounters> d_ctr;
-  FbHostBuf<FbCounters> h_ctr;
-  // per-call SetOccupancy staging
-  FbHostBuf<uint32_t> h_ev;
-  FbDevBuf<uint32_t> d_ev;
-  size_t n_ev = 0;
-  // ray casting
-  FbDevBuf<float> d_xyz;
-  FbDevBuf<uint32_t> ray_list;
-  FbDevBuf<int> ray_len, ray_reach;
-  FbDevBuf<unsigned> ray_dirty;
-  unsigned frame_tag = 0, owner_tag = 0;
-  // queries
-  FbDevBuf<double> d_qin, d_qout;
-  FbDevBuf<char> d_seg;             // fiesta_check_segments: [ab 6n][hit_t n][min_dist n] doubles, [hit_idx n] int64, [status n] int32
-  FbCorrBufs corr;                  // fiesta_inflate_boxes / fiesta_corridors
-  FbPoseBufs pose;                  // fiesta_check_poses / fiesta_check_poses_device
-  cudaEvent_t ev[4] = {};
-  cudaEvent_t ev_q[2] = {};         // device queries: map stream -> caller's stream, and back
-  FbDevBuf<unsigned long long> d_dbg;
-  // depth front end (next #1)
-  FbDevBuf<uint16_t> d_img[2];
-  unsigned image_cnt = 0;
-  FbDevBuf<float> d_dpts, d_dcloud;
-  FbDevBuf<uint8_t> d_dflags;
-  FbDevBuf<uint32_t> d_dsel;
-  FbDevBuf<unsigned> d_dcount;
-  FbDevBuf<char> d_dtmp;
-  unsigned last_cloud_n = 0;
-  int mode = FIESTA_MODE_EXACT;
-  int shard_rank = 0, shard_world = 1, tile_x_lo = 0, tile_x_hi = 0;
-  FbDevBuf<unsigned> d_halo_changed;
-  // FAST mode: some relaxation (UpdateESDF / shard_relax) ran under an update box that is not the whole grid, so voxels
-  // outside it may hold values their neighbours never offered them; from then on every queued voxel pulls (DESIGN 3.3)
-  bool local_box_seen = false;
-  FbExact X;
-  fiesta_stats st{};
-  // pinned host mirror (next #3): union of the update boxes that were current while records could change
-  struct fiesta_host_mirror *mirror = nullptr;
-  int dirty_lo[3]{}, dirty_hi[3]{};
-  bool dirty_any = false, pending_obs = false;  // pending_obs: observations counted under the current box and not integrated yet
-};
 static void mark_dirty(fiesta_map *m) {                                   // tracked without a mirror too: events staged before a mirror is
   const FbGeom &g = m->g;                                                   // created are integrated after it
   for (int i = 0; i < 3; ++i) {
@@ -296,7 +228,7 @@ __global__ void k_query(FbGeom g, const uint32_t *cobs, const double *occ, doubl
 }
 
 // ====================================================================== host helpers
-static void set_box_flag(FbGeom &g) {
+void set_box_flag(FbGeom &g) {
   g.box_is_full = g.min_vec[0] == 0 && g.min_vec[1] == 0 && g.min_vec[2] == 0 && g.max_vec[0] == g.gx - 1 &&
                   g.max_vec[1] == g.gy - 1 && g.max_vec[2] == g.gz - 1;
 }
@@ -332,7 +264,7 @@ static int fetch_counters(fiesta_map *m) {
   if (m->mode == FIESTA_MODE_FAST) { m->n_ins = m->h_ctr->n_ins; m->n_del = m->h_ctr->n_del; }
   return FIESTA_OK;
 }
-static int flush_events(fiesta_map *m) {
+int flush_events(fiesta_map *m) {
   if (m->n_ev == 0) return FIESTA_OK;
   CK(cudaMemcpyAsync(m->d_ev, m->h_ev, m->n_ev * sizeof(uint32_t), cudaMemcpyHostToDevice, m->stream));
   if (m->mode == FIESTA_MODE_EXACT && m->X.key_base + m->n_ev >= FB_KEY_MASK) { fb_set_error("more than 2^44 observations between two UpdateOccupancy calls"); return FIESTA_ERR_LIMIT; }
@@ -363,8 +295,6 @@ static inline int host_set_occupancy_vox(fiesta_map *m, const int *v, int occ, i
 }
 
 // ====================================================================== C ABI
-extern "C" {
-
 const char *fiesta_last_error(void) { return g_last_error.c_str(); }
 
 void fiesta_host_mirror_destroy(struct fiesta_host_mirror *p);
@@ -379,8 +309,7 @@ void fiesta_destroy(fiesta_map *m) {
   delete m;                                                               // the buffers free themselves
 }
 
-// fiesta_create; a snapshot load passes honour_env = false, so that the mode it restores is not overridden by FIESTA_B200_MODE
-static int create_map(const fiesta_config *cfg, fiesta_map **out, bool honour_env) {
+int create_map(const fiesta_config *cfg, fiesta_map **out, bool honour_env) {
   if (!cfg || !out) { fb_set_error("fiesta_create: null argument"); return FIESTA_ERR_INVALID; }
   *out = nullptr;
   if (!(cfg->resolution > 0)) { fb_set_error("fiesta_create: resolution must be > 0"); return FIESTA_ERR_INVALID; }
@@ -468,6 +397,14 @@ int fiesta_get_config(const fiesta_map *m, fiesta_config *out) {
   return FIESTA_OK;
 }
 
+int rebuild_occbits(fiesta_map *m) {
+  const size_t words = ((size_t)m->g.ptotal + 31) / 32;
+  k_rebuild_occbits<<<(unsigned)((words + 255) / 256), 256, 0, m->stream>>>(m->occ, m->g.ptotal, m->l_occ, m->occbits);
+  m->st.kernel_launches++;
+  CK(cudaGetLastError());
+  return FIESTA_OK;
+}
+
 int fiesta_set_parameters(fiesta_map *m, double p_hit, double p_miss, double p_min, double p_max, double p_occ) {
   if (!m) return FIESTA_ERR_INVALID;
   const double old_occ = m->l_occ;
@@ -475,10 +412,8 @@ int fiesta_set_parameters(fiesta_map *m, double p_hit, double p_miss, double p_m
   m->l_min = log(p_min / (1 - p_min)); m->l_max = log(p_max / (1 - p_max)); m->l_occ = log(p_occ / (1 - p_occ));
   if (m->params_set && m->l_occ != old_occ) {                              // Exist() (ESDFMap.cpp:46-48) compares with the CURRENT threshold:
     CK(cudaSetDevice(m->device));                                         // bring the occupancy bitmap the ESDF kernels read in line with it
-    const size_t words = ((size_t)m->g.ptotal + 31) / 32;
-    k_rebuild_occbits<<<(unsigned)((words + 255) / 256), 256, 0, m->stream>>>(m->occ, m->g.ptotal, m->l_occ, m->occbits);
-    m->st.kernel_launches++;
-    CK(cudaGetLastError());
+    int r;
+    if ((r = rebuild_occbits(m))) return r;
   }
   m->params_set = true;
   return FIESTA_OK;
@@ -645,7 +580,7 @@ int fiesta_raycast_frame(fiesta_map *m, const float *xyz, int64_t n, const doubl
 }
 
 // the depth front end's buffers for images of N pixels, with no previous image or cloud
-static int alloc_depth(fiesta_map *m, size_t N) {
+int alloc_depth(fiesta_map *m, size_t N) {
   // d_img[0] is released first and allocated last, so its capacity is 0 until all six buffers hold N pixels: a call that
   // fails part-way leaves the next call to reallocate them all
   m->d_img[0] = FbDevBuf<uint16_t>();
@@ -834,13 +769,16 @@ int fiesta_set_original_range(fiesta_map *m) {
 }
 
 // ---- queries
+static void launch_query(const fiesta_map *m, const double *pos, int64_t n, int mode, double *out, double *grad, cudaStream_t s) {
+  k_query<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(m->g, m->cobs, m->occ, m->l_occ, pos, n, mode, out, grad);
+}
 static int run_query(fiesta_map *m, const double *pos, int64_t n, int mode, double *out, double *grad) {
   if (n <= 0) return FIESTA_OK;
   CK(cudaSetDevice(m->device));
   CK(m->d_qin.grow((size_t)n * 3, m->stream));
   CK(m->d_qout.grow((size_t)n * 4, m->stream));                           // [dist n][grad 3n]
   CK(cudaMemcpyAsync(m->d_qin, pos, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, m->stream));
-  k_query<<<(unsigned)((n + 127) / 128), 128, 0, m->stream>>>(m->g, m->cobs, m->occ, m->l_occ, m->d_qin, n, mode, m->d_qout, m->d_qout + n);
+  launch_query(m, m->d_qin, n, mode, m->d_qout, m->d_qout + n, m->stream);
   m->st.kernel_launches++;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, m->d_qout, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
@@ -896,7 +834,7 @@ int fiesta_get_dist_grad_trilinear_batch(fiesta_map *m, const double *pos, int64
 // before the call (the query sees every earlier update), and the map's stream waits for the query (a later update cannot rewrite
 // the records while the query reads them).  Under graph capture those two cross-stream waits would pull the map's stream into the
 // caller's graph, so a capturing stream is refused.
-static int device_query_begin(fiesta_map *m, const char *fn, cudaStream_t s) {
+int device_query_begin(fiesta_map *m, const char *fn, cudaStream_t s) {
   CK(cudaSetDevice(m->device));
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   CK(cudaStreamIsCapturing(s, &cs));
@@ -905,7 +843,7 @@ static int device_query_begin(fiesta_map *m, const char *fn, cudaStream_t s) {
   CK(cudaStreamWaitEvent(s, m->ev_q[0], 0));
   return FIESTA_OK;
 }
-static int device_query_end(fiesta_map *m, cudaStream_t s) {
+int device_query_end(fiesta_map *m, cudaStream_t s) {
   CK(cudaGetLastError());
   CK(cudaEventRecord(m->ev_q[1], s));
   CK(cudaStreamWaitEvent(m->stream, m->ev_q[1], 0));
@@ -916,7 +854,7 @@ static int device_point_query(fiesta_map *m, const char *fn, const double *d_pos
   int r;
   if ((r = device_query_begin(m, fn, s))) return r;
   if (n > 0) {
-    k_query<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(m->g, m->cobs, m->occ, m->l_occ, d_pos, n, mode, d_out, d_grad);
+    launch_query(m, d_pos, n, mode, d_out, d_grad, s);
     m->st.kernel_launches++;
   }
   return device_query_end(m, s);
@@ -930,52 +868,22 @@ int fiesta_get_dist_grad_trilinear_batch_device(fiesta_map *m, const double *d_p
   return device_point_query(m, "fiesta_get_dist_grad_trilinear_batch_device", d_pos, n, 1, d_dist, d_grad, stream);
 }
 
-// ---- segment clearance (fb_segment.h, fb_segment.cu)
-static bool segment_args_ok(const char *fn, int64_t n, double clearance, int flags, bool buffers) {
+// ---- argument checks shared by the entry points (fb_map.h)
+bool count_buffers_ok(const char *fn, int64_t n, bool buffers) {
   if (n < 0 || (n > 0 && !buffers)) { fb_set_error("%s: negative count or null buffer", fn); return false; }
+  return true;
+}
+bool clearance_flags_ok(const char *fn, double clearance, int flags) {
   if (!(clearance >= 0.0 && clearance < (double)FIESTA_INFINITY)) { fb_set_error("%s: the clearance must be >= 0 and below +10000", fn); return false; }
   if (flags & ~FIESTA_SEGMENT_UNKNOWN_BLOCKS) { fb_set_error("%s: unknown flag bits", fn); return false; }
   return true;
 }
-int fiesta_check_segments(fiesta_map *m, const double *ab, int64_t n, double clearance, int flags, int32_t *status, int64_t *hit_idx,
-                          double *hit_t, double *min_dist) {
-  if (!m || !segment_args_ok("fiesta_check_segments", n, clearance, flags, ab && status && hit_idx && hit_t && min_dist)) return FIESTA_ERR_INVALID;
-  if (n == 0) return FIESTA_OK;
-  CK(cudaSetDevice(m->device));
-  CK(m->d_seg.grow((size_t)n * 76, m->stream));
-  double *d_ab = reinterpret_cast<double *>(m->d_seg.p), *d_t = d_ab + 6 * n, *d_min = d_t + n;
-  int64_t *d_idx = reinterpret_cast<int64_t *>(d_min + n);
-  int32_t *d_st = reinterpret_cast<int32_t *>(d_idx + n);
-  CK(cudaMemcpyAsync(d_ab, ab, (size_t)n * 48, cudaMemcpyHostToDevice, m->stream));
-  CK(fb_segment_clearance(m->g, m->cobs, d_ab, n, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, d_st, d_idx, d_t, d_min, m->stream));
-  m->st.kernel_launches++;
-  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(hit_idx, d_idx, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(hit_t, d_t, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(min_dist, d_min, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  return FIESTA_OK;
-}
-int fiesta_check_segments_device(fiesta_map *m, const double *d_ab, int64_t n, double clearance, int flags, int32_t *d_status,
-                                 int64_t *d_hit_idx, double *d_hit_t, double *d_min_dist, void *stream) {
-  const char *fn = "fiesta_check_segments_device";
-  if (!m || !segment_args_ok(fn, n, clearance, flags, d_ab && d_status && d_hit_idx && d_hit_t && d_min_dist)) return FIESTA_ERR_INVALID;
-  const cudaStream_t s = (cudaStream_t)stream;
-  int r;
-  if ((r = device_query_begin(m, fn, s))) return r;
-  if (n > 0) {
-    CK(fb_segment_clearance(m->g, m->cobs, d_ab, n, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, d_status, d_hit_idx, d_hit_t, d_min_dist, s));
-    m->st.kernel_launches++;
-  }
-  return device_query_end(m, s);
-}
-
-// ---- robot-shaped collision checks (fb_pose.h, fb_pose.cu): oriented boxes at many poses
-static int pose_args(const fiesta_map *m, const char *fn, int64_t n, const double *h, double clearance, int flags, bool buffers) {
+// robot-shaped collision checks (fb_pose.h): every form, the host mirror's included
+int pose_args(const fiesta_map *m, const char *fn, int64_t n, const double *h, double clearance, int flags, bool buffers) {
   if (!h) { fb_set_error("%s: null half_extents", fn); return FIESTA_ERR_INVALID; }
   for (int k = 0; k < 3; ++k)
     if (!(h[k] >= 0.0 && h[k] <= DBL_MAX)) { fb_set_error("%s: half extents must be finite and >= 0", fn); return FIESTA_ERR_INVALID; }
-  if (!segment_args_ok(fn, n, clearance, flags, buffers)) return FIESTA_ERR_INVALID;
+  if (!count_buffers_ok(fn, n, buffers) || !clearance_flags_ok(fn, clearance, flags)) return FIESTA_ERR_INVALID;
   if ((h[0] + h[1]) + h[2] > FB_POSE_MAX_SPAN * m->g.res) {
     fb_set_error("%s: h0 + h1 + h2 = %g m exceeds %d voxels", fn, (h[0] + h[1]) + h[2], FB_POSE_MAX_SPAN);
     return FIESTA_ERR_LIMIT;
@@ -983,690 +891,28 @@ static int pose_args(const fiesta_map *m, const char *fn, int64_t n, const doubl
   if (n >= INT32_MAX) { fb_set_error("%s: n = %lld poses, the limit is 2^31 - 2", fn, (long long)n); return FIESTA_ERR_LIMIT; }
   return FIESTA_OK;
 }
-int fiesta_check_poses(fiesta_map *m, const double *poses, int64_t n, const double half_extents[3], double clearance, int flags,
-                       int32_t *status, int32_t *n_blocked, int64_t *hit_idx) {
-  const char *fn = "fiesta_check_poses";
-  if (!m) return FIESTA_ERR_INVALID;
-  int r;
-  if ((r = pose_args(m, fn, n, half_extents, clearance, flags, poses && status && n_blocked && hit_idx))) return r;
-  if (n == 0) return FIESTA_OK;
-  CK(cudaSetDevice(m->device));
-  CK(m->pose.io.grow((size_t)n * 112, m->stream));
-  double *d_poses = reinterpret_cast<double *>(m->pose.io.p);
-  int64_t *d_idx = reinterpret_cast<int64_t *>(d_poses + 12 * n);
-  int32_t *d_st = reinterpret_cast<int32_t *>(d_idx + n), *d_nb = d_st + n;
-  CK(cudaMemcpyAsync(d_poses, poses, (size_t)n * 96, cudaMemcpyHostToDevice, m->stream));
-  int launches = 0;
-  if ((r = fb_pose_check_batch(m->g, m->cobs, d_poses, n, half_extents, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, d_st, d_nb, d_idx,
-                               m->pose, m->stream, &launches)))
-    return r;
-  m->st.kernel_launches += launches;
-  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(n_blocked, d_nb, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(hit_idx, d_idx, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  return FIESTA_OK;
-}
-int fiesta_check_poses_device(fiesta_map *m, const double *d_poses, int64_t n, const double half_extents[3], double clearance, int flags,
-                              int32_t *d_status, int32_t *d_n_blocked, int64_t *d_hit_idx, void *stream) {
-  const char *fn = "fiesta_check_poses_device";
-  if (!m) return FIESTA_ERR_INVALID;
-  int r;
-  if ((r = pose_args(m, fn, n, half_extents, clearance, flags, d_poses && d_status && d_n_blocked && d_hit_idx))) return r;
-  const cudaStream_t s = (cudaStream_t)stream;
-  if ((r = device_query_begin(m, fn, s))) return r;
-  if (n > 0) {
-    int launches = 0;
-    if ((r = fb_pose_check_batch(m->g, m->cobs, d_poses, n, half_extents, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, d_status,
-                                 d_n_blocked, d_hit_idx, m->pose, s, &launches)))
-      return r;
-    m->st.kernel_launches += launches;
-  }
-  return device_query_end(m, s);
-}
-
-// ---- cost-to-go field (fb_nav.h, fb_nav.cu): a box's geodesic distance to a goal set through free space at a clearance
-struct fiesta_nav_field {
-  fiesta_map *m = nullptr;
-  int blocks = 0;                   // co-resident CTAs of k_nav_relax (cooperative launch)
-  int wblocks = 0;                  // co-resident CTAs of k_navu_withdraw
-  FbDevBuf<double> D, d_goals;
-  FbDevBuf<uint32_t> stamp, list[2];
-  FbDevBuf<FbNavCtr> ctr;
-  FbHostBuf<FbNavCtr> h_ctr;
-  FbDevBuf<double> d_pd;            // fiesta_nav_paths: [starts 3n][cost n]
-  FbDevBuf<int32_t> d_pi;           //                   [status n][len n][vox 3 n max_len]
-  FbDevBuf<uint8_t> u_flags;        // fiesta_nav_update: one scratch byte per box voxel
-  FbDevBuf<FbNavUCtr> u_ctr;
-  FbHostBuf<FbNavUCtr> h_uctr;
-  // fiesta_nav_matrix: its own buffers, so that a matrix leaves the last field, export and paths as they were
-  int mblocks = 0;                  // co-resident CTAs of k_navm_relax
-  FbDevBuf<uint32_t> M;             // per box voxel: move mask
-  FbDevBuf<double> MD, m_pts, m_cost;   // [channel][box voxel] fields; points [sources 3 n_src][targets 3 n_tgt]; cost
-  FbDevBuf<uint32_t> m_stamp, m_list[2];  // per (channel, tile)
-  FbDevBuf<int32_t> m_st, m_rows;   // per point: status; rows: placed sources in index order, then the others
-  FbDevBuf<long long> m_idx, m_src, m_tgt;  // per point: box index or -1; placed sources' box indices; placed targets' box indices
-  FbDevBuf<FbNavMCtr> m_ctr;
-  FbDevBuf<FbNavMTot> m_tot;
-  FbHostBuf<FbNavMTot> h_mtot;
-  cudaEvent_t ev[2] = {};
-  FbNavBox box{};
-  double w[3]{};
-  bool valid = false;               // D holds a field computed for `box`
-  long long n_goals = 0;            // goals (in d_goals), clearance and flags of the last compute: what fiesta_nav_update keeps
-  double clearance = 0.0;
-  int flags = 0;
-};
-void fiesta_nav_destroy(fiesta_nav_field *f) {
-  if (!f) return;
-  cudaSetDevice(f->m->device);
-  cudaStreamSynchronize(f->m->stream);
-  for (cudaEvent_t e : f->ev) if (e) cudaEventDestroy(e);
-  delete f;
-}
-int fiesta_nav_create(fiesta_map *m, fiesta_nav_field **out) {
-  if (!m || !out) { fb_set_error("fiesta_nav_create: null argument"); return FIESTA_ERR_INVALID; }
-  *out = nullptr;
-  CK(cudaSetDevice(m->device));
-  std::unique_ptr<fiesta_nav_field, void (*)(fiesta_nav_field *)> f(new (std::nothrow) fiesta_nav_field(), fiesta_nav_destroy);
-  if (!f) { fb_set_error("out of host memory"); return FIESTA_ERR_INVALID; }
-  f->m = m;
-  f->blocks = fb_nav_relax_blocks(m->device);
-  f->mblocks = fb_navm_relax_blocks(m->device);
-  f->wblocks = fb_nav_withdraw_blocks(m->device);
-  if (f->blocks <= 0 || f->mblocks <= 0 || f->wblocks <= 0) { fb_set_error("fiesta_nav_create: the relaxation kernel does not fit on this device"); return FIESTA_ERR_CUDA; }
-  for (cudaEvent_t &e : f->ev) CK(cudaEventCreate(&e));
-  CK(f->ctr.alloc(1));
-  CK(f->h_ctr.alloc(1));
-  CK(f->m_ctr.alloc(1));
-  CK(f->m_tot.alloc(1));
-  CK(f->h_mtot.alloc(1));
-  CK(f->u_ctr.alloc(1));
-  CK(f->h_uctr.alloc(1));
-  for (int k = 0; k < 3; ++k) f->w[k] = m->g.res * sqrt((double)(k + 1));
-  *out = f.release();
-  return FIESTA_OK;
-}
-int fiesta_nav_compute(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *goals_xyz, int64_t n_goals,
-                       double clearance, int flags, fiesta_nav_stats *stats) {
-  const char *fn = "fiesta_nav_compute";
-  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
-  if (!segment_args_ok(fn, n_goals, clearance, flags, goals_xyz != nullptr)) return FIESTA_ERR_INVALID;
-  fiesta_map *m = f->m;
-  const FbGeom &g = m->g;
+bool box_axis_ok(const char *fn, const FbGeom &g, const int *lo, const int *hi, int k) {
   const int gs[3] = {g.gx, g.gy, g.gz};
-  FbNavArgs a{};
+  if (lo[k] >= 0 && lo[k] <= hi[k] && hi[k] < gs[k]) return true;
+  fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
+  return false;
+}
+bool box_arg(const char *fn, const FbGeom &g, const int *lo, const int *hi, FbNavBox *b) {
   for (int k = 0; k < 3; ++k) {
-    if (!(box_lo[k] >= 0 && box_lo[k] <= box_hi[k] && box_hi[k] < gs[k])) {
-      fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
-      return FIESTA_ERR_INVALID;
-    }
-    a.b.lo[k] = box_lo[k];
-    a.b.n[k] = box_hi[k] - box_lo[k] + 1;
-    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
-    a.w[k] = f->w[k];
-  }
-  const size_t nv = (size_t)a.b.n[0] * a.b.n[1] * a.b.n[2], nt = (size_t)a.tn[0] * a.tn[1] * a.tn[2];
-  CK(cudaSetDevice(m->device));
-  f->valid = false;
-  cudaError_t e = f->D.grow(nv, m->stream);
-  for (FbDevBuf<uint32_t> *b : {&f->stamp, &f->list[0], &f->list[1]})
-    if (e == cudaSuccess) e = b->grow(nt, m->stream);
-  if (e == cudaSuccess && n_goals > 0) e = f->d_goals.grow((size_t)n_goals * 3, m->stream);
-  if (e != cudaSuccess) {
-    cudaGetLastError();                                                   // not sticky: later calls must not see it
-    fb_set_error("%s: cannot allocate the field of %zu voxels: %s", fn, nv, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
-  a.D = f->D; a.stamp = f->stamp; a.list[0] = f->list[0]; a.list[1] = f->list[1]; a.ctr = f->ctr;
-  if (n_goals > 0) CK(cudaMemcpyAsync(f->d_goals, goals_xyz, (size_t)n_goals * 24, cudaMemcpyHostToDevice, m->stream));
-  CK(cudaMemsetAsync(f->stamp, 0, nt * 4, m->stream));
-  CK(cudaMemsetAsync(f->ctr, 0, sizeof(FbNavCtr), m->stream));
-  CK(cudaEventRecord(f->ev[0], m->stream));
-  CK(fb_nav_compute(g, m->cobs, a, f->d_goals, n_goals, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, f->blocks, m->stream));
-  m->st.kernel_launches += n_goals > 0 ? 4 : 3;
-  CK(cudaEventRecord(f->ev[1], m->stream));
-  CK(cudaMemcpyAsync(f->h_ctr, f->ctr, sizeof(FbNavCtr), cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  f->box = a.b;
-  f->valid = true;
-  f->n_goals = n_goals;
-  f->clearance = clearance;
-  f->flags = flags;
-  if (stats) {
-    const FbNavCtr &c = *f->h_ctr;
-    *stats = fiesta_nav_stats{};
-    stats->box_voxels = (int64_t)nv;
-    stats->blocked = (int64_t)c.blocked;
-    stats->reached = (int64_t)c.reached;
-    stats->goals_placed = (int64_t)c.goals_placed;
-    stats->generations = (int64_t)c.generations;
-    stats->tile_visits = (int64_t)c.tile_visits;
-    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
-  }
-  return FIESTA_OK;
-}
-int fiesta_nav_update(fiesta_nav_field *f, fiesta_nav_update_stats *stats) {
-  const char *fn = "fiesta_nav_update";
-  if (!f) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
-  if (!f->valid) { fb_set_error("%s: no field has been computed", fn); return FIESTA_ERR_INVALID; }
-  fiesta_map *m = f->m;
-  FbNavArgs a{};
-  a.b = f->box;
-  for (int k = 0; k < 3; ++k) {
-    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
-    a.w[k] = f->w[k];
-  }
-  const size_t nv = (size_t)a.b.n[0] * a.b.n[1] * a.b.n[2];
-  CK(cudaSetDevice(m->device));
-  if (cudaError_t e = f->u_flags.grow(nv, m->stream)) {                  // before anything is written: the field stays valid
-    cudaGetLastError();
-    fb_set_error("%s: cannot allocate the scratch of %zu voxels: %s", fn, nv, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
-  a.D = f->D; a.stamp = f->stamp; a.list[0] = f->list[0]; a.list[1] = f->list[1]; a.ctr = f->ctr;
-  f->valid = false;                                                       // until the update has finished
-  CK(cudaEventRecord(f->ev[0], m->stream));
-  CK(fb_nav_update(m->g, m->cobs, a, f->u_flags, f->u_ctr, f->d_goals, f->n_goals, f->clearance, f->flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS,
-                   f->blocks, f->wblocks, m->stream));
-  m->st.kernel_launches += f->n_goals > 0 ? 6 : 5;
-  CK(cudaEventRecord(f->ev[1], m->stream));
-  CK(cudaMemcpyAsync(f->h_ctr, f->ctr, sizeof(FbNavCtr), cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(f->h_uctr, f->u_ctr, sizeof(FbNavUCtr), cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  f->valid = true;
-  if (stats) {
-    const FbNavCtr &c = *f->h_ctr;
-    const FbNavUCtr &u = *f->h_uctr;
-    *stats = fiesta_nav_update_stats{};
-    stats->box_voxels = (int64_t)nv;
-    stats->became_blocked = (int64_t)u.became_blocked;
-    stats->became_free = (int64_t)u.became_free;
-    stats->withdrawn = (int64_t)u.withdrawn;
-    stats->goals_placed = (int64_t)c.goals_placed;
-    stats->goals_new = (int64_t)u.goals_new;
-    stats->seed_tiles = (int64_t)u.seed_tiles;
-    stats->withdraw_generations = (int64_t)u.wave.generations;
-    stats->generations = (int64_t)c.generations;
-    stats->tile_visits = (int64_t)c.tile_visits;
-    stats->blocked = (int64_t)c.blocked;
-    stats->reached = (int64_t)c.reached;
-    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
-  }
-  return FIESTA_OK;
-}
-int fiesta_nav_export(const fiesta_nav_field *f, double *out) {
-  if (!f || !out) { fb_set_error("fiesta_nav_export: null argument"); return FIESTA_ERR_INVALID; }
-  if (!f->valid) { fb_set_error("fiesta_nav_export: no field has been computed"); return FIESTA_ERR_INVALID; }
-  const fiesta_map *m = f->m;
-  CK(cudaSetDevice(m->device));
-  CK(cudaMemcpyAsync(out, f->D, (size_t)f->box.n[0] * f->box.n[1] * f->box.n[2] * 8, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  return FIESTA_OK;
-}
-int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, int32_t max_len, int32_t *status, int32_t *len, double *cost,
-                     int32_t *vox_xyz) {
-  const char *fn = "fiesta_nav_paths";
-  if (!f || n < 0 || max_len < 1 || (n > 0 && !(starts_xyz && status && len && cost && vox_xyz))) {
-    fb_set_error("%s: null buffer, negative count or max_len < 1", fn);
-    return FIESTA_ERR_INVALID;
-  }
-  if (!f->valid) { fb_set_error("%s: no field has been computed", fn); return FIESTA_ERR_INVALID; }
-  if (n == 0) return FIESTA_OK;
-  fiesta_map *m = f->m;
-  CK(cudaSetDevice(m->device));
-  const size_t nv = (size_t)n * max_len * 3;
-  cudaError_t e = f->d_pd.grow((size_t)n * 4, m->stream);
-  if (e == cudaSuccess) e = f->d_pi.grow((size_t)n * 2 + nv, m->stream);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    fb_set_error("%s: cannot allocate %lld paths of %d voxels: %s", fn, (long long)n, (int)max_len, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
-  double *d_starts = f->d_pd, *d_cost = d_starts + 3 * n;
-  int32_t *d_st = f->d_pi, *d_len = d_st + n, *d_vox = d_len + n;
-  CK(cudaMemcpyAsync(d_starts, starts_xyz, (size_t)n * 24, cudaMemcpyHostToDevice, m->stream));
-  CK(cudaMemsetAsync(d_vox, 0xff, nv * 4, m->stream));                    // -1 past each path's end
-  CK(fb_nav_paths(m->g, f->box, f->D, f->w, d_starts, n, max_len, d_st, d_len, d_cost, d_vox, m->stream));
-  m->st.kernel_launches++;
-  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(len, d_len, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(cost, d_cost, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(vox_xyz, d_vox, nv * 4, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  return FIESTA_OK;
-}
-int fiesta_nav_matrix(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *sources_xyz, int64_t n_src,
-                      const double *targets_xyz, int64_t n_tgt, double clearance, int flags, int32_t *src_status, int32_t *tgt_status,
-                      double *cost, fiesta_nav_matrix_stats *stats) {
-  const char *fn = "fiesta_nav_matrix";
-  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
-  if (n_src < 0 || n_tgt < 0 || (n_src > 0 && !(sources_xyz && src_status)) || (n_tgt > 0 && !(targets_xyz && tgt_status)) ||
-      (n_src > 0 && n_tgt > 0 && !cost)) {
-    fb_set_error("%s: negative count or null buffer", fn);
-    return FIESTA_ERR_INVALID;
-  }
-  if (!segment_args_ok(fn, 0, clearance, flags, true)) return FIESTA_ERR_INVALID;
-  fiesta_map *m = f->m;
-  const int gs[3] = {m->g.gx, m->g.gy, m->g.gz};
-  FbNavMArgs a{};
-  for (int k = 0; k < 3; ++k) {
-    if (!(box_lo[k] >= 0 && box_lo[k] <= box_hi[k] && box_hi[k] < gs[k])) {
-      fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
-      return FIESTA_ERR_INVALID;
-    }
-    a.b.lo[k] = box_lo[k];
-    a.b.n[k] = box_hi[k] - box_lo[k] + 1;
-    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
-    a.w[k] = f->w[k];
-  }
-  if (n_src > 0 && n_tgt > 0 && n_src >= ((1ll << 31) + n_tgt - 1) / n_tgt) {
-    fb_set_error("%s: n_src * n_tgt must be below 2^31", fn);
-    return FIESTA_ERR_LIMIT;
-  }
-  const long long nv = (long long)a.b.n[0] * a.b.n[1] * a.b.n[2], nt = (long long)a.tn[0] * a.tn[1] * a.tn[2], np = n_src + n_tgt;
-  a.nv = nv;
-  a.nt = (unsigned)nt;
-  cudaStream_t s = m->stream;
-  CK(cudaSetDevice(m->device));
-  // (1) move masks, statuses and box indices of every point; the statuses and indices come back for the host to plan the passes
-  cudaError_t e = f->M.grow((size_t)nv, s);
-  if (e == cudaSuccess && np > 0) e = f->m_pts.grow((size_t)np * 3, s);
-  if (e == cudaSuccess && np > 0) e = f->m_st.grow((size_t)np, s);
-  if (e == cudaSuccess && np > 0) e = f->m_idx.grow((size_t)np, s);
-  if (e != cudaSuccess) {
-    cudaGetLastError();                                                   // not sticky: later calls must not see it
-    fb_set_error("%s: cannot allocate the move masks of %lld voxels: %s", fn, nv, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
-  CK(cudaEventRecord(f->ev[0], s));
-  if (n_src > 0) CK(cudaMemcpyAsync(f->m_pts, sources_xyz, (size_t)n_src * 24, cudaMemcpyHostToDevice, s));
-  if (n_tgt > 0) CK(cudaMemcpyAsync(f->m_pts + 3 * n_src, targets_xyz, (size_t)n_tgt * 24, cudaMemcpyHostToDevice, s));
-  CK(fb_navm_locate(m->g, m->cobs, a.b, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, f->M, f->m_pts, np, f->m_st, f->m_idx, s));
-  m->st.kernel_launches += np > 0 ? 3 : 2;
-  std::vector<int32_t> st((size_t)np);
-  std::vector<long long> idx((size_t)np);
-  if (np > 0) {
-    CK(cudaMemcpyAsync(st.data(), f->m_st, (size_t)np * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(idx.data(), f->m_idx, (size_t)np * 8, cudaMemcpyDeviceToHost, s));
-  }
-  CK(cudaStreamSynchronize(s));
-  // rows: the placed sources in index order (channel k of the passes is placed source k), then the others (NaN rows)
-  std::vector<int32_t> rows;
-  std::vector<long long> src, tgt;
-  long long n_ps = 0;
-  for (long long i = 0; i < n_src; ++i) n_ps += st[i] == FB_NAVM_PLACED;
-  if (n_tgt > 0) {                                                         // then n_src < 2^31
-    for (long long i = 0; i < n_src; ++i)
-      if (st[i] == FB_NAVM_PLACED) { rows.push_back((int32_t)i); src.push_back(idx[i]); }
-    for (long long i = 0; i < n_src; ++i)
-      if (st[i] != FB_NAVM_PLACED) rows.push_back((int32_t)i);
-  }
-  for (long long j = n_src; j < np; ++j)
-    if (st[j] == FB_NAVM_PLACED) tgt.push_back(idx[j]);
-  const long long n_pt = (long long)tgt.size();
-  // (2) passes of C channels: C = min(32, sources left, max(1, floor(2^32 B / (8 B x box voxels))))
-  const long long per_pass = std::max(1ll, std::min((long long)FB_NAVM_CH, (1ll << 32) / (8 * nv)));
-  const long long C = std::min(per_pass, n_ps);
-  const bool work = n_ps > 0 && n_pt > 0;
-  if (work && C * nt >= (long long)0xffffffffu) {
-    fb_set_error("%s: the box has too many tiles", fn);
-    return FIESTA_ERR_LIMIT;
-  }
-  e = cudaSuccess;
-  if (n_src > 0 && n_tgt > 0) e = f->m_cost.grow((size_t)(n_src * n_tgt), s);
-  if (e == cudaSuccess && n_src > 0 && n_tgt > 0) e = f->m_rows.grow((size_t)n_src, s);
-  if (work) {
-    if (e == cudaSuccess) e = f->MD.grow((size_t)(C * nv), s);
-    for (FbDevBuf<uint32_t> *b : {&f->m_stamp, &f->m_list[0], &f->m_list[1]})
-      if (e == cudaSuccess) e = b->grow((size_t)(C * nt), s);
-    if (e == cudaSuccess) e = f->m_src.grow((size_t)n_ps, s);
-    if (e == cudaSuccess) e = f->m_tgt.grow((size_t)n_pt, s);
-  }
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    fb_set_error("%s: cannot allocate %lld fields of %lld voxels and the %lld x %lld matrix: %s", fn, C, nv, (long long)n_src,
-                 (long long)n_tgt, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
-  if (n_src > 0 && n_tgt > 0) CK(cudaMemcpyAsync(f->m_rows, rows.data(), (size_t)n_src * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemsetAsync(f->m_tot, 0, sizeof(FbNavMTot), s));
-  long long passes = 0;
-  if (work) {
-    CK(cudaMemcpyAsync(f->m_src, src.data(), (size_t)n_ps * 8, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(f->m_tgt, tgt.data(), (size_t)n_pt * 8, cudaMemcpyHostToDevice, s));
-    a.D = f->MD; a.M = f->M; a.stamp = f->m_stamp; a.list[0] = f->m_list[0]; a.list[1] = f->m_list[1];
-    a.ctr = f->m_ctr; a.tot = f->m_tot; a.tgt = f->m_tgt; a.n_tgt = (int)n_pt;
-    for (long long p0 = 0; p0 < n_ps; p0 += C, ++passes) {
-      a.nch = (int)std::min(C, n_ps - p0);
-      CK(cudaMemsetAsync(f->m_stamp, 0, (size_t)(a.nch * nt) * 4, s));
-      CK(cudaMemsetAsync(f->m_ctr, 0, sizeof(FbNavMCtr), s));
-      CK(fb_navm_pass(a, f->m_src + p0, f->mblocks, s));
-      CK(fb_navm_gather(f->MD, nv, f->m_rows + p0, a.nch, f->m_idx + n_src, n_tgt, f->m_cost, s));
-      m->st.kernel_launches += 4;
-    }
-  }
-  // NaN rows: every source when no target is placed, else the sources not placed
-  const long long nan_from = work ? n_ps : 0;
-  if (n_src > nan_from && n_tgt > 0) {
-    CK(fb_navm_gather(nullptr, nv, f->m_rows + nan_from, n_src - nan_from, f->m_idx + n_src, n_tgt, f->m_cost, s));
-    m->st.kernel_launches++;
-  }
-  CK(cudaEventRecord(f->ev[1], s));
-  if (n_src > 0 && n_tgt > 0) CK(cudaMemcpyAsync(cost, f->m_cost, (size_t)(n_src * n_tgt) * 8, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(f->h_mtot, f->m_tot, sizeof(FbNavMTot), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  if (n_src > 0) memcpy(src_status, st.data(), (size_t)n_src * 4);
-  if (n_tgt > 0) memcpy(tgt_status, st.data() + n_src, (size_t)n_tgt * 4);
-  if (stats) {
-    const FbNavMTot &t = *f->h_mtot;
-    *stats = fiesta_nav_matrix_stats{};
-    stats->sources_placed = n_ps;
-    stats->targets_placed = n_pt;
-    stats->passes = passes;
-    stats->generations = (int64_t)t.generations;
-    stats->tile_visits = (int64_t)t.tile_visits;
-    stats->sources_retired_early = (int64_t)t.retired_early;
-    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
-  }
-  return FIESTA_OK;
-}
-
-// ---- frontier extraction (fb_frontier.h, fb_frontier.cu): free voxels of a box that border unknown space, clustered
-struct fiesta_frontiers {
-  fiesta_map *m = nullptr;
-  FbFrBufs B;
-  FbViewBufs V;                     // fiesta_frontiers_score_viewpoints
-  cudaEvent_t ev[2] = {};
-  FbNavBox box{};
-  fiesta_frontier_stats st{};
-  bool valid = false;               // B holds the result of a compute over `box`
-};
-void fiesta_frontiers_destroy(fiesta_frontiers *f) {
-  if (!f) return;
-  cudaSetDevice(f->m->device);
-  cudaStreamSynchronize(f->m->stream);
-  for (cudaEvent_t e : f->ev) if (e) cudaEventDestroy(e);
-  delete f;
-}
-int fiesta_frontiers_create(fiesta_map *m, fiesta_frontiers **out) {
-  if (!m || !out) { fb_set_error("fiesta_frontiers_create: null argument"); return FIESTA_ERR_INVALID; }
-  *out = nullptr;
-  CK(cudaSetDevice(m->device));
-  std::unique_ptr<fiesta_frontiers, void (*)(fiesta_frontiers *)> f(new (std::nothrow) fiesta_frontiers(), fiesta_frontiers_destroy);
-  if (!f) { fb_set_error("out of host memory"); return FIESTA_ERR_INVALID; }
-  f->m = m;
-  for (cudaEvent_t &e : f->ev) CK(cudaEventCreate(&e));
-  CK(f->B.ctr.alloc(1));
-  CK(f->B.h_ctr.alloc(1));
-  *out = f.release();
-  return FIESTA_OK;
-}
-int fiesta_frontiers_compute(fiesta_frontiers *f, const int box_lo[3], const int box_hi[3], double clearance, int64_t min_cluster_size,
-                             fiesta_frontier_stats *stats) {
-  const char *fn = "fiesta_frontiers_compute";
-  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
-  if (!segment_args_ok(fn, 0, clearance, 0, true)) return FIESTA_ERR_INVALID;
-  if (min_cluster_size < 1) { fb_set_error("%s: min_cluster_size must be >= 1", fn); return FIESTA_ERR_INVALID; }
-  fiesta_map *m = f->m;
-  const int gs[3] = {m->g.gx, m->g.gy, m->g.gz};
-  FbNavBox b{};
-  for (int k = 0; k < 3; ++k) {
-    if (!(box_lo[k] >= 0 && box_lo[k] <= box_hi[k] && box_hi[k] < gs[k])) {
-      fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
-      return FIESTA_ERR_INVALID;
-    }
-    b.lo[k] = box_lo[k];
-    b.n[k] = box_hi[k] - box_lo[k] + 1;
-  }
-  CK(cudaSetDevice(m->device));
-  f->valid = false;
-  int launches = 0;
-  CK(cudaEventRecord(f->ev[0], m->stream));
-  const int r = fb_frontier_compute(m->g, m->cobs, m->occ, m->l_occ, b, clearance, (long long)min_cluster_size, f->B, m->stream, &launches);
-  m->st.kernel_launches += launches;
-  if (r != FIESTA_OK) return r;
-  CK(cudaEventRecord(f->ev[1], m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  const FbFrCtr &c = *f->B.h_ctr;
-  f->st = fiesta_frontier_stats{};
-  f->st.box_voxels = (int64_t)b.n[0] * b.n[1] * b.n[2];
-  f->st.frontier_voxels = (int64_t)c.frontier;
-  f->st.clusters = (int64_t)c.roots;
-  f->st.kept_clusters = (int64_t)c.sel[1];
-  f->st.kept_voxels = (int64_t)c.kept_voxels;
-  CK(cudaEventElapsedTime(&f->st.ms_compute, f->ev[0], f->ev[1]));
-  f->box = b;
-  f->valid = true;
-  if (stats) *stats = f->st;
-  return FIESTA_OK;
-}
-int fiesta_frontiers_clusters(const fiesta_frontiers *f, int64_t cap, int64_t *size, int32_t *rep_xyz, int32_t *bbox_lo_xyz,
-                              int32_t *bbox_hi_xyz, double *centroid_xyz) {
-  const char *fn = "fiesta_frontiers_clusters";
-  if (!f || cap < 0 || (cap > 0 && !(size && rep_xyz && bbox_lo_xyz && bbox_hi_xyz && centroid_xyz))) {
-    fb_set_error("%s: null buffer or negative capacity", fn);
-    return FIESTA_ERR_INVALID;
-  }
-  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
-  const size_t n = (size_t)(cap < f->st.kept_clusters ? cap : f->st.kept_clusters), C = f->B.C;
-  if (n == 0) return FIESTA_OK;
-  const fiesta_map *m = f->m;
-  CK(cudaSetDevice(m->device));
-  CK(cudaMemcpyAsync(size, f->B.o_size, n * 8, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(rep_xyz, f->B.o_i32, n * 12, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(bbox_lo_xyz, f->B.o_i32 + 3 * C, n * 12, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(bbox_hi_xyz, f->B.o_i32 + 6 * C, n * 12, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaMemcpyAsync(centroid_xyz, f->B.o_cen, n * 24, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  return FIESTA_OK;
-}
-int fiesta_frontiers_voxels(const fiesta_frontiers *f, int64_t cap, int32_t *vox_xyz) {
-  const char *fn = "fiesta_frontiers_voxels";
-  if (!f || cap < 0 || (cap > 0 && !vox_xyz)) { fb_set_error("%s: null buffer or negative capacity", fn); return FIESTA_ERR_INVALID; }
-  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
-  const size_t n = (size_t)(cap < f->st.kept_voxels ? cap : f->st.kept_voxels);
-  if (n == 0) return FIESTA_OK;
-  const fiesta_map *m = f->m;
-  CK(cudaSetDevice(m->device));
-  CK(cudaMemcpyAsync(vox_xyz, f->B.m_xyz, n * 12, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  return FIESTA_OK;
-}
-int fiesta_frontiers_export(const fiesta_frontiers *f, int32_t *labels) {
-  if (!f || !labels) { fb_set_error("fiesta_frontiers_export: null argument"); return FIESTA_ERR_INVALID; }
-  if (!f->valid) { fb_set_error("fiesta_frontiers_export: no frontiers have been computed"); return FIESTA_ERR_INVALID; }
-  const fiesta_map *m = f->m;
-  CK(cudaSetDevice(m->device));
-  CK(cudaMemcpyAsync(labels, f->B.L, (size_t)f->st.box_voxels * 4, cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  return FIESTA_OK;
-}
-// viewpoint coverage of the clusters (fb_view.h, fb_view.cu)
-int fiesta_frontiers_score_viewpoints(fiesta_frontiers *f, const int32_t *cluster, const double *pos_xyz, int64_t n, const double *orient,
-                                      int32_t n_orient, const fiesta_sensor_model *sensor, double clearance, int flags, int32_t *status,
-                                      int32_t *score, fiesta_viewpoint_stats *stats) {
-  const char *fn = "fiesta_frontiers_score_viewpoints";
-  if (!f || !sensor || !orient) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
-  if (!segment_args_ok(fn, n, clearance, flags, cluster && pos_xyz && status && score)) return FIESTA_ERR_INVALID;
-  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
-  if (n_orient < 1) { fb_set_error("%s: n_orient must be >= 1", fn); return FIESTA_ERR_INVALID; }
-  const fiesta_sensor_model sm = *sensor;
-  const double sv[3] = {sm.max_range, sm.tan_half_fov[0], sm.tan_half_fov[1]};
-  for (double x : sv)
-    if (!(std::isfinite(x) && x > 0)) { fb_set_error("%s: max_range and tan_half_fov must be finite and > 0", fn); return FIESTA_ERR_INVALID; }
-  if (n_orient > FIESTA_VIEWPOINT_MAX_ORIENT) {
-    fb_set_error("%s: at most %d orientations per call", fn, FIESTA_VIEWPOINT_MAX_ORIENT);
-    return FIESTA_ERR_LIMIT;
-  }
-  for (int k = 0; k < 9 * n_orient; ++k)
-    if (!std::isfinite(orient[k])) { fb_set_error("%s: orientation entry %d is not finite", fn, k); return FIESTA_ERR_INVALID; }
-  const int64_t K = f->st.kept_clusters;
-  for (int64_t i = 0; i < n; ++i)
-    if (!(cluster[i] >= 0 && cluster[i] < K)) {
-      fb_set_error("%s: cluster[%lld] = %d is not a kept cluster id (there are %lld)", fn, (long long)i, (int)cluster[i], (long long)K);
-      return FIESTA_ERR_INVALID;
-    }
-  if (n >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 candidates per call", fn); return FIESTA_ERR_LIMIT; }
-  if (stats) *stats = fiesta_viewpoint_stats{};
-  if (n == 0) return FIESTA_OK;
-  fiesta_map *m = f->m;
-  const cudaStream_t s = m->stream;
-  FbViewBufs &V = f->V;
-  CK(cudaSetDevice(m->device));
-  cudaError_t e = V.pos.grow((size_t)n * 3, s);
-  if (e == cudaSuccess) e = V.cl.grow((size_t)n, s);
-  if (e == cudaSuccess) e = V.status.grow((size_t)n, s);
-  if (e == cudaSuccess) e = V.work.grow((size_t)n + 1, s);
-  if (e == cudaSuccess) e = V.score.grow((size_t)n * n_orient, s);
-  if (e == cudaSuccess) e = V.moff.grow((size_t)K, s);
-  if (e == cudaSuccess) e = V.orient.grow(9 * FIESTA_VIEWPOINT_MAX_ORIENT, s);
-  if (e == cudaSuccess) e = V.ctr.grow(1, s);
-  if (e == cudaSuccess && !V.h_ctr) e = V.h_ctr.alloc(1);
-  if (e != cudaSuccess) {
-    cudaGetLastError();                                                   // not sticky: later calls must not see it
-    fb_set_error("%s: cannot allocate the buffers of %lld candidates: %s", fn, (long long)n, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
-  CK(cudaMemcpyAsync(V.pos, pos_xyz, (size_t)n * 24, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(V.cl, cluster, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(V.orient, orient, (size_t)n_orient * 72, cudaMemcpyHostToDevice, s));
-  CK(cudaMemsetAsync(V.score, 0, (size_t)n * n_orient * 4, s));
-  CK(cudaMemsetAsync(V.ctr, 0, sizeof(FbViewCtr), s));
-  int launches = 0;
-  CK(cudaEventRecord(f->ev[0], s));
-  const int r = fb_view_score(m->g, m->cobs, f->B.o_size, f->B.m_xyz, (unsigned)K, V, f->B.tmp, (long long)n, (int)n_orient, sm, clearance,
-                              flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, s, &launches);
-  m->st.kernel_launches += launches;
-  if (r != FIESTA_OK) return r;
-  CK(cudaEventRecord(f->ev[1], s));
-  CK(cudaMemcpyAsync(V.h_ctr, V.ctr, sizeof(FbViewCtr), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(status, V.status, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(score, V.score, (size_t)n * n_orient * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  if (stats) {
-    stats->candidates_scored = (int64_t)V.h_ctr->scored;
-    stats->pairs_walked = (int64_t)V.h_ctr->walked;
-    stats->pairs_visible = (int64_t)V.h_ctr->visible;
-    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
-  }
-  return FIESTA_OK;
-}
-
-// ---- safe flight corridors (fb_corridor.h, fb_corridor.cu): free boxes inflated in a limit box, and chains of them along paths
-static bool corridor_args_ok(const char *fn, const fiesta_map *m, const int *box_lo, const int *box_hi, const int32_t *max_steps,
-                             int64_t n, double clearance, int flags, bool buffers) {
-  if (!m || !box_lo || !box_hi || !max_steps) { fb_set_error("%s: null argument", fn); return false; }
-  if (!segment_args_ok(fn, n, clearance, flags, buffers)) return false;
-  const int gs[3] = {m->g.gx, m->g.gy, m->g.gz};
-  for (int k = 0; k < 3; ++k) {
-    if (!(box_lo[k] >= 0 && box_lo[k] <= box_hi[k] && box_hi[k] < gs[k])) {
-      fb_set_error("%s: the box must satisfy 0 <= lo <= hi < grid size on every axis", fn);
-      return false;
-    }
-    if (max_steps[k] < 0) { fb_set_error("%s: max_steps must be >= 0", fn); return false; }
+    if (!box_axis_ok(fn, g, lo, hi, k)) return false;
+    if (b) { b->lo[k] = lo[k]; b->n[k] = hi[k] - lo[k] + 1; }
   }
   return true;
 }
-// Grow the buffers, then record the start event and build the limit box's masks.
-static int corridor_begin(fiesta_map *m, const char *fn, const int *box_lo, const int *box_hi, double clearance, int flags,
-                          size_t in_words, size_t off_words, size_t out_words) {
-  FbCorrBufs &B = m->corr;
-  const FbCorrMask M = fb_corr_mask_geom(box_lo, box_hi);
-  const cudaStream_t s = m->stream;
-  CK(cudaSetDevice(m->device));
-  cudaError_t e = B.mask.grow((size_t)fb_corr_mask_words(M), s);
-  if (e == cudaSuccess) e = B.in.grow(in_words, s);
-  if (e == cudaSuccess && off_words) e = B.off.grow(off_words, s);
-  if (e == cudaSuccess) e = B.out.grow(out_words, s);
-  if (e == cudaSuccess) e = B.ctr.grow(1, s);
-  if (e == cudaSuccess && !B.h_ctr) e = B.h_ctr.alloc(1);
-  if (e != cudaSuccess) {
-    cudaGetLastError();                                                   // not sticky: later calls must not see it
-    fb_set_error("%s: cannot allocate the buffers: %s", fn, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
-  CK(cudaEventRecord(m->ev[0], s));
-  CK(cudaMemsetAsync(B.ctr, 0, sizeof(FbCorrCtr), s));
-  CK(fb_corr_launch_mask(m->g, m->cobs, box_lo, box_hi, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, B.mask, s));
-  m->st.kernel_launches += 2;
-  return FIESTA_OK;
-}
-// After the copies out have been enqueued: synchronise and fill the statistics.
-static int corridor_end(fiesta_map *m, const int *box_lo, const int *box_hi, fiesta_corridor_stats *stats) {
-  FbCorrBufs &B = m->corr;
-  CK(cudaEventRecord(m->ev[1], m->stream));
-  CK(cudaMemcpyAsync(B.h_ctr, B.ctr, sizeof(FbCorrCtr), cudaMemcpyDeviceToHost, m->stream));
-  CK(cudaStreamSynchronize(m->stream));
-  if (stats) {
-    *stats = fiesta_corridor_stats{};
-    stats->boxes = (int64_t)B.h_ctr->boxes;
-    stats->layers_tested = (int64_t)B.h_ctr->tested;
-    stats->layers_grown = (int64_t)B.h_ctr->grown;
-    stats->mask_voxels = 1;
-    for (int k = 0; k < 3; ++k) stats->mask_voxels *= (int64_t)(box_hi[k] - box_lo[k] + 1);
-    CK(cudaEventElapsedTime(&stats->ms_compute, m->ev[0], m->ev[1]));
-  }
-  return FIESTA_OK;
-}
-int fiesta_inflate_boxes(fiesta_map *m, const int box_lo[3], const int box_hi[3], const int32_t *seed_lo_xyz, const int32_t *seed_hi_xyz,
-                         int64_t n, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *out_lo_xyz,
-                         int32_t *out_hi_xyz, fiesta_corridor_stats *stats) {
-  const char *fn = "fiesta_inflate_boxes";
-  if (!corridor_args_ok(fn, m, box_lo, box_hi, max_steps, n, clearance, flags, seed_lo_xyz && seed_hi_xyz && status && out_lo_xyz && out_hi_xyz))
-    return FIESTA_ERR_INVALID;
-  if (n >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 seeds per call", fn); return FIESTA_ERR_LIMIT; }
-  if (stats) *stats = fiesta_corridor_stats{};
-  if (n == 0) return FIESTA_OK;
-  int r;
-  if ((r = corridor_begin(m, fn, box_lo, box_hi, clearance, flags, (size_t)n * 6, 0, (size_t)n * 7))) return r;
-  FbCorrBufs &B = m->corr;
-  const cudaStream_t s = m->stream;
-  int32_t *d_st = B.out, *d_lo = d_st + n, *d_hi = d_lo + 3 * n;
-  CK(cudaMemcpyAsync(B.in, seed_lo_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(B.in + 3 * n, seed_hi_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, s));
-  CK(fb_corr_launch_seeds(box_lo, box_hi, max_steps, B.mask, B.in, n, d_st, d_lo, d_hi, B.ctr, s));
-  m->st.kernel_launches++;
-  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(out_lo_xyz, d_lo, (size_t)n * 12, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(out_hi_xyz, d_hi, (size_t)n * 12, cudaMemcpyDeviceToHost, s));
-  return corridor_end(m, box_lo, box_hi, stats);
-}
-int fiesta_corridors(fiesta_map *m, const int box_lo[3], const int box_hi[3], const int32_t *path_vox_xyz, const int64_t *path_off,
-                     int64_t n_paths, const int32_t max_steps[3], double clearance, int flags, int32_t *status, int32_t *n_boxes,
-                     int32_t *blocked_at, int32_t *box_lo_xyz, int32_t *box_hi_xyz, int32_t *first, fiesta_corridor_stats *stats) {
-  const char *fn = "fiesta_corridors";
-  if (!corridor_args_ok(fn, m, box_lo, box_hi, max_steps, n_paths, clearance, flags, path_off && status && n_boxes && blocked_at))
-    return FIESTA_ERR_INVALID;
-  if (n_paths > 0 && path_off[0] != 0) { fb_set_error("%s: path_off[0] must be 0", fn); return FIESTA_ERR_INVALID; }
-  for (int64_t p = 0; p < n_paths; ++p)
-    if (path_off[p + 1] < path_off[p]) { fb_set_error("%s: path_off decreases at %lld", fn, (long long)p); return FIESTA_ERR_INVALID; }
-  const int64_t total = n_paths > 0 ? path_off[n_paths] : 0;
-  if (total > 0 && !(path_vox_xyz && box_lo_xyz && box_hi_xyz && first)) { fb_set_error("%s: null buffer", fn); return FIESTA_ERR_INVALID; }
-  if (total >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 path voxels per call", fn); return FIESTA_ERR_LIMIT; }
-  if (stats) *stats = fiesta_corridor_stats{};
-  if (total == 0) {                                                       // only empty paths: status 0, no boxes
-    for (int64_t p = 0; p < n_paths; ++p) { status[p] = FB_CORR_OK; n_boxes[p] = 0; blocked_at[p] = -1; }
-    return FIESTA_OK;
-  }
-  const size_t T = (size_t)total, np = (size_t)n_paths;
-  int r;
-  if ((r = corridor_begin(m, fn, box_lo, box_hi, clearance, flags, T * 3, np + 1, np * 3 + T * 7))) return r;
-  FbCorrBufs &B = m->corr;
-  const cudaStream_t s = m->stream;
-  int32_t *d_st = B.out, *d_nb = d_st + np, *d_bl = d_nb + np, *d_lo = d_bl + np, *d_hi = d_lo + 3 * T, *d_first = d_hi + 3 * T;
-  CK(cudaMemcpyAsync(B.in, path_vox_xyz, T * 12, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(B.off, path_off, (np + 1) * 8, cudaMemcpyHostToDevice, s));
-  CK(cudaMemsetAsync(d_lo, 0xff, T * 28, s));                            // -1 in every slot no box is written to
-  CK(fb_corr_launch_paths(box_lo, box_hi, max_steps, B.mask, B.in, B.off, n_paths, d_st, d_nb, d_bl, d_lo, d_hi, d_first, B.ctr, s));
-  m->st.kernel_launches++;
-  CK(cudaMemcpyAsync(status, d_st, np * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(n_boxes, d_nb, np * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(blocked_at, d_bl, np * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(box_lo_xyz, d_lo, T * 12, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(box_hi_xyz, d_hi, T * 12, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(first, d_first, T * 4, cudaMemcpyDeviceToHost, s));
-  return corridor_end(m, box_lo, box_hi, stats);
+int alloc_failed(cudaError_t e, const char *fmt, ...) {
+  cudaGetLastError();                                                     // not sticky: later calls must not see it
+  char buf[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  fb_set_error("%s: %s", buf, cudaGetErrorString(e));
+  return FIESTA_ERR_CUDA;
 }
 
 // ---- planner query plan: fixed batch size, pinned host buffers, the copy-in / kernel / copy-out sequence captured once as a
@@ -1678,23 +924,21 @@ struct fiesta_query_plan {
   FbDevBuf<double> d_pos, d_out;
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;
+  ~fiesta_query_plan() {
+    if (exec) cudaGraphExecDestroy(exec);
+    if (graph) cudaGraphDestroy(graph);
+  }
 };
-void fiesta_query_plan_destroy(fiesta_query_plan *p) {
-  if (!p) return;
-  cudaSetDevice(p->m->device);
-  cudaStreamSynchronize(p->m->stream);
-  if (p->exec) cudaGraphExecDestroy(p->exec);
-  if (p->graph) cudaGraphDestroy(p->graph);
-  delete p;
-}
+void fiesta_query_plan_destroy(fiesta_query_plan *p) { handle_destroy(p); }
 int fiesta_query_plan_create(fiesta_map *m, int64_t n, fiesta_query_plan **out) {
   if (!m || !out || n <= 0) { fb_set_error("fiesta_query_plan_create: bad argument"); return FIESTA_ERR_INVALID; }
   if (!m->params_set) { fb_set_error("fiesta_query_plan_create: call SetParameters first (the occupancy threshold is captured)"); return FIESTA_ERR_INVALID; }
   *out = nullptr;
-  CK(cudaSetDevice(m->device));
-  std::unique_ptr<fiesta_query_plan, void (*)(fiesta_query_plan *)> p(new (std::nothrow) fiesta_query_plan(), fiesta_query_plan_destroy);
+  FbHandle<fiesta_query_plan> p;
+  int r;
+  if ((r = handle_new(m, p))) return r;
   if (!p) return FIESTA_ERR_INVALID;
-  p->m = m; p->n = n;
+  p->n = n;
   CK(p->h_pos.alloc((size_t)n * 3));
   CK(p->h_out.alloc((size_t)n * 4));
   CK(p->d_pos.alloc((size_t)n * 3));
@@ -1702,7 +946,7 @@ int fiesta_query_plan_create(fiesta_map *m, int64_t n, fiesta_query_plan **out) 
   CK(cudaStreamSynchronize(m->stream));
   CK(cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal));
   cudaMemcpyAsync(p->d_pos, p->h_pos, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, m->stream);
-  k_query<<<(unsigned)((n + 127) / 128), 128, 0, m->stream>>>(m->g, m->cobs, m->occ, m->l_occ, p->d_pos, n, 1, p->d_out, p->d_out + n);
+  launch_query(m, p->d_pos, n, 1, p->d_out, p->d_out + n, m->stream);
   cudaMemcpyAsync(p->h_out, p->d_out, (size_t)n * 4 * sizeof(double), cudaMemcpyDeviceToHost, m->stream);
   CK(cudaStreamEndCapture(m->stream, &p->graph));
   CK(cudaGraphInstantiate(&p->exec, p->graph, 0));
@@ -1735,9 +979,12 @@ struct fiesta_host_mirror {
   FbDevBuf<unsigned> d_n;
   FbHostBuf<unsigned> h_n;
   int64_t last_changed = 0, last_scanned = 0, refreshes = 0, full_copies = 0;
+  ~fiesta_host_mirror() {
+    if (m && m->mirror == this) m->mirror = nullptr;
+  }
 };
-__global__ void k_mirror_diff(FbGeom g, const uint32_t *cobs, uint32_t *shadow, int lx, int ly, int lz, int ex, int ey, int ez, uint2 *chg,
-                              unsigned cap, unsigned *n) {
+extern "C" __global__ void k_mirror_diff(FbGeom g, const uint32_t *cobs, uint32_t *shadow, int lx, int ly, int lz, int ex, int ey, int ez,
+                                         uint2 *chg, unsigned cap, unsigned *n) {
   const long long vol = (long long)ex * ey * ez;
   for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < vol; t += (long long)gridDim.x * blockDim.x) {
     const int z = lz + (int)(t % ez), y = ly + (int)(t / ez % ey), x = lx + (int)(t / ((long long)ez * ey));
@@ -1749,13 +996,7 @@ __global__ void k_mirror_diff(FbGeom g, const uint32_t *cobs, uint32_t *shadow, 
     if (diff && slot < cap) chg[slot] = make_uint2((unsigned)ii, c);      // on overflow the host falls back to one full copy
   }
 }
-void fiesta_host_mirror_destroy(fiesta_host_mirror *p) {
-  if (!p) return;
-  cudaSetDevice(p->m->device);
-  cudaStreamSynchronize(p->m->stream);
-  if (p->m->mirror == p) p->m->mirror = nullptr;
-  delete p;
-}
+void fiesta_host_mirror_destroy(fiesta_host_mirror *p) { handle_destroy(p); }
 static int mirror_full_copy(fiesta_host_mirror *p) {
   fiesta_map *m = p->m;
   const size_t P = (size_t)m->g.ptotal;
@@ -1769,10 +1010,10 @@ int fiesta_host_mirror_create(fiesta_map *m, fiesta_host_mirror **out) {
   if (!m || !out) { fb_set_error("fiesta_host_mirror_create: null argument"); return FIESTA_ERR_INVALID; }
   *out = nullptr;
   if (m->mirror) { fb_set_error("fiesta_host_mirror_create: this map already has a host mirror"); return FIESTA_ERR_INVALID; }
-  CK(cudaSetDevice(m->device));
-  std::unique_ptr<fiesta_host_mirror, void (*)(fiesta_host_mirror *)> p(new (std::nothrow) fiesta_host_mirror(), fiesta_host_mirror_destroy);
+  FbHandle<fiesta_host_mirror> p;
+  int r;
+  if ((r = handle_new(m, p))) return r;
   if (!p) return FIESTA_ERR_INVALID;
-  p->m = m;
   const size_t P = (size_t)m->g.ptotal;
   size_t cap = P / 32 > (1u << 20) ? P / 32 : (1u << 20);
   if (cap > P) cap = P;
@@ -1783,7 +1024,6 @@ int fiesta_host_mirror_create(fiesta_map *m, fiesta_host_mirror **out) {
   CK(p->d_shadow.alloc(P));
   CK(p->d_chg.alloc(cap));
   CK(p->d_n.alloc(1));
-  int r;
   if ((r = flush_events(m)) || (r = mirror_full_copy(p.get()))) return r;
   p->full_copies = 0;
   m->mirror = p.get();                                                    // the dirty box is kept: the first refresh rescans it
@@ -1855,7 +1095,8 @@ int fiesta_host_mirror_get_dist_grad_trilinear_batch(const fiesta_host_mirror *p
 }
 int fiesta_host_mirror_check_segments(const fiesta_host_mirror *p, const double *ab, int64_t n, double clearance, int flags,
                                       int32_t *status, int64_t *hit_idx, double *hit_t, double *min_dist) {
-  if (!p || !segment_args_ok("fiesta_host_mirror_check_segments", n, clearance, flags, ab && status && hit_idx && hit_t && min_dist)) return FIESTA_ERR_INVALID;
+  const char *fn = "fiesta_host_mirror_check_segments";
+  if (!p || !count_buffers_ok(fn, n, ab && status && hit_idx && hit_t && min_dist) || !clearance_flags_ok(fn, clearance, flags)) return FIESTA_ERR_INVALID;
   const bool unknown_blocks = (flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS) != 0;
   for (int64_t i = 0; i < n; ++i)
     fb_seg_check(p->m->g, p->h_rec, ab + 6 * i, clearance, unknown_blocks, status + i, hit_idx + i, hit_t + i, min_dist + i);
@@ -1995,142 +1236,6 @@ int fiesta_get_slice_marker(fiesta_map *m, int slice, double max_dist, double *x
   return FIESTA_OK;
 }
 
-// ---- map snapshots (format: fb_snapshot.h; kernels: fb_snapshot.cu; DESIGN.md §3.12)
-static FbSnapArrays snap_arrays(fiesta_map *m) {
-  return FbSnapArrays{m->g, m->cobs, m->occ, m->cnt, m->mode == FIESTA_MODE_EXACT ? m->X.LS.p : nullptr};
-}
-// the fiesta_stats counters in snapshot order: every one but kernel_launches (raycast_rounds' slot is not used)
-static int64_t *snap_stat(fiesta_stats &st, int i) {
-  int64_t *f[FB_SNAP_NSTATS] = {&st.occupancy_updates, &st.inserts, &st.deletes, &st.voxels_changed, &st.expansions, &st.voxels_reset,
-                                &st.tile_visits, &st.generations, &st.rays_cast, &st.rays_dropped, &st.ray_voxels, &st.raycast_rounds,
-                                &st.touched_voxels};
-  return f[i];
-}
-static std::vector<unsigned long long> snap_offsets(const FbGeom &g, int exact, const uint32_t *list, size_t n) {
-  std::vector<unsigned long long> off(n + 1);
-  off[0] = 0;
-  for (size_t t = 0; t < n; ++t) off[t + 1] = off[t] + fb_snap_tile_bytes(g.gx, g.gy, g.gz, exact, list[t]);
-  return off;
-}
-int fiesta_snapshot_save(fiesta_map *m, void *buf, int64_t cap, int64_t *size) {
-  const char *fn = "fiesta_snapshot_save";
-  if (!m || !size || cap < 0 || (cap > 0 && !buf)) { fb_set_error("%s: bad argument", fn); return FIESTA_ERR_INVALID; }
-  *size = 0;
-  if (m->n_ev > 0) { fb_set_error("%s: SetOccupancy events are staged (UpdateOccupancy has not run)", fn); return FIESTA_ERR_INVALID; }
-  if (m->n_touch_tiles > 0) { fb_set_error("%s: the occupancy queue is not empty (UpdateOccupancy has not run)", fn); return FIESTA_ERR_INVALID; }
-  if (m->n_ins > 0 || m->n_del > 0) { fb_set_error("%s: inserts or deletes are pending (UpdateESDF has not run)", fn); return FIESTA_ERR_INVALID; }
-  if (m->shard_world > 1) { fb_set_error("%s: an x-slab shard cannot be saved", fn); return FIESTA_ERR_INVALID; }
-  CK(cudaSetDevice(m->device));
-  const FbSnapArrays A = snap_arrays(m);
-  const int exact = m->mode == FIESTA_MODE_EXACT;
-  FbSnapBufs B;
-  unsigned n = 0;
-  int r;
-  if ((r = fb_snap_list_tiles(A, B, &n, m->stream))) return r;
-  m->st.kernel_launches += 2;
-  std::vector<uint32_t> list(n);
-  if (n) {
-    CK(cudaMemcpyAsync(list.data(), B.list, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-    CK(cudaStreamSynchronize(m->stream));
-  }
-  const std::vector<unsigned long long> off = snap_offsets(m->g, exact, list.data(), n);
-  const int64_t depth_pixels = m->image_cnt ? (int64_t)m->d_img[0].cap : 0;
-  FbSnapLayout L;
-  fb_snap_layout(n, off[n], depth_pixels, &L);
-  *size = (int64_t)L.total;
-  if (!buf) return FIESTA_OK;                                             // size query
-  if (cap < *size) { fb_set_error("%s: the buffer holds %lld bytes, the snapshot needs %lld", fn, (long long)cap, (long long)*size); return FIESTA_ERR_LIMIT; }
-  uint8_t *p = static_cast<uint8_t *>(buf);
-  int launches = 0;
-  if ((r = fb_snap_pack(A, B, off, p + L.payload_off, m->stream, &launches))) return r;
-  m->st.kernel_launches += launches;
-  memset(p + L.list_off, 0, L.payload_off - L.list_off);
-  for (unsigned t = 0; t < n; ++t) fb_snap_st32(p + L.list_off + 4 * t, list[t]);
-  memset(p + L.depth_off, 0, L.depth_bytes);
-  if (depth_pixels) {
-    CK(cudaMemcpyAsync(p + L.depth_off, m->d_img[m->image_cnt & 1], (size_t)depth_pixels * 2, cudaMemcpyDeviceToHost, m->stream));
-    CK(cudaStreamSynchronize(m->stream));
-  }
-  FbSnapHeader h{};
-  h.version = FB_SNAP_VERSION; h.mode = (uint32_t)m->mode;
-  for (int i = 0; i < 3; ++i) {
-    h.origin[i] = m->cfg.origin[i]; h.map_size[i] = m->cfg.map_size[i];
-    h.min_vec[i] = m->g.min_vec[i]; h.max_vec[i] = m->g.max_vec[i]; h.last_min_vec[i] = m->g.last_min_vec[i]; h.last_max_vec[i] = m->g.last_max_vec[i];
-  }
-  h.resolution = m->cfg.resolution;
-  h.grid[0] = m->g.gx; h.grid[1] = m->g.gy; h.grid[2] = m->g.gz;
-  h.params_set = m->params_set ? 1 : 0;
-  h.l_hit = m->l_hit; h.l_miss = m->l_miss; h.l_min = m->l_min; h.l_max = m->l_max; h.l_occ = m->l_occ;
-  h.flags = m->local_box_seen ? FB_SNAP_LOCAL_BOX_SEEN : 0u;
-  h.image_cnt = m->image_cnt;
-  h.tclock = exact ? m->X.tclock : 0; h.key_base = exact ? m->X.key_base : 0;
-  for (int i = 0; i < FB_SNAP_NSTATS; ++i) h.stats[i] = i == FB_SNAP_STAT_ROUNDS ? 0 : *snap_stat(m->st, i);
-  h.depth_pixels = depth_pixels;
-  h.n_tiles = n;
-  h.list_sum = fb_snap_checksum(p + L.list_off, (L.payload_off - L.list_off) / 8);
-  h.depth_sum = fb_snap_checksum(p + L.depth_off, L.depth_bytes / 8);
-  fb_snap_encode(h, p);
-  return FIESTA_OK;
-}
-int fiesta_snapshot_load(const void *buf, int64_t size, int32_t device, fiesta_map **out) {
-  const char *fn = "fiesta_snapshot_load";
-  if (!out) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
-  *out = nullptr;
-  if (!buf || size < 0) { fb_set_error("%s: bad argument", fn); return FIESTA_ERR_INVALID; }
-  const uint8_t *p = static_cast<const uint8_t *>(buf);
-  FbSnapHeader h;
-  FbSnapLayout L;
-  char err[256];
-  if (fb_snap_parse(p, size, &h, &L, err, (int)sizeof(err))) { fb_set_error("%s: %s", fn, err); return FIESTA_ERR_INVALID; }
-  fiesta_config cfg{};
-  for (int i = 0; i < 3; ++i) { cfg.origin[i] = h.origin[i]; cfg.map_size[i] = h.map_size[i]; }
-  cfg.resolution = h.resolution; cfg.device = device; cfg.mode = (int32_t)h.mode;
-  fiesta_map *raw = nullptr;
-  int r;
-  if ((r = create_map(&cfg, &raw, false))) return r;                     // the mode is the snapshot's, whatever FIESTA_B200_MODE says
-  std::unique_ptr<fiesta_map, void (*)(fiesta_map *)> m(raw, fiesta_destroy);   // destroyed on any failure below
-  FbGeom &g = m->g;
-  if (g.gx != h.grid[0] || g.gy != h.grid[1] || g.gz != h.grid[2]) { fb_set_error("%s: the rebuilt grid differs from the stored one", fn); return FIESTA_ERR_INVALID; }
-  m->params_set = h.params_set != 0;
-  m->l_hit = h.l_hit; m->l_miss = h.l_miss; m->l_min = h.l_min; m->l_max = h.l_max; m->l_occ = h.l_occ;
-  for (int i = 0; i < 3; ++i) {
-    g.min_vec[i] = h.min_vec[i]; g.max_vec[i] = h.max_vec[i]; g.last_min_vec[i] = h.last_min_vec[i]; g.last_max_vec[i] = h.last_max_vec[i];
-  }
-  set_box_flag(g);
-  m->local_box_seen = (h.flags & FB_SNAP_LOCAL_BOX_SEEN) != 0;
-  if (m->mode == FIESTA_MODE_EXACT) { m->X.tclock = h.tclock; m->X.key_base = h.key_base; }
-  for (int i = 0; i < FB_SNAP_NSTATS; ++i) if (i != FB_SNAP_STAT_ROUNDS) *snap_stat(m->st, i) = h.stats[i];
-  std::vector<uint32_t> list((size_t)h.n_tiles);
-  for (size_t t = 0; t < list.size(); ++t) list[t] = fb_snap_ld32(p + L.list_off + 4 * t);
-  const std::vector<unsigned long long> off = snap_offsets(g, m->mode == FIESTA_MODE_EXACT, list.data(), list.size());
-  FbSnapBufs B;
-  unsigned bad = 0, why = 0;
-  int launches = 0;
-  if ((r = fb_snap_unpack(snap_arrays(m.get()), B, list.data(), off, p + L.payload_off, h.tclock, &bad, &why, m->stream, &launches))) return r;
-  m->st.kernel_launches += launches;
-  if (why) {
-    fb_set_error("%s: stored tile %u (grid tile %u) is malformed:%s%s%s%s%s%s", fn, bad, list[bad], (why & FB_SNAP_BAD_SUM) ? " checksum mismatch;" : "",
-                 (why & FB_SNAP_BAD_COBS) ? " closest-obstacle record outside the grid;" : "", (why & FB_SNAP_BAD_BIT31) ? " bad bit 31 of a record;" : "",
-                 (why & FB_SNAP_BAD_OCC) ? " log-odds not finite;" : "", (why & FB_SNAP_BAD_LS) ? " relink time not below the relink clock;" : "",
-                 (why & FB_SNAP_BAD_CNT) ? " more hits than observations;" : "");
-    return FIESTA_ERR_INVALID;
-  }
-  // rebuilt, not stored: the Exist() bitmap, and FAST mode's staging copy of the records
-  const size_t words = ((size_t)g.ptotal + 31) / 32;
-  k_rebuild_occbits<<<(unsigned)((words + 255) / 256), 256, 0, m->stream>>>(m->occ, g.ptotal, m->l_occ, m->occbits);
-  m->st.kernel_launches++;
-  CK(cudaGetLastError());
-  if (m->mode == FIESTA_MODE_FAST) CK(cudaMemcpyAsync(m->cobs_b, m->cobs, (size_t)g.ptotal * 4, cudaMemcpyDeviceToDevice, m->stream));
-  if (h.depth_pixels > 0) {
-    if ((r = alloc_depth(m.get(), (size_t)h.depth_pixels))) return r;
-    CK(cudaMemcpyAsync(m->d_img[h.image_cnt & 1], p + L.depth_off, (size_t)h.depth_pixels * 2, cudaMemcpyHostToDevice, m->stream));
-  }
-  m->image_cnt = h.image_cnt;
-  CK(cudaStreamSynchronize(m->stream));
-  *out = m.release();
-  return FIESTA_OK;
-}
-
 int fiesta_get_stats(fiesta_map *m, fiesta_stats *out) {
   if (!m || !out) return FIESTA_ERR_INVALID;
   *out = m->st;
@@ -2143,4 +1248,3 @@ int fiesta_synchronize(fiesta_map *m) {
   return FIESTA_OK;
 }
 
-}  // extern "C"

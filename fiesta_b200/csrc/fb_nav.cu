@@ -16,7 +16,7 @@
 // voxel -- a goal placed by k_nav_goals included -- always queues every tile holding one of its 26 neighbours, so when the list is empty no voxel can improve; fl-addition is
 // monotone, so that fixpoint is the least one, the same bits a sequential Dijkstra gives, whatever the tile schedule.
 #include <cooperative_groups.h>
-#include "fb_common.cuh"
+#include "fb_nav.cuh"
 #include "fb_segment.h"
 
 namespace cg = cooperative_groups;
@@ -405,15 +405,23 @@ static unsigned nav_blocks(long long n) {
   return (unsigned)(want < FB_SMS * 16ll ? want : FB_SMS * 16ll);
 }
 
-int fb_nav_relax_blocks(int device) {
+static int nav_relax_blocks(int device) {
   int per_sm = 0, sms = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_nav_relax, NAV_THREADS, 0) != cudaSuccess) return 0;
   if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
   return per_sm * sms;                                                    // every block co-resident: required by grid.sync()
 }
 
-cudaError_t fb_nav_compute(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, const double *goals, long long n_goals, double r,
-                           int unknown_blocks, int nblocks, cudaStream_t s) {
+static int nav_withdraw_blocks(int device) {
+  int per_sm = 0, sms = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_navu_withdraw, NAV_THREADS, 0) != cudaSuccess) return 0;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
+  return per_sm * sms;
+}
+
+// The whole compute on stream s: 3 launches, 4 with goals.  Expects the stamps and a.ctr zeroed.
+static cudaError_t nav_compute_launch(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, const double *goals, long long n_goals,
+                                      double r, int unknown_blocks, int nblocks, cudaStream_t s) {
   const long long n = (long long)a.b.n[0] * a.b.n[1] * a.b.n[2];
   k_nav_init<<<nav_blocks(n), 256, 0, s>>>(g, cobs, a, r, unknown_blocks);
   if (n_goals > 0) k_nav_goals<<<(unsigned)((n_goals + 127) / 128), 128, 0, s>>>(g, a, goals, n_goals);
@@ -425,16 +433,10 @@ cudaError_t fb_nav_compute(const FbGeom &g, const uint32_t *cobs, const FbNavArg
   return cudaGetLastError();
 }
 
-int fb_nav_withdraw_blocks(int device) {
-  int per_sm = 0, sms = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_navu_withdraw, NAV_THREADS, 0) != cudaSuccess) return 0;
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
-  return per_sm * sms;
-}
-
 // The whole update on stream s: 5 launches, 6 with goals.  a.D holds the old field; a.ctr and u are cleared here.
-cudaError_t fb_nav_update(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, uint8_t *flags, FbNavUCtr *u, const double *goals,
-                          long long n_goals, double r, int unknown_blocks, int nblocks, int wblocks, cudaStream_t s) {
+static cudaError_t nav_update_launch(const FbGeom &g, const uint32_t *cobs, const FbNavArgs &a, uint8_t *flags, FbNavUCtr *u,
+                                     const double *goals, long long n_goals, double r, int unknown_blocks, int nblocks, int wblocks,
+                                     cudaStream_t s) {
   const long long n = (long long)a.b.n[0] * a.b.n[1] * a.b.n[2];
   const size_t nt = (size_t)a.tn[0] * a.tn[1] * a.tn[2];
   FbNavArgs w = a;                                                        // the wave: same lists and stamps, its own counters
@@ -446,7 +448,7 @@ cudaError_t fb_nav_update(const FbGeom &g, const uint32_t *cobs, const FbNavArgs
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   void *wargs[] = {(void *)&w, (void *)&flags};
   if ((e = cudaLaunchCooperativeKernel((void *)k_navu_withdraw, dim3(wblocks), dim3(NAV_THREADS), wargs, 0, s)) != cudaSuccess) return e;
-  // old costs are read until here; the re-relaxation starts from clean stamps and counters, as in fb_nav_compute
+  // old costs are read until here; the re-relaxation starts from clean stamps and counters, as in fiesta_nav_compute
   if ((e = cudaMemsetAsync(a.stamp, 0, nt * 4, s)) != cudaSuccess) return e;
   if ((e = cudaMemsetAsync(a.ctr, 0, sizeof(FbNavCtr), s)) != cudaSuccess) return e;
   k_navu_apply<<<nav_blocks(n), 256, 0, s>>>(a, flags, u);
@@ -459,9 +461,162 @@ cudaError_t fb_nav_update(const FbGeom &g, const uint32_t *cobs, const FbNavArgs
   return cudaGetLastError();
 }
 
-cudaError_t fb_nav_paths(const FbGeom &g, const FbNavBox &b, const double *D, const double *w, const double *starts, long long n, int max_len,
-                         int32_t *status, int32_t *len, double *cost, int32_t *vox, cudaStream_t s) {
-  if (n <= 0) return cudaSuccess;
-  k_nav_path<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(g, b, D, w[0], w[1], w[2], starts, n, max_len, status, len, cost, vox);
-  return cudaGetLastError();
+// ---------------------------------------------------------------- entry points (include/fiesta_b200.h)
+void fiesta_nav_destroy(fiesta_nav_field *f) { handle_destroy(f); }
+int fiesta_nav_create(fiesta_map *m, fiesta_nav_field **out) {
+  if (!m || !out) { fb_set_error("fiesta_nav_create: null argument"); return FIESTA_ERR_INVALID; }
+  *out = nullptr;
+  FbHandle<fiesta_nav_field> f;
+  int r;
+  if ((r = handle_new(m, f))) return r;
+  if (!f) { fb_set_error("out of host memory"); return FIESTA_ERR_INVALID; }
+  f->blocks = nav_relax_blocks(m->device);
+  f->mblocks = fb_navm_relax_blocks(m->device);
+  f->wblocks = nav_withdraw_blocks(m->device);
+  if (f->blocks <= 0 || f->mblocks <= 0 || f->wblocks <= 0) { fb_set_error("fiesta_nav_create: the relaxation kernel does not fit on this device"); return FIESTA_ERR_CUDA; }
+  for (cudaEvent_t &e : f->ev) CK(cudaEventCreate(&e));
+  CK(f->ctr.alloc(1));
+  CK(f->h_ctr.alloc(1));
+  CK(f->m_ctr.alloc(1));
+  CK(f->m_tot.alloc(1));
+  CK(f->h_mtot.alloc(1));
+  CK(f->u_ctr.alloc(1));
+  CK(f->h_uctr.alloc(1));
+  for (int k = 0; k < 3; ++k) f->w[k] = m->g.res * sqrt((double)(k + 1));
+  *out = f.release();
+  return FIESTA_OK;
+}
+int fiesta_nav_compute(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *goals_xyz, int64_t n_goals,
+                       double clearance, int flags, fiesta_nav_stats *stats) {
+  const char *fn = "fiesta_nav_compute";
+  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (!count_buffers_ok(fn, n_goals, goals_xyz != nullptr) || !clearance_flags_ok(fn, clearance, flags)) return FIESTA_ERR_INVALID;
+  fiesta_map *m = f->m;
+  const FbGeom &g = m->g;
+  FbNavArgs a{};
+  if (!box_arg(fn, g, box_lo, box_hi, &a.b)) return FIESTA_ERR_INVALID;
+  for (int k = 0; k < 3; ++k) {
+    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
+    a.w[k] = f->w[k];
+  }
+  const size_t nv = (size_t)a.b.n[0] * a.b.n[1] * a.b.n[2], nt = (size_t)a.tn[0] * a.tn[1] * a.tn[2];
+  CK(cudaSetDevice(m->device));
+  f->valid = false;
+  cudaError_t e = f->D.grow(nv, m->stream);
+  for (FbDevBuf<uint32_t> *b : {&f->stamp, &f->list[0], &f->list[1]})
+    if (e == cudaSuccess) e = b->grow(nt, m->stream);
+  if (e == cudaSuccess && n_goals > 0) e = f->d_goals.grow((size_t)n_goals * 3, m->stream);
+  if (e != cudaSuccess) return alloc_failed(e, "%s: cannot allocate the field of %zu voxels", fn, nv);
+  a.D = f->D; a.stamp = f->stamp; a.list[0] = f->list[0]; a.list[1] = f->list[1]; a.ctr = f->ctr;
+  if (n_goals > 0) CK(cudaMemcpyAsync(f->d_goals, goals_xyz, (size_t)n_goals * 24, cudaMemcpyHostToDevice, m->stream));
+  CK(cudaMemsetAsync(f->stamp, 0, nt * 4, m->stream));
+  CK(cudaMemsetAsync(f->ctr, 0, sizeof(FbNavCtr), m->stream));
+  CK(cudaEventRecord(f->ev[0], m->stream));
+  CK(nav_compute_launch(g, m->cobs, a, f->d_goals, n_goals, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, f->blocks, m->stream));
+  m->st.kernel_launches += n_goals > 0 ? 4 : 3;
+  CK(cudaEventRecord(f->ev[1], m->stream));
+  CK(cudaMemcpyAsync(f->h_ctr, f->ctr, sizeof(FbNavCtr), cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  f->box = a.b;
+  f->valid = true;
+  f->n_goals = n_goals;
+  f->clearance = clearance;
+  f->flags = flags;
+  if (stats) {
+    const FbNavCtr &c = *f->h_ctr;
+    *stats = fiesta_nav_stats{};
+    stats->box_voxels = (int64_t)nv;
+    stats->blocked = (int64_t)c.blocked;
+    stats->reached = (int64_t)c.reached;
+    stats->goals_placed = (int64_t)c.goals_placed;
+    stats->generations = (int64_t)c.generations;
+    stats->tile_visits = (int64_t)c.tile_visits;
+    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
+  }
+  return FIESTA_OK;
+}
+int fiesta_nav_update(fiesta_nav_field *f, fiesta_nav_update_stats *stats) {
+  const char *fn = "fiesta_nav_update";
+  if (!f) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (!f->valid) { fb_set_error("%s: no field has been computed", fn); return FIESTA_ERR_INVALID; }
+  fiesta_map *m = f->m;
+  FbNavArgs a{};
+  a.b = f->box;
+  for (int k = 0; k < 3; ++k) {
+    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
+    a.w[k] = f->w[k];
+  }
+  const size_t nv = (size_t)a.b.n[0] * a.b.n[1] * a.b.n[2];
+  CK(cudaSetDevice(m->device));
+  if (cudaError_t e = f->u_flags.grow(nv, m->stream))                    // before anything is written: the field stays valid
+    return alloc_failed(e, "%s: cannot allocate the scratch of %zu voxels", fn, nv);
+  a.D = f->D; a.stamp = f->stamp; a.list[0] = f->list[0]; a.list[1] = f->list[1]; a.ctr = f->ctr;
+  f->valid = false;                                                       // until the update has finished
+  CK(cudaEventRecord(f->ev[0], m->stream));
+  CK(nav_update_launch(m->g, m->cobs, a, f->u_flags, f->u_ctr, f->d_goals, f->n_goals, f->clearance, f->flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS,
+                       f->blocks, f->wblocks, m->stream));
+  m->st.kernel_launches += f->n_goals > 0 ? 6 : 5;
+  CK(cudaEventRecord(f->ev[1], m->stream));
+  CK(cudaMemcpyAsync(f->h_ctr, f->ctr, sizeof(FbNavCtr), cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(f->h_uctr, f->u_ctr, sizeof(FbNavUCtr), cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  f->valid = true;
+  if (stats) {
+    const FbNavCtr &c = *f->h_ctr;
+    const FbNavUCtr &u = *f->h_uctr;
+    *stats = fiesta_nav_update_stats{};
+    stats->box_voxels = (int64_t)nv;
+    stats->became_blocked = (int64_t)u.became_blocked;
+    stats->became_free = (int64_t)u.became_free;
+    stats->withdrawn = (int64_t)u.withdrawn;
+    stats->goals_placed = (int64_t)c.goals_placed;
+    stats->goals_new = (int64_t)u.goals_new;
+    stats->seed_tiles = (int64_t)u.seed_tiles;
+    stats->withdraw_generations = (int64_t)u.wave.generations;
+    stats->generations = (int64_t)c.generations;
+    stats->tile_visits = (int64_t)c.tile_visits;
+    stats->blocked = (int64_t)c.blocked;
+    stats->reached = (int64_t)c.reached;
+    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
+  }
+  return FIESTA_OK;
+}
+int fiesta_nav_export(const fiesta_nav_field *f, double *out) {
+  if (!f || !out) { fb_set_error("fiesta_nav_export: null argument"); return FIESTA_ERR_INVALID; }
+  if (!f->valid) { fb_set_error("fiesta_nav_export: no field has been computed"); return FIESTA_ERR_INVALID; }
+  const fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  CK(cudaMemcpyAsync(out, f->D, (size_t)f->box.n[0] * f->box.n[1] * f->box.n[2] * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+int fiesta_nav_paths(fiesta_nav_field *f, const double *starts_xyz, int64_t n, int32_t max_len, int32_t *status, int32_t *len, double *cost,
+                     int32_t *vox_xyz) {
+  const char *fn = "fiesta_nav_paths";
+  if (!f || n < 0 || max_len < 1 || (n > 0 && !(starts_xyz && status && len && cost && vox_xyz))) {
+    fb_set_error("%s: null buffer, negative count or max_len < 1", fn);
+    return FIESTA_ERR_INVALID;
+  }
+  if (!f->valid) { fb_set_error("%s: no field has been computed", fn); return FIESTA_ERR_INVALID; }
+  if (n == 0) return FIESTA_OK;
+  fiesta_map *m = f->m;
+  CK(cudaSetDevice(m->device));
+  const size_t nv = (size_t)n * max_len * 3;
+  cudaError_t e = f->d_pd.grow((size_t)n * 4, m->stream);
+  if (e == cudaSuccess) e = f->d_pi.grow((size_t)n * 2 + nv, m->stream);
+  if (e != cudaSuccess) return alloc_failed(e, "%s: cannot allocate %lld paths of %d voxels", fn, (long long)n, (int)max_len);
+  double *d_starts = f->d_pd, *d_cost = d_starts + 3 * n;
+  int32_t *d_st = f->d_pi, *d_len = d_st + n, *d_vox = d_len + n;
+  CK(cudaMemcpyAsync(d_starts, starts_xyz, (size_t)n * 24, cudaMemcpyHostToDevice, m->stream));
+  CK(cudaMemsetAsync(d_vox, 0xff, nv * 4, m->stream));                    // -1 past each path's end
+  k_nav_path<<<(unsigned)((n + 127) / 128), 128, 0, m->stream>>>(m->g, f->box, f->D, f->w[0], f->w[1], f->w[2], d_starts, n, max_len, d_st,
+                                                                 d_len, d_cost, d_vox);
+  CK(cudaGetLastError());
+  m->st.kernel_launches++;
+  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(len, d_len, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(cost, d_cost, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(vox_xyz, d_vox, nv * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
 }

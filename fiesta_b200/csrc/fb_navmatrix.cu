@@ -15,7 +15,10 @@
 // decrease, a decrease of a boundary voxel queues every tile that holds one of its neighbours, and the least fixpoint does not
 // depend on the schedule.  Retirement only drops work whose writes could not reach a target any more.
 #include <cooperative_groups.h>
-#include "fb_common.cuh"
+#include <string.h>
+#include <algorithm>
+#include <vector>
+#include "fb_nav.cuh"
 #include "fb_segment.h"
 
 namespace cg = cooperative_groups;
@@ -257,8 +260,9 @@ int fb_navm_relax_blocks(int device) {
   return per_sm * sms;                                                  // every block co-resident: required by grid.sync()
 }
 
-cudaError_t fb_navm_locate(const FbGeom &g, const uint32_t *cobs, const FbNavBox &b, double r, int unknown_blocks, uint32_t *M,
-                           const double *pts, long long n, int32_t *status, long long *idx, cudaStream_t s) {
+// 2 launches, 3 with points
+static cudaError_t navm_locate(const FbGeom &g, const uint32_t *cobs, const FbNavBox &b, double r, int unknown_blocks, uint32_t *M,
+                               const double *pts, long long n, int32_t *status, long long *idx, cudaStream_t s) {
   const long long nv = (long long)b.n[0] * b.n[1] * b.n[2];
   k_navm_trav<<<navm_blocks(nv), 256, 0, s>>>(g, cobs, b, r, unknown_blocks, M);
   k_navm_mask<<<navm_blocks(nv), 256, 0, s>>>(b, M);
@@ -266,8 +270,8 @@ cudaError_t fb_navm_locate(const FbGeom &g, const uint32_t *cobs, const FbNavBox
   return cudaGetLastError();
 }
 
-// One pass: a.nch channels, sources src_idx[0 .. nch); expects ctr zeroed and stamp zeroed on the pass's items.
-cudaError_t fb_navm_pass(const FbNavMArgs &a, const long long *src_idx, int nblocks, cudaStream_t s) {
+// One pass, 3 launches: a.nch channels, sources src_idx[0 .. nch); expects ctr zeroed and stamp zeroed on the pass's items.
+static cudaError_t navm_pass(const FbNavMArgs &a, const long long *src_idx, int nblocks, cudaStream_t s) {
   k_navm_fill<<<navm_blocks(a.nch * a.nv), 256, 0, s>>>(a.D, a.nch * a.nv);
   k_navm_place<<<1, FB_NAVM_CH, 0, s>>>(a, src_idx);
   cudaError_t e = cudaGetLastError();
@@ -276,10 +280,133 @@ cudaError_t fb_navm_pass(const FbNavMArgs &a, const long long *src_idx, int nblo
   return cudaLaunchCooperativeKernel((void *)k_navm_relax, dim3(nblocks), dim3(NAVM_THREADS), args, 0, s);
 }
 
-cudaError_t fb_navm_gather(const double *D, long long nv, const int32_t *rows, long long n_rows, const long long *tgt_idx, long long n_tgt,
-                           double *cost, cudaStream_t s) {
+static cudaError_t navm_gather(const double *D, long long nv, const int32_t *rows, long long n_rows, const long long *tgt_idx,
+                               long long n_tgt, double *cost, cudaStream_t s) {
   const long long n = n_rows * n_tgt;
   if (n <= 0) return cudaSuccess;
   k_navm_gather<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(D, nv, rows, n_rows, tgt_idx, n_tgt, cost);
   return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------- entry point (include/fiesta_b200.h)
+int fiesta_nav_matrix(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *sources_xyz, int64_t n_src,
+                      const double *targets_xyz, int64_t n_tgt, double clearance, int flags, int32_t *src_status, int32_t *tgt_status,
+                      double *cost, fiesta_nav_matrix_stats *stats) {
+  const char *fn = "fiesta_nav_matrix";
+  if (!f || !box_lo || !box_hi) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (n_src < 0 || n_tgt < 0 || (n_src > 0 && !(sources_xyz && src_status)) || (n_tgt > 0 && !(targets_xyz && tgt_status)) ||
+      (n_src > 0 && n_tgt > 0 && !cost)) {
+    fb_set_error("%s: negative count or null buffer", fn);
+    return FIESTA_ERR_INVALID;
+  }
+  if (!clearance_flags_ok(fn, clearance, flags)) return FIESTA_ERR_INVALID;
+  fiesta_map *m = f->m;
+  FbNavMArgs a{};
+  if (!box_arg(fn, m->g, box_lo, box_hi, &a.b)) return FIESTA_ERR_INVALID;
+  for (int k = 0; k < 3; ++k) {
+    a.tn[k] = (a.b.n[k] + FB_TILE - 1) / FB_TILE;
+    a.w[k] = f->w[k];
+  }
+  if (n_src > 0 && n_tgt > 0 && n_src >= ((1ll << 31) + n_tgt - 1) / n_tgt) {
+    fb_set_error("%s: n_src * n_tgt must be below 2^31", fn);
+    return FIESTA_ERR_LIMIT;
+  }
+  const long long nv = (long long)a.b.n[0] * a.b.n[1] * a.b.n[2], nt = (long long)a.tn[0] * a.tn[1] * a.tn[2], np = n_src + n_tgt;
+  a.nv = nv;
+  a.nt = (unsigned)nt;
+  cudaStream_t s = m->stream;
+  CK(cudaSetDevice(m->device));
+  // (1) move masks, statuses and box indices of every point; the statuses and indices come back for the host to plan the passes
+  cudaError_t e = f->M.grow((size_t)nv, s);
+  if (e == cudaSuccess && np > 0) e = f->m_pts.grow((size_t)np * 3, s);
+  if (e == cudaSuccess && np > 0) e = f->m_st.grow((size_t)np, s);
+  if (e == cudaSuccess && np > 0) e = f->m_idx.grow((size_t)np, s);
+  if (e != cudaSuccess) return alloc_failed(e, "%s: cannot allocate the move masks of %lld voxels", fn, nv);
+  CK(cudaEventRecord(f->ev[0], s));
+  if (n_src > 0) CK(cudaMemcpyAsync(f->m_pts, sources_xyz, (size_t)n_src * 24, cudaMemcpyHostToDevice, s));
+  if (n_tgt > 0) CK(cudaMemcpyAsync(f->m_pts + 3 * n_src, targets_xyz, (size_t)n_tgt * 24, cudaMemcpyHostToDevice, s));
+  CK(navm_locate(m->g, m->cobs, a.b, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, f->M, f->m_pts, np, f->m_st, f->m_idx, s));
+  m->st.kernel_launches += np > 0 ? 3 : 2;
+  std::vector<int32_t> st((size_t)np);
+  std::vector<long long> idx((size_t)np);
+  if (np > 0) {
+    CK(cudaMemcpyAsync(st.data(), f->m_st, (size_t)np * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(idx.data(), f->m_idx, (size_t)np * 8, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  // rows: the placed sources in index order (channel k of the passes is placed source k), then the others (NaN rows)
+  std::vector<int32_t> rows;
+  std::vector<long long> src, tgt;
+  long long n_ps = 0;
+  for (long long i = 0; i < n_src; ++i) n_ps += st[i] == FB_NAVM_PLACED;
+  if (n_tgt > 0) {                                                         // then n_src < 2^31
+    for (long long i = 0; i < n_src; ++i)
+      if (st[i] == FB_NAVM_PLACED) { rows.push_back((int32_t)i); src.push_back(idx[i]); }
+    for (long long i = 0; i < n_src; ++i)
+      if (st[i] != FB_NAVM_PLACED) rows.push_back((int32_t)i);
+  }
+  for (long long j = n_src; j < np; ++j)
+    if (st[j] == FB_NAVM_PLACED) tgt.push_back(idx[j]);
+  const long long n_pt = (long long)tgt.size();
+  // (2) passes of C channels: C = min(32, sources left, max(1, floor(2^32 B / (8 B x box voxels))))
+  const long long per_pass = std::max(1ll, std::min((long long)FB_NAVM_CH, (1ll << 32) / (8 * nv)));
+  const long long C = std::min(per_pass, n_ps);
+  const bool work = n_ps > 0 && n_pt > 0;
+  if (work && C * nt >= (long long)0xffffffffu) {
+    fb_set_error("%s: the box has too many tiles", fn);
+    return FIESTA_ERR_LIMIT;
+  }
+  e = cudaSuccess;
+  if (n_src > 0 && n_tgt > 0) e = f->m_cost.grow((size_t)(n_src * n_tgt), s);
+  if (e == cudaSuccess && n_src > 0 && n_tgt > 0) e = f->m_rows.grow((size_t)n_src, s);
+  if (work) {
+    if (e == cudaSuccess) e = f->MD.grow((size_t)(C * nv), s);
+    for (FbDevBuf<uint32_t> *b : {&f->m_stamp, &f->m_list[0], &f->m_list[1]})
+      if (e == cudaSuccess) e = b->grow((size_t)(C * nt), s);
+    if (e == cudaSuccess) e = f->m_src.grow((size_t)n_ps, s);
+    if (e == cudaSuccess) e = f->m_tgt.grow((size_t)n_pt, s);
+  }
+  if (e != cudaSuccess)
+    return alloc_failed(e, "%s: cannot allocate %lld fields of %lld voxels and the %lld x %lld matrix", fn, C, nv, (long long)n_src, (long long)n_tgt);
+  if (n_src > 0 && n_tgt > 0) CK(cudaMemcpyAsync(f->m_rows, rows.data(), (size_t)n_src * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(f->m_tot, 0, sizeof(FbNavMTot), s));
+  long long passes = 0;
+  if (work) {
+    CK(cudaMemcpyAsync(f->m_src, src.data(), (size_t)n_ps * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(f->m_tgt, tgt.data(), (size_t)n_pt * 8, cudaMemcpyHostToDevice, s));
+    a.D = f->MD; a.M = f->M; a.stamp = f->m_stamp; a.list[0] = f->m_list[0]; a.list[1] = f->m_list[1];
+    a.ctr = f->m_ctr; a.tot = f->m_tot; a.tgt = f->m_tgt; a.n_tgt = (int)n_pt;
+    for (long long p0 = 0; p0 < n_ps; p0 += C, ++passes) {
+      a.nch = (int)std::min(C, n_ps - p0);
+      CK(cudaMemsetAsync(f->m_stamp, 0, (size_t)(a.nch * nt) * 4, s));
+      CK(cudaMemsetAsync(f->m_ctr, 0, sizeof(FbNavMCtr), s));
+      CK(navm_pass(a, f->m_src + p0, f->mblocks, s));
+      CK(navm_gather(f->MD, nv, f->m_rows + p0, a.nch, f->m_idx + n_src, n_tgt, f->m_cost, s));
+      m->st.kernel_launches += 4;
+    }
+  }
+  // NaN rows: every source when no target is placed, else the sources not placed
+  const long long nan_from = work ? n_ps : 0;
+  if (n_src > nan_from && n_tgt > 0) {
+    CK(navm_gather(nullptr, nv, f->m_rows + nan_from, n_src - nan_from, f->m_idx + n_src, n_tgt, f->m_cost, s));
+    m->st.kernel_launches++;
+  }
+  CK(cudaEventRecord(f->ev[1], s));
+  if (n_src > 0 && n_tgt > 0) CK(cudaMemcpyAsync(cost, f->m_cost, (size_t)(n_src * n_tgt) * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(f->h_mtot, f->m_tot, sizeof(FbNavMTot), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (n_src > 0) memcpy(src_status, st.data(), (size_t)n_src * 4);
+  if (n_tgt > 0) memcpy(tgt_status, st.data() + n_src, (size_t)n_tgt * 4);
+  if (stats) {
+    const FbNavMTot &t = *f->h_mtot;
+    *stats = fiesta_nav_matrix_stats{};
+    stats->sources_placed = n_ps;
+    stats->targets_placed = n_pt;
+    stats->passes = passes;
+    stats->generations = (int64_t)t.generations;
+    stats->tile_visits = (int64_t)t.tile_visits;
+    stats->sources_retired_early = (int64_t)t.retired_early;
+    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
+  }
+  return FIESTA_OK;
 }

@@ -15,7 +15,7 @@
 // warp waiting for its largest pose, and a warp per pose would idle most lanes on small ones; items of about FB_POSE_CHUNK
 // voxels balance both.  All outputs are integer sums, minima and flags of per-voxel decisions: they do not depend on the schedule.
 #include <cub/cub.cuh>
-#include "fb_common.cuh"
+#include "fb_map.h"
 #include "fb_pose.h"
 #include "fb_view.h"      // fb_view_find: the owner of a position in a flat work list
 
@@ -139,23 +139,20 @@ __global__ void k_pose_finish(long long n, int32_t *status, const int32_t *__res
   hit_idx[i] = -1;
 }
 
-// ---------------------------------------------------------------- host side
-int fb_pose_check_batch(const FbGeom &g, const uint32_t *cobs, const double *poses, long long n, const double *h, double clearance,
-                        int unknown_blocks, int32_t *status, int32_t *n_blocked, int64_t *hit_idx, FbPoseBufs &B, cudaStream_t s,
-                        int *launches) {
+// ---------------------------------------------------------------- entry points (include/fiesta_b200.h)
+// Both forms, validated (fb_pose.h limits), on device buffers: the four launches on stream s.
+static int poses_launch(fiesta_map *m, const double *poses, long long n, const double *h, double clearance, int flags, int32_t *status,
+                        int32_t *n_blocked, int64_t *hit_idx, cudaStream_t s) {
   if (n <= 0) return FIESTA_OK;
+  FbPoseBufs &B = m->pose;
   const FbPoseBody body = {{h[0], h[1], h[2]}};
   size_t bytes = 0;
   CK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, B.work.p, B.work.p, (int)(n + 1), s));
   cudaError_t e = B.work.grow((size_t)n + 1, s);
   if (e == cudaSuccess) e = B.tmp.grow(bytes ? bytes : 16, s);
-  if (e != cudaSuccess) {
-    cudaGetLastError();                                                   // not sticky: later calls must not see it
-    fb_set_error("fiesta_check_poses: cannot allocate %zu bytes of work-list storage: %s", (size_t)(n + 1) * 8 + bytes, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
+  if (e != cudaSuccess) return alloc_failed(e, "fiesta_check_poses: cannot allocate %zu bytes of work-list storage", (size_t)(n + 1) * 8 + bytes);
   const unsigned setup_blocks = (unsigned)((n + 1 + 255) / 256);
-  k_pose_setup<<<setup_blocks, 256, 0, s>>>(g, poses, n, body, status, n_blocked, hit_idx, B.work);
+  k_pose_setup<<<setup_blocks, 256, 0, s>>>(m->g, poses, n, body, status, n_blocked, hit_idx, B.work);
   CK(cudaGetLastError());
   bytes = B.tmp.cap;
   CK(cub::DeviceScan::ExclusiveSum(B.tmp.p, bytes, B.work.p, B.work.p, (int)(n + 1), s));
@@ -165,10 +162,45 @@ int fb_pose_check_batch(const FbGeom &g, const uint32_t *cobs, const double *pos
   CK(cudaGetDevice(&dev));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const unsigned blocks = (unsigned)((per_sm > 0 ? per_sm : 1) * sms);
-  k_pose_check<<<blocks, 32 * POSE_WARPS, 0, s>>>(g, cobs, poses, n, body, clearance, unknown_blocks, B.work, status, n_blocked, hit_idx);
+  k_pose_check<<<blocks, 32 * POSE_WARPS, 0, s>>>(m->g, m->cobs, poses, n, body, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, B.work,
+                                                  status, n_blocked, hit_idx);
   CK(cudaGetLastError());
   k_pose_finish<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(n, status, n_blocked, hit_idx);
   CK(cudaGetLastError());
-  *launches += 4;
+  m->st.kernel_launches += 4;
   return FIESTA_OK;
+}
+
+int fiesta_check_poses(fiesta_map *m, const double *poses, int64_t n, const double half_extents[3], double clearance, int flags,
+                       int32_t *status, int32_t *n_blocked, int64_t *hit_idx) {
+  const char *fn = "fiesta_check_poses";
+  if (!m) return FIESTA_ERR_INVALID;
+  int r;
+  if ((r = pose_args(m, fn, n, half_extents, clearance, flags, poses && status && n_blocked && hit_idx))) return r;
+  if (n == 0) return FIESTA_OK;
+  CK(cudaSetDevice(m->device));
+  CK(m->pose.io.grow((size_t)n * 112, m->stream));
+  double *d_poses = reinterpret_cast<double *>(m->pose.io.p);
+  int64_t *d_idx = reinterpret_cast<int64_t *>(d_poses + 12 * n);
+  int32_t *d_st = reinterpret_cast<int32_t *>(d_idx + n), *d_nb = d_st + n;
+  CK(cudaMemcpyAsync(d_poses, poses, (size_t)n * 96, cudaMemcpyHostToDevice, m->stream));
+  if ((r = poses_launch(m, d_poses, n, half_extents, clearance, flags, d_st, d_nb, d_idx, m->stream))) return r;
+  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(n_blocked, d_nb, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(hit_idx, d_idx, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+
+int fiesta_check_poses_device(fiesta_map *m, const double *d_poses, int64_t n, const double half_extents[3], double clearance, int flags,
+                              int32_t *d_status, int32_t *d_n_blocked, int64_t *d_hit_idx, void *stream) {
+  const char *fn = "fiesta_check_poses_device";
+  if (!m) return FIESTA_ERR_INVALID;
+  int r;
+  if ((r = pose_args(m, fn, n, half_extents, clearance, flags, d_poses && d_status && d_n_blocked && d_hit_idx))) return r;
+  const cudaStream_t s = (cudaStream_t)stream;
+  if ((r = device_query_begin(m, fn, s)) ||
+      (r = poses_launch(m, d_poses, n, half_extents, clearance, flags, d_status, d_n_blocked, d_hit_idx, s)))
+    return r;
+  return device_query_end(m, s);
 }

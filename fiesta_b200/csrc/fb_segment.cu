@@ -5,7 +5,7 @@
 // voxels in t order, each from its exactly computed entry voxel); the earliest lane whose slab blocks comes from a ballot, the
 // minimum distance up to and including its blocking voxel from a warp reduction over the lanes up to it, and the warp stops
 // after the first sweep that blocks.  The result equals fb_seg_check's sequential walk bit for bit.
-#include "fb_common.cuh"
+#include "fb_map.h"
 #include "fb_segment.h"
 
 #define FB_SEG_WARPS 8
@@ -46,11 +46,50 @@ __global__ void __launch_bounds__(32 * FB_SEG_WARPS) k_segment_clearance(FbGeom 
   }
 }
 
-cudaError_t fb_segment_clearance(const FbGeom &g, const uint32_t *cobs, const double *ab, long long n, double r, int unknown_blocks,
-                                 int32_t *status, int64_t *hit_idx, double *hit_t, double *min_dist, cudaStream_t s) {
-  if (n <= 0) return cudaSuccess;
+// ---------------------------------------------------------------- entry points (include/fiesta_b200.h)
+// Both forms, validated, on device buffers: the launch on stream s.
+static int segments_launch(fiesta_map *m, const double *ab, int64_t n, double clearance, int flags, int32_t *status, int64_t *hit_idx,
+                           double *hit_t, double *min_dist, cudaStream_t s) {
+  if (n <= 0) return FIESTA_OK;
   const long long want = (n + FB_SEG_WARPS - 1) / FB_SEG_WARPS;
   const unsigned blocks = (unsigned)(want < FB_SMS * 64ll ? want : FB_SMS * 64ll);
-  k_segment_clearance<<<blocks, 32 * FB_SEG_WARPS, 0, s>>>(g, cobs, ab, n, r, unknown_blocks, status, hit_idx, hit_t, min_dist);
-  return cudaGetLastError();
+  k_segment_clearance<<<blocks, 32 * FB_SEG_WARPS, 0, s>>>(m->g, m->cobs, ab, n, clearance, flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, status,
+                                                           hit_idx, hit_t, min_dist);
+  CK(cudaGetLastError());
+  m->st.kernel_launches++;
+  return FIESTA_OK;
+}
+
+int fiesta_check_segments(fiesta_map *m, const double *ab, int64_t n, double clearance, int flags, int32_t *status, int64_t *hit_idx,
+                          double *hit_t, double *min_dist) {
+  const char *fn = "fiesta_check_segments";
+  if (!m || !count_buffers_ok(fn, n, ab && status && hit_idx && hit_t && min_dist) || !clearance_flags_ok(fn, clearance, flags))
+    return FIESTA_ERR_INVALID;
+  if (n == 0) return FIESTA_OK;
+  CK(cudaSetDevice(m->device));
+  CK(m->d_seg.grow((size_t)n * 76, m->stream));
+  double *d_ab = reinterpret_cast<double *>(m->d_seg.p), *d_t = d_ab + 6 * n, *d_min = d_t + n;
+  int64_t *d_idx = reinterpret_cast<int64_t *>(d_min + n);
+  int32_t *d_st = reinterpret_cast<int32_t *>(d_idx + n);
+  CK(cudaMemcpyAsync(d_ab, ab, (size_t)n * 48, cudaMemcpyHostToDevice, m->stream));
+  int r;
+  if ((r = segments_launch(m, d_ab, n, clearance, flags, d_st, d_idx, d_t, d_min, m->stream))) return r;
+  CK(cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(hit_idx, d_idx, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(hit_t, d_t, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaMemcpyAsync(min_dist, d_min, (size_t)n * 8, cudaMemcpyDeviceToHost, m->stream));
+  CK(cudaStreamSynchronize(m->stream));
+  return FIESTA_OK;
+}
+
+int fiesta_check_segments_device(fiesta_map *m, const double *d_ab, int64_t n, double clearance, int flags, int32_t *d_status,
+                                 int64_t *d_hit_idx, double *d_hit_t, double *d_min_dist, void *stream) {
+  const char *fn = "fiesta_check_segments_device";
+  if (!m || !count_buffers_ok(fn, n, d_ab && d_status && d_hit_idx && d_hit_t && d_min_dist) || !clearance_flags_ok(fn, clearance, flags))
+    return FIESTA_ERR_INVALID;
+  const cudaStream_t s = (cudaStream_t)stream;
+  int r;
+  if ((r = device_query_begin(m, fn, s)) || (r = segments_launch(m, d_ab, n, clearance, flags, d_status, d_hit_idx, d_hit_t, d_min_dist, s)))
+    return r;
+  return device_query_end(m, s);
 }

@@ -1,16 +1,31 @@
-// fiesta_b200 -- device side of map snapshots (fb_snapshot.h, DESIGN.md §3.12): the classification of the 8^3 tiles that hold
-// anything but the default state, and the pack / unpack of their payload through bounded staging, with per-tile checksums and,
-// on load, the validation of every word before any other kernel can read it.
+// fiesta_b200 -- map snapshots (format: fb_snapshot.h, DESIGN.md §3.12): the classification of the 8^3 tiles that hold anything
+// but the default state, the pack / unpack of their payload through bounded staging, with per-tile checksums and, on load, the
+// validation of every word before any other kernel can read it; and fiesta_snapshot_save / fiesta_snapshot_load around them.
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <string.h>
-#include "fb_common.cuh"
+#include <vector>
+#include "fb_map.h"
 #include "fb_snapshot.h"
 
 static_assert(FB_SNAP_MAX_GX == FB_MAX_GX && FB_SNAP_MAX_GY == FB_MAX_GY && FB_SNAP_MAX_GZ == FB_MAX_GZ, "grid limits");
 static_assert(FB_SNAP_MAX_PTOTAL == (long long)FB_LIST_IDX_MASK, "voxel limit");
 
 #define SNAP_THREADS 256
+#define FB_SNAP_STAGE (16u << 20)  // bytes of each of the two device and two pinned staging buffers of a save or load
+struct FbSnapArrays {              // the per-voxel state a snapshot carries; LS is null in FAST mode
+  FbGeom g;
+  uint32_t *cobs;
+  double *occ;
+  unsigned long long *cnt, *LS;
+};
+struct FbSnapBufs {                // per-tile scratch of one save or load
+  FbDevBuf<uint8_t> flag;          // per grid tile: holds non-default state
+  FbDevBuf<uint32_t> list, d_n;    // stored tiles ascending; selection count, or {first bad tile, reasons} on load
+  FbDevBuf<unsigned long long> off;  // per stored tile: payload offset, and the end
+  FbHostBuf<uint32_t> h_n;
+  FbDevBuf<char> tmp;              // CUB temporary storage
+};
 
 // global index of the k-th in-grid voxel (z fastest) of the tile at tile coordinates tc with extents n
 __device__ __forceinline__ long long snap_voxel(const FbGeom &g, const int *tc, const int *n, int k) {
@@ -134,7 +149,8 @@ __global__ void __launch_bounds__(SNAP_THREADS) k_snap_unpack(FbGeom g, uint32_t
 }
 
 // ====================================================================== host side
-int fb_snap_list_tiles(const FbSnapArrays &A, FbSnapBufs &B, unsigned *n_out, cudaStream_t s) {
+// Lists the tiles with non-default state into B.list (ascending) and their count into *n_out.
+static int snap_list_tiles(const FbSnapArrays &A, FbSnapBufs &B, unsigned *n_out, cudaStream_t s, int *launches) {
   const FbGeom &g = A.g;
   const unsigned T = (unsigned)g.ntiles;
   CK(B.flag.alloc(T)); CK(B.list.alloc(T)); CK(B.d_n.alloc(1)); CK(B.h_n.alloc(1));
@@ -148,6 +164,7 @@ int fb_snap_list_tiles(const FbSnapArrays &A, FbSnapBufs &B, unsigned *n_out, cu
   CK(cudaMemcpyAsync(B.h_n.p, B.d_n.p, 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   *n_out = *B.h_n.p;
+  *launches += 2;
   return FIESTA_OK;
 }
 
@@ -186,7 +203,9 @@ void snap_chunks(const std::vector<unsigned long long> &off, std::vector<unsigne
 }
 }  // namespace
 
-int fb_snap_pack(const FbSnapArrays &A, FbSnapBufs &B, const std::vector<unsigned long long> &off, uint8_t *dst, cudaStream_t s, int *launches) {
+// Payload of the B.list tiles, whose offsets (and the end) are `off`, written to host memory dst + off[t].
+static int snap_pack(const FbSnapArrays &A, FbSnapBufs &B, const std::vector<unsigned long long> &off, uint8_t *dst, cudaStream_t s,
+                     int *launches) {
   const unsigned n = (unsigned)off.size() - 1;
   if (n == 0) return FIESTA_OK;
   CK(B.off.alloc(n + 1));
@@ -220,8 +239,10 @@ int fb_snap_pack(const FbSnapArrays &A, FbSnapBufs &B, const std::vector<unsigne
   return FIESTA_OK;
 }
 
-int fb_snap_unpack(const FbSnapArrays &A, FbSnapBufs &B, const uint32_t *h_list, const std::vector<unsigned long long> &off, const uint8_t *src,
-                   unsigned long long tclock, unsigned *bad_tile, unsigned *reasons, cudaStream_t s, int *launches) {
+// Scatters the payload at src + off[t] of the h_list tiles into A; *bad_tile = the first tile position that failed validation
+// (0xffffffff: none), *reasons = the FB_SNAP_BAD_* bits.
+static int snap_unpack(const FbSnapArrays &A, FbSnapBufs &B, const uint32_t *h_list, const std::vector<unsigned long long> &off,
+                       const uint8_t *src, unsigned long long tclock, unsigned *bad_tile, unsigned *reasons, cudaStream_t s, int *launches) {
   const unsigned n = (unsigned)off.size() - 1;
   *bad_tile = 0xffffffffu; *reasons = 0;
   if (n == 0) return FIESTA_OK;
@@ -256,5 +277,138 @@ int fb_snap_unpack(const FbSnapArrays &A, FbSnapBufs &B, const uint32_t *h_list,
   CK(cudaMemcpyAsync(B.h_n.p, B.d_n.p, 8, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   *bad_tile = B.h_n.p[0]; *reasons = B.h_n.p[1];
+  return FIESTA_OK;
+}
+
+// ====================================================================== entry points (include/fiesta_b200.h)
+static FbSnapArrays snap_arrays(fiesta_map *m) {
+  return FbSnapArrays{m->g, m->cobs, m->occ, m->cnt, m->mode == FIESTA_MODE_EXACT ? m->X.LS.p : nullptr};
+}
+// the fiesta_stats counters in snapshot order: every one but kernel_launches (raycast_rounds' slot is not used)
+static int64_t *snap_stat(fiesta_stats &st, int i) {
+  int64_t *f[FB_SNAP_NSTATS] = {&st.occupancy_updates, &st.inserts, &st.deletes, &st.voxels_changed, &st.expansions, &st.voxels_reset,
+                                &st.tile_visits, &st.generations, &st.rays_cast, &st.rays_dropped, &st.ray_voxels, &st.raycast_rounds,
+                                &st.touched_voxels};
+  return f[i];
+}
+static std::vector<unsigned long long> snap_offsets(const FbGeom &g, int exact, const uint32_t *list, size_t n) {
+  std::vector<unsigned long long> off(n + 1);
+  off[0] = 0;
+  for (size_t t = 0; t < n; ++t) off[t + 1] = off[t] + fb_snap_tile_bytes(g.gx, g.gy, g.gz, exact, list[t]);
+  return off;
+}
+int fiesta_snapshot_save(fiesta_map *m, void *buf, int64_t cap, int64_t *size) {
+  const char *fn = "fiesta_snapshot_save";
+  if (!m || !size || cap < 0 || (cap > 0 && !buf)) { fb_set_error("%s: bad argument", fn); return FIESTA_ERR_INVALID; }
+  *size = 0;
+  if (m->n_ev > 0) { fb_set_error("%s: SetOccupancy events are staged (UpdateOccupancy has not run)", fn); return FIESTA_ERR_INVALID; }
+  if (m->n_touch_tiles > 0) { fb_set_error("%s: the occupancy queue is not empty (UpdateOccupancy has not run)", fn); return FIESTA_ERR_INVALID; }
+  if (m->n_ins > 0 || m->n_del > 0) { fb_set_error("%s: inserts or deletes are pending (UpdateESDF has not run)", fn); return FIESTA_ERR_INVALID; }
+  if (m->shard_world > 1) { fb_set_error("%s: an x-slab shard cannot be saved", fn); return FIESTA_ERR_INVALID; }
+  CK(cudaSetDevice(m->device));
+  const FbSnapArrays A = snap_arrays(m);
+  const int exact = m->mode == FIESTA_MODE_EXACT;
+  FbSnapBufs B;
+  unsigned n = 0;
+  int r, launches = 0;
+  if ((r = snap_list_tiles(A, B, &n, m->stream, &launches))) return r;
+  m->st.kernel_launches += launches;
+  std::vector<uint32_t> list(n);
+  if (n) {
+    CK(cudaMemcpyAsync(list.data(), B.list, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaStreamSynchronize(m->stream));
+  }
+  const std::vector<unsigned long long> off = snap_offsets(m->g, exact, list.data(), n);
+  const int64_t depth_pixels = m->image_cnt ? (int64_t)m->d_img[0].cap : 0;
+  FbSnapLayout L;
+  fb_snap_layout(n, off[n], depth_pixels, &L);
+  *size = (int64_t)L.total;
+  if (!buf) return FIESTA_OK;                                             // size query
+  if (cap < *size) { fb_set_error("%s: the buffer holds %lld bytes, the snapshot needs %lld", fn, (long long)cap, (long long)*size); return FIESTA_ERR_LIMIT; }
+  uint8_t *p = static_cast<uint8_t *>(buf);
+  launches = 0;
+  if ((r = snap_pack(A, B, off, p + L.payload_off, m->stream, &launches))) return r;
+  m->st.kernel_launches += launches;
+  memset(p + L.list_off, 0, L.payload_off - L.list_off);
+  for (unsigned t = 0; t < n; ++t) fb_snap_st32(p + L.list_off + 4 * t, list[t]);
+  memset(p + L.depth_off, 0, L.depth_bytes);
+  if (depth_pixels) {
+    CK(cudaMemcpyAsync(p + L.depth_off, m->d_img[m->image_cnt & 1], (size_t)depth_pixels * 2, cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaStreamSynchronize(m->stream));
+  }
+  FbSnapHeader h{};
+  h.version = FB_SNAP_VERSION; h.mode = (uint32_t)m->mode;
+  for (int i = 0; i < 3; ++i) {
+    h.origin[i] = m->cfg.origin[i]; h.map_size[i] = m->cfg.map_size[i];
+    h.min_vec[i] = m->g.min_vec[i]; h.max_vec[i] = m->g.max_vec[i]; h.last_min_vec[i] = m->g.last_min_vec[i]; h.last_max_vec[i] = m->g.last_max_vec[i];
+  }
+  h.resolution = m->cfg.resolution;
+  h.grid[0] = m->g.gx; h.grid[1] = m->g.gy; h.grid[2] = m->g.gz;
+  h.params_set = m->params_set ? 1 : 0;
+  h.l_hit = m->l_hit; h.l_miss = m->l_miss; h.l_min = m->l_min; h.l_max = m->l_max; h.l_occ = m->l_occ;
+  h.flags = m->local_box_seen ? FB_SNAP_LOCAL_BOX_SEEN : 0u;
+  h.image_cnt = m->image_cnt;
+  h.tclock = exact ? m->X.tclock : 0; h.key_base = exact ? m->X.key_base : 0;
+  for (int i = 0; i < FB_SNAP_NSTATS; ++i) h.stats[i] = i == FB_SNAP_STAT_ROUNDS ? 0 : *snap_stat(m->st, i);
+  h.depth_pixels = depth_pixels;
+  h.n_tiles = n;
+  h.list_sum = fb_snap_checksum(p + L.list_off, (L.payload_off - L.list_off) / 8);
+  h.depth_sum = fb_snap_checksum(p + L.depth_off, L.depth_bytes / 8);
+  fb_snap_encode(h, p);
+  return FIESTA_OK;
+}
+int fiesta_snapshot_load(const void *buf, int64_t size, int32_t device, fiesta_map **out) {
+  const char *fn = "fiesta_snapshot_load";
+  if (!out) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  *out = nullptr;
+  if (!buf || size < 0) { fb_set_error("%s: bad argument", fn); return FIESTA_ERR_INVALID; }
+  const uint8_t *p = static_cast<const uint8_t *>(buf);
+  FbSnapHeader h;
+  FbSnapLayout L;
+  char err[256];
+  if (fb_snap_parse(p, size, &h, &L, err, (int)sizeof(err))) { fb_set_error("%s: %s", fn, err); return FIESTA_ERR_INVALID; }
+  fiesta_config cfg{};
+  for (int i = 0; i < 3; ++i) { cfg.origin[i] = h.origin[i]; cfg.map_size[i] = h.map_size[i]; }
+  cfg.resolution = h.resolution; cfg.device = device; cfg.mode = (int32_t)h.mode;
+  fiesta_map *raw = nullptr;
+  int r;
+  if ((r = create_map(&cfg, &raw, false))) return r;                     // the mode is the snapshot's, whatever FIESTA_B200_MODE says
+  std::unique_ptr<fiesta_map, void (*)(fiesta_map *)> m(raw, fiesta_destroy);   // destroyed on any failure below
+  FbGeom &g = m->g;
+  if (g.gx != h.grid[0] || g.gy != h.grid[1] || g.gz != h.grid[2]) { fb_set_error("%s: the rebuilt grid differs from the stored one", fn); return FIESTA_ERR_INVALID; }
+  m->params_set = h.params_set != 0;
+  m->l_hit = h.l_hit; m->l_miss = h.l_miss; m->l_min = h.l_min; m->l_max = h.l_max; m->l_occ = h.l_occ;
+  for (int i = 0; i < 3; ++i) {
+    g.min_vec[i] = h.min_vec[i]; g.max_vec[i] = h.max_vec[i]; g.last_min_vec[i] = h.last_min_vec[i]; g.last_max_vec[i] = h.last_max_vec[i];
+  }
+  set_box_flag(g);
+  m->local_box_seen = (h.flags & FB_SNAP_LOCAL_BOX_SEEN) != 0;
+  if (m->mode == FIESTA_MODE_EXACT) { m->X.tclock = h.tclock; m->X.key_base = h.key_base; }
+  for (int i = 0; i < FB_SNAP_NSTATS; ++i) if (i != FB_SNAP_STAT_ROUNDS) *snap_stat(m->st, i) = h.stats[i];
+  std::vector<uint32_t> list((size_t)h.n_tiles);
+  for (size_t t = 0; t < list.size(); ++t) list[t] = fb_snap_ld32(p + L.list_off + 4 * t);
+  const std::vector<unsigned long long> off = snap_offsets(g, m->mode == FIESTA_MODE_EXACT, list.data(), list.size());
+  FbSnapBufs B;
+  unsigned bad = 0, why = 0;
+  int launches = 0;
+  if ((r = snap_unpack(snap_arrays(m.get()), B, list.data(), off, p + L.payload_off, h.tclock, &bad, &why, m->stream, &launches))) return r;
+  m->st.kernel_launches += launches;
+  if (why) {
+    fb_set_error("%s: stored tile %u (grid tile %u) is malformed:%s%s%s%s%s%s", fn, bad, list[bad], (why & FB_SNAP_BAD_SUM) ? " checksum mismatch;" : "",
+                 (why & FB_SNAP_BAD_COBS) ? " closest-obstacle record outside the grid;" : "", (why & FB_SNAP_BAD_BIT31) ? " bad bit 31 of a record;" : "",
+                 (why & FB_SNAP_BAD_OCC) ? " log-odds not finite;" : "", (why & FB_SNAP_BAD_LS) ? " relink time not below the relink clock;" : "",
+                 (why & FB_SNAP_BAD_CNT) ? " more hits than observations;" : "");
+    return FIESTA_ERR_INVALID;
+  }
+  // rebuilt, not stored: the Exist() bitmap, and FAST mode's staging copy of the records
+  if ((r = rebuild_occbits(m.get()))) return r;
+  if (m->mode == FIESTA_MODE_FAST) CK(cudaMemcpyAsync(m->cobs_b, m->cobs, (size_t)g.ptotal * 4, cudaMemcpyDeviceToDevice, m->stream));
+  if (h.depth_pixels > 0) {
+    if ((r = alloc_depth(m.get(), (size_t)h.depth_pixels))) return r;
+    CK(cudaMemcpyAsync(m->d_img[h.image_cnt & 1], p + L.depth_off, (size_t)h.depth_pixels * 2, cudaMemcpyHostToDevice, m->stream));
+  }
+  m->image_cnt = h.image_cnt;
+  CK(cudaStreamSynchronize(m->stream));
+  *out = m.release();
   return FIESTA_OK;
 }

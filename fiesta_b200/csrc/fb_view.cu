@@ -14,7 +14,8 @@
 // neighbours in the cluster's index order, so the lanes' walks have similar length and read the same cache lines.  Every output
 // is an integer sum of per-pair integer decisions (integer atomics), so it does not depend on the schedule.
 #include <cub/cub.cuh>
-#include "fb_common.cuh"
+#include <cmath>
+#include "fb_frontier.cuh"
 #include "fb_view.h"
 
 #define VIEW_WARPS 8
@@ -88,19 +89,16 @@ static int view_cub(FbDevBuf<char> &tmp, cudaStream_t s, Call call) {
   size_t bytes = 0;
   CK(call((void *)nullptr, bytes));
   const cudaError_t e = tmp.grow(bytes ? bytes : 16, s);
-  if (e != cudaSuccess) {
-    cudaGetLastError();                                                   // not sticky: later calls must not see it
-    fb_set_error("fiesta_frontiers_score_viewpoints: cannot allocate %zu bytes of scan storage: %s", bytes, cudaGetErrorString(e));
-    return FIESTA_ERR_CUDA;
-  }
+  if (e != cudaSuccess) return alloc_failed(e, "fiesta_frontiers_score_viewpoints: cannot allocate %zu bytes of scan storage", bytes);
   bytes = tmp.cap;
   CK(call((void *)tmp.p, bytes));
   return FIESTA_OK;
 }
 
-int fb_view_score(const FbGeom &g, const uint32_t *cobs, const int64_t *size, const int32_t *m_xyz, unsigned K, FbViewBufs &V,
-                  FbDevBuf<char> &tmp, long long n, int n_orient, const fiesta_sensor_model &sm, double clearance, int unknown_blocks,
-                  cudaStream_t s, int *launches) {
+// Expects V.pos / cl / orient filled for n >= 1 candidates and V.score / ctr zeroed; size / m_xyz are the frontier result's.
+static int view_score(const FbGeom &g, const uint32_t *cobs, const int64_t *size, const int32_t *m_xyz, unsigned K, FbViewBufs &V,
+                      FbDevBuf<char> &tmp, long long n, int n_orient, const fiesta_sensor_model &sm, double clearance, int unknown_blocks,
+                      cudaStream_t s, int *launches) {
   int rc;
   const unsigned setup_blocks = (unsigned)((n + 1 + 255) / 256);
   k_view_setup<<<setup_blocks, 256, 0, s>>>(g, cobs, V.pos, V.cl, n, clearance, size, V.status, V.work, V.ctr);
@@ -119,5 +117,72 @@ int fb_view_score(const FbGeom &g, const uint32_t *cobs, const int64_t *size, co
                                                   V.score, V.ctr);
   CK(cudaGetLastError());
   *launches += 4;
+  return FIESTA_OK;
+}
+
+// ---------------------------------------------------------------- entry point (include/fiesta_b200.h)
+int fiesta_frontiers_score_viewpoints(fiesta_frontiers *f, const int32_t *cluster, const double *pos_xyz, int64_t n, const double *orient,
+                                      int32_t n_orient, const fiesta_sensor_model *sensor, double clearance, int flags, int32_t *status,
+                                      int32_t *score, fiesta_viewpoint_stats *stats) {
+  const char *fn = "fiesta_frontiers_score_viewpoints";
+  if (!f || !sensor || !orient) { fb_set_error("%s: null argument", fn); return FIESTA_ERR_INVALID; }
+  if (!count_buffers_ok(fn, n, cluster && pos_xyz && status && score) || !clearance_flags_ok(fn, clearance, flags)) return FIESTA_ERR_INVALID;
+  if (!f->valid) { fb_set_error("%s: no frontiers have been computed", fn); return FIESTA_ERR_INVALID; }
+  if (n_orient < 1) { fb_set_error("%s: n_orient must be >= 1", fn); return FIESTA_ERR_INVALID; }
+  const fiesta_sensor_model sm = *sensor;
+  const double sv[3] = {sm.max_range, sm.tan_half_fov[0], sm.tan_half_fov[1]};
+  for (double x : sv)
+    if (!(std::isfinite(x) && x > 0)) { fb_set_error("%s: max_range and tan_half_fov must be finite and > 0", fn); return FIESTA_ERR_INVALID; }
+  if (n_orient > FIESTA_VIEWPOINT_MAX_ORIENT) {
+    fb_set_error("%s: at most %d orientations per call", fn, FIESTA_VIEWPOINT_MAX_ORIENT);
+    return FIESTA_ERR_LIMIT;
+  }
+  for (int k = 0; k < 9 * n_orient; ++k)
+    if (!std::isfinite(orient[k])) { fb_set_error("%s: orientation entry %d is not finite", fn, k); return FIESTA_ERR_INVALID; }
+  const int64_t K = f->st.kept_clusters;
+  for (int64_t i = 0; i < n; ++i)
+    if (!(cluster[i] >= 0 && cluster[i] < K)) {
+      fb_set_error("%s: cluster[%lld] = %d is not a kept cluster id (there are %lld)", fn, (long long)i, (int)cluster[i], (long long)K);
+      return FIESTA_ERR_INVALID;
+    }
+  if (n >= 0x7fffffffll) { fb_set_error("%s: at most 2^31 - 2 candidates per call", fn); return FIESTA_ERR_LIMIT; }
+  if (stats) *stats = fiesta_viewpoint_stats{};
+  if (n == 0) return FIESTA_OK;
+  fiesta_map *m = f->m;
+  const cudaStream_t s = m->stream;
+  FbViewBufs &V = f->V;
+  CK(cudaSetDevice(m->device));
+  cudaError_t e = V.pos.grow((size_t)n * 3, s);
+  if (e == cudaSuccess) e = V.cl.grow((size_t)n, s);
+  if (e == cudaSuccess) e = V.status.grow((size_t)n, s);
+  if (e == cudaSuccess) e = V.work.grow((size_t)n + 1, s);
+  if (e == cudaSuccess) e = V.score.grow((size_t)n * n_orient, s);
+  if (e == cudaSuccess) e = V.moff.grow((size_t)K, s);
+  if (e == cudaSuccess) e = V.orient.grow(9 * FIESTA_VIEWPOINT_MAX_ORIENT, s);
+  if (e == cudaSuccess) e = V.ctr.grow(1, s);
+  if (e == cudaSuccess && !V.h_ctr) e = V.h_ctr.alloc(1);
+  if (e != cudaSuccess) return alloc_failed(e, "%s: cannot allocate the buffers of %lld candidates", fn, (long long)n);
+  CK(cudaMemcpyAsync(V.pos, pos_xyz, (size_t)n * 24, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(V.cl, cluster, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(V.orient, orient, (size_t)n_orient * 72, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(V.score, 0, (size_t)n * n_orient * 4, s));
+  CK(cudaMemsetAsync(V.ctr, 0, sizeof(FbViewCtr), s));
+  int launches = 0;
+  CK(cudaEventRecord(f->ev[0], s));
+  const int r = view_score(m->g, m->cobs, f->B.o_size, f->B.m_xyz, (unsigned)K, V, f->B.tmp, (long long)n, (int)n_orient, sm, clearance,
+                           flags & FIESTA_SEGMENT_UNKNOWN_BLOCKS, s, &launches);
+  m->st.kernel_launches += launches;
+  if (r != FIESTA_OK) return r;
+  CK(cudaEventRecord(f->ev[1], s));
+  CK(cudaMemcpyAsync(V.h_ctr, V.ctr, sizeof(FbViewCtr), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(status, V.status, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(score, V.score, (size_t)n * n_orient * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (stats) {
+    stats->candidates_scored = (int64_t)V.h_ctr->scored;
+    stats->pairs_walked = (int64_t)V.h_ctr->walked;
+    stats->pairs_visible = (int64_t)V.h_ctr->visible;
+    CK(cudaEventElapsedTime(&stats->ms_compute, f->ev[0], f->ev[1]));
+  }
   return FIESTA_OK;
 }
