@@ -58,6 +58,11 @@ class NavMatrixStats(C.Structure):
                                          "sources_retired_early")] + [("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
 
 
+class SignedStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("box_voxels", "obstacles", "interior", "max_depth_sq")] + [
+        ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
+
+
 class FrontierStats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("box_voxels", "frontier_voxels", "clusters", "kept_clusters", "kept_voxels")] + [
         ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
@@ -112,6 +117,9 @@ SYMBOLS = [
     "fiesta_inflate_boxes", "fiesta_corridors",
     "fiesta_check_poses", "fiesta_check_poses_device", "fiesta_host_mirror_check_poses",
     "fiesta_snapshot_save", "fiesta_snapshot_load", "fiesta_get_config",
+    "fiesta_signed_create", "fiesta_signed_destroy", "fiesta_signed_compute", "fiesta_signed_export",
+    "fiesta_signed_get_distance_batch", "fiesta_signed_get_dist_grad_trilinear_batch", "fiesta_signed_get_distance_batch_device",
+    "fiesta_signed_get_dist_grad_trilinear_batch_device",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -175,6 +183,16 @@ def load_library():
         L.fiesta_nav_paths.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 4
         L.fiesta_nav_update.argtypes = [C.c_void_p, C.c_void_p]
         L.fiesta_nav_matrix.argtypes = [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_int64, C.c_double, C.c_int] + [C.c_void_p] * 4
+        L.fiesta_signed_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+        L.fiesta_signed_destroy.argtypes = [C.c_void_p]
+        L.fiesta_signed_destroy.restype = None
+        L.fiesta_signed_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.fiesta_signed_export.argtypes = [C.c_void_p, C.c_void_p]
+        L.fiesta_signed_get_distance_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+        L.fiesta_signed_get_dist_grad_trilinear_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+        L.fiesta_signed_get_distance_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+        L.fiesta_signed_get_dist_grad_trilinear_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                                                         C.c_void_p]
         L.fiesta_frontiers_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
         L.fiesta_frontiers_destroy.argtypes = [C.c_void_p]
         L.fiesta_frontiers_destroy.restype = None
@@ -390,6 +408,76 @@ class NavField:
     def close(self):
         if self._h:
             self._m._L.fiesta_nav_destroy(self._h)
+            self._h = None
+
+
+class SignedField:
+    """fiesta_signed_field: signed distance over a voxel box -- FIESTA's distance outside obstacles, minus the exact Euclidean depth
+    inside them -- with GetDistance / GetDistWithGradTrilinear queries that read it inside the box and the map elsewhere.  A field
+    refuses export and queries after UpdateOccupancy / UpdateESDF until it is computed again.  The buffers grow to the largest box
+    computed; close() it before the map."""
+
+    def __init__(self, m):
+        self._m = m
+        h = C.c_void_p()
+        m._ck(m._L.fiesta_signed_create(m._h, C.byref(h)), "fiesta_signed_create")
+        self._h = h
+        self.shape = None
+
+    def compute(self, box_lo, box_hi):
+        """Field over the inclusive voxel box [box_lo, box_hi] -> stats dict."""
+        lo, hi = np.ascontiguousarray(box_lo, dtype=np.int32), np.ascontiguousarray(box_hi, dtype=np.int32)
+        if lo.shape != (3,) or hi.shape != (3,):
+            raise ValueError("SignedField.compute: box_lo and box_hi must be 3 voxel coordinates each")
+        st = SignedStats()
+        self._m._ck(self._m._L.fiesta_signed_compute(self._h, lo.ctypes, hi.ctypes, C.byref(st)), "SignedField.compute")
+        self.shape = tuple(int(b - a + 1) for a, b in zip(lo, hi))
+        return {n: getattr(st, n) for n, _ in st._fields_ if n != "reserved_f"}
+
+    def export(self):
+        """S of the last computed box as a (Bx, By, Bz) float64 array."""
+        if self.shape is None:
+            raise FiestaError("SignedField.export: no field has been computed")
+        out = np.empty(self.shape)
+        self._m._ck(self._m._L.fiesta_signed_export(self._h, out.ctypes), "SignedField.export")
+        return out
+
+    def GetDistanceBatch(self, pos):
+        pos = _f64(pos).reshape(-1, 3)
+        out = np.empty(len(pos))
+        self._m._ck(self._m._L.fiesta_signed_get_distance_batch(self._h, pos.ctypes, C.c_int64(len(pos)), out.ctypes),
+                    "SignedField.GetDistanceBatch")
+        return out
+
+    def GetDistWithGradTrilinearBatch(self, pos):
+        pos = _f64(pos).reshape(-1, 3)
+        d = np.empty(len(pos))
+        g = np.empty((len(pos), 3))
+        self._m._ck(self._m._L.fiesta_signed_get_dist_grad_trilinear_batch(self._h, pos.ctypes, C.c_int64(len(pos)), d.ctypes, g.ctypes),
+                    "SignedField.GetDistWithGradTrilinearBatch")
+        return d, g
+
+    def GetDistanceBatchDevice(self, pos):
+        """GetDistance for a CUDA float64 (n, 3) tensor, on the current torch stream (fiesta_signed_get_distance_batch_device)."""
+        torch, stream = self._m._device_tensor(pos, 3, "SignedField.GetDistanceBatchDevice")
+        d = torch.empty(pos.shape[0], dtype=torch.float64, device=pos.device)
+        self._m._ck(self._m._L.fiesta_signed_get_distance_batch_device(self._h, pos.data_ptr(), pos.shape[0], d.data_ptr(), stream),
+                    "SignedField.GetDistanceBatchDevice")
+        return d
+
+    def GetDistWithGradTrilinearBatchDevice(self, pos):
+        """GetDistWithGradTrilinear for a CUDA float64 (n, 3) tensor, on the current torch stream -> (dist (n,), grad (n, 3))."""
+        torch, stream = self._m._device_tensor(pos, 3, "SignedField.GetDistWithGradTrilinearBatchDevice")
+        d = torch.empty(pos.shape[0], dtype=torch.float64, device=pos.device)
+        g = torch.empty((pos.shape[0], 3), dtype=torch.float64, device=pos.device)
+        self._m._ck(self._m._L.fiesta_signed_get_dist_grad_trilinear_batch_device(self._h, pos.data_ptr(), pos.shape[0], d.data_ptr(),
+                                                                                  g.data_ptr(), stream),
+                    "SignedField.GetDistWithGradTrilinearBatchDevice")
+        return d, g
+
+    def close(self):
+        if self._h:
+            self._m._L.fiesta_signed_destroy(self._h)
             self._h = None
 
 
@@ -752,6 +840,10 @@ class ESDFMap:
     def NavField(self):
         """Cost-to-go field of a voxel box through free space at a clearance, with path extraction (fiesta_nav_*)."""
         return NavField(self)
+
+    def SignedField(self):
+        """Signed distance of a voxel box: negative inside obstacles by the exact depth to free space (fiesta_signed_*)."""
+        return SignedField(self)
 
     def Frontiers(self):
         """Frontier voxels of a box (free voxels bordering unknown space) in clusters, with statistics (fiesta_frontiers_*)."""

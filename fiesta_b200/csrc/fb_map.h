@@ -89,6 +89,9 @@ struct fiesta_map {
   struct fiesta_host_mirror *mirror = nullptr;
   int dirty_lo[3]{}, dirty_hi[3]{};
   bool dirty_any = false, pending_obs = false;  // pending_obs: observations counted under the current box and not integrated yet
+  // records epoch: incremented by every call that can change the records (UpdateOccupancy, UpdateESDF, shard ingest / relax);
+  // a signed field (fb_signed.cu) computed under an older epoch refuses to be read
+  unsigned long long records_epoch = 0;
 };
 
 // Map functions: FIESTA_OK or a FIESTA_ERR_* code with fiesta_last_error() set.

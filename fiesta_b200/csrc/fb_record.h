@@ -83,4 +83,64 @@ FB_HD bool fb_pos_in_map(const FbGeom &g, const double *p) {
 FB_HD void fb_pos2vox(const FbGeom &g, const double *p, int *v) {
   for (int k = 0; k < 3; ++k) v[k] = (int)floor((p[k] - g.origin[k]) / g.res);
 }
+
+// The point queries, generic in the voxel read: `rd(x, y, z)` is GetDistance(Vector3i) of the field being queried.  The map's
+// own queries (device kernel, query plan, host mirror) read the records with FbRecordRead; the signed field (fb_signed.h) reads
+// its signed values inside its box and the records elsewhere.  Every other operation is shared.
+struct FbRecordRead {
+  const FbGeom &g;
+  const uint32_t *cobs;
+  FB_HD double operator()(int x, int y, int z) const { return fb_get_distance_vox(g, cobs, x, y, z); }
+};
+// GetDistance(Vector3d) (ESDFMap.cpp:467-475)
+template <class Read> FB_HD double fb_query_distance(const FbGeom &g, const Read &rd, const double *p) {
+  if (!fb_pos_in_map(g, p)) return (double)FIESTA_UNDEFINED;
+  int v[3];
+  fb_pos2vox(g, p, v);
+  return rd(v[0], v[1], v[2]);
+}
+// GetDistWithGradTrilinear (ESDFMap.cpp:481-540), operation for operation (fp64, no contraction: -fmad=false on the device,
+// no FMA target on the host).
+template <class Read> FB_HD double fb_query_trilinear(const FbGeom &g, const Read &rd, const double *p, double *grad) {
+  if (!fb_pos_in_map(g, p)) { grad[0] = grad[1] = grad[2] = 0.0; return -1.0; }
+  int b[3];
+  double bp[3], f[3];
+#ifdef __CUDACC__
+#pragma unroll
+#endif
+  for (int k = 0; k < 3; ++k) {
+    const double pm = p[k] - 0.5 * g.res * 1.0;                           // pos - 0.5*resolution_*Ones()
+    b[k] = (int)floor((pm - g.origin[k]) / g.res);
+    bp[k] = (b[k] + 0.5) * g.res + g.origin[k];                           // Vox2Pos
+    f[k] = (p[k] - bp[k]) * g.res_inv;
+  }
+  double c[2][2][2];
+#ifdef __CUDACC__
+#pragma unroll
+#endif
+  for (int x = 0; x < 2; ++x)
+#ifdef __CUDACC__
+#pragma unroll
+#endif
+    for (int y = 0; y < 2; ++y)
+#ifdef __CUDACC__
+#pragma unroll
+#endif
+      for (int z = 0; z < 2; ++z) c[x][y][z] = rd(b[0] + x, b[1] + y, b[2] + z);
+  const double v00 = (1 - f[0]) * c[0][0][0] + f[0] * c[1][0][0];
+  const double v01 = (1 - f[0]) * c[0][0][1] + f[0] * c[1][0][1];
+  const double v10 = (1 - f[0]) * c[0][1][0] + f[0] * c[1][1][0];
+  const double v11 = (1 - f[0]) * c[0][1][1] + f[0] * c[1][1][1];
+  const double v0 = (1 - f[1]) * v00 + f[1] * v10;
+  const double v1 = (1 - f[1]) * v01 + f[1] * v11;
+  grad[2] = (v1 - v0) * g.res_inv;
+  grad[1] = ((1 - f[2]) * (v10 - v00) + f[2] * (v11 - v01)) * g.res_inv;
+  double g0 = (1 - f[2]) * (1 - f[1]) * (c[1][0][0] - c[0][0][0]);
+  g0 += (1 - f[2]) * f[1] * (c[1][1][0] - c[0][1][0]);
+  g0 += f[2] * (1 - f[1]) * (c[1][0][1] - c[0][0][1]);
+  g0 += f[2] * f[1] * (c[1][1][1] - c[0][1][1]);
+  g0 *= g.res_inv;
+  grad[0] = g0;
+  return (1 - f[2]) * v0 + f[2] * v1;
+}
 #endif

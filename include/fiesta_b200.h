@@ -283,7 +283,8 @@ int fiesta_host_mirror_check_poses(const fiesta_host_mirror *p, const double *po
  *                outside the box or the map (PosInMap) or NaN (cost NaN, len 0), 3 = truncated after max_len voxels.
  * The field object owns its device buffers, which grow to the largest box used: 8 bytes per box voxel plus 12 bytes per 8^3 tile,
  * with the library's 50 % growth headroom (about 1.6 GB for a 512^3 box; 6.5 GB for a 1024 x 1024 x 512 box, which next to an
- * EXACT map of that grid -- 68.1 GiB on a 79.2 GiB card -- is tight).  It runs on the map's stream; the calls are synchronous.
+ * EXACT map of that grid -- 68.1 GiB on a 79.2 GiB card -- is tight; a signed field of the same box takes as much, 8 bytes per
+ * box voxel).  It runs on the map's stream; the calls are synchronous.
  * Destroy it before the map.  Errors:
  * FIESTA_ERR_INVALID for a box outside the grid or inverted, a clearance or flags that fiesta_check_segments rejects, null
  * buffers, max_len < 1, or export / paths before a compute; nothing changes then.  FIESTA_ERR_CUDA when the buffers cannot be
@@ -362,6 +363,57 @@ typedef struct fiesta_nav_matrix_stats {
 int fiesta_nav_matrix(fiesta_nav_field *f, const int box_lo[3], const int box_hi[3], const double *sources_xyz, int64_t n_src,
                       const double *targets_xyz, int64_t n_tgt, double clearance, int flags, int32_t *src_status, int32_t *tgt_status,
                       double *cost /* n_src * n_tgt, row i = source i */, fiesta_nav_matrix_stats *stats /* nullable */);
+
+/* ---- signed distance (gradient-based trajectory optimisers: a way out for waypoints inside obstacles) ----
+ * FIESTA's field is exactly 0 on every obstacle voxel, so a waypoint inside a wall sees distance 0 and gradient 0 there.  The
+ * signed field of an inclusive voxel box B = [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis) keeps FIESTA's distance
+ * outside obstacles and goes negative inside them, by the depth to free space.  It is a snapshot of the records at the time of
+ * fiesta_signed_compute.
+ *   obstacle     a grid voxel whose distance reads exactly 0 in fiesta_export_distance (its closest obstacle is itself).  An
+ *                EXACT-mode voxel under a local-map reset reads +10000 and is not one.  Every other voxel is a non-obstacle: free,
+ *                unreached or never observed.
+ *   depth        for an obstacle voxel v of B, q(v) = the least dx^2 + dy^2 + dz^2 (voxel units, exact integers) from v to a
+ *                non-obstacle voxel OF B; voxels outside B are not candidates, so give the box a margin where true depths near its
+ *                faces matter.
+ *   S(v)         for a voxel of B, each fp64 operation rounded on its own: GetDistance(Vector3i v) for a non-obstacle (never
+ *                observed reads +10000); (1.0 - sqrt((double)q(v))) * resolution for an obstacle, so surface voxels (q == 1) stay
+ *                +0.0 and deeper ones go negative (the pos - neg + resolution convention of ESDF-based planners); -inf for an
+ *                obstacle when B holds no non-obstacle voxel.  fiesta_signed_export writes S for the box, index as
+ *                fiesta_nav_export.
+ *   queries      fiesta_signed_get_distance_batch / _get_dist_grad_trilinear_batch run the expressions of
+ *                fiesta_get_distance_batch_pos / fiesta_get_dist_grad_trilinear_batch operation for operation; only the voxel read
+ *                differs: a voxel inside B reads S, one outside B (or outside the grid) reads what the map's queries read.  So a
+ *                position none of whose 8 stencil voxels (its voxel, for the distance) is an obstacle with q > 1 gets the map
+ *                query's bits exactly.  The _device forms follow the ordering rules of the stream-ordered queries below (and
+ *                refuse a capturing stream) and return the host forms' bits.
+ * Every output is a fixed integer or fp64 expression of the records: the same bits on every run and as an exact Euclidean
+ * distance transform of the obstacle mask (tests/signedref.py: scipy.ndimage.distance_transform_edt).
+ * Staleness: the map keeps a records epoch that fiesta_update_occupancy, fiesta_update_esdf, fiesta_shard_ingest and
+ * fiesta_shard_relax increment.  Export and queries on a field computed under an older epoch return FIESTA_ERR_INVALID (compute
+ * again), so the voxels inside and outside B always describe the same records.
+ * Memory on the field object, grown as needed with the library's 50 % headroom: 4 bytes of q and 4 bytes of scratch per box voxel
+ * (about 1.6 GB for a 512^3 box); export stages 8 bytes per box voxel for the duration of the call.  Host calls run on the map's
+ * stream and are synchronous.  Destroy the field before the map.  Errors, after which nothing changes: FIESTA_ERR_INVALID for a
+ * box outside the grid or inverted, null buffers where there is work or a negative n, export or queries before a compute or on
+ * a stale field; FIESTA_ERR_CUDA when the buffers cannot be allocated, after which the field must be computed again. */
+typedef struct fiesta_signed_field fiesta_signed_field;
+typedef struct fiesta_signed_stats {
+  int64_t box_voxels, obstacles;
+  int64_t interior;                       /* obstacles with S < 0: q > 1, or every obstacle when B has no non-obstacle voxel */
+  int64_t max_depth_sq;                   /* largest finite q, 0 if none; -1 when B has no non-obstacle voxel and obstacles > 0 */
+  float ms_compute;                       /* device time of the three passes */
+  float reserved_f[1];
+} fiesta_signed_stats;
+int fiesta_signed_create(fiesta_map *m, fiesta_signed_field **out);
+void fiesta_signed_destroy(fiesta_signed_field *f);
+int fiesta_signed_compute(fiesta_signed_field *f, const int box_lo[3], const int box_hi[3], fiesta_signed_stats *stats /* nullable */);
+int fiesta_signed_export(const fiesta_signed_field *f, double *out);   /* box_voxels doubles */
+int fiesta_signed_get_distance_batch(fiesta_signed_field *f, const double *pos_xyz, int64_t n, double *out_dist);
+int fiesta_signed_get_dist_grad_trilinear_batch(fiesta_signed_field *f, const double *pos_xyz, int64_t n, double *out_dist,
+                                                double *out_grad_xyz);
+int fiesta_signed_get_distance_batch_device(fiesta_signed_field *f, const double *d_pos_xyz, int64_t n, double *d_dist, void *stream);
+int fiesta_signed_get_dist_grad_trilinear_batch_device(fiesta_signed_field *f, const double *d_pos_xyz, int64_t n, double *d_dist,
+                                                        double *d_grad_xyz, void *stream);
 
 /* ---- frontier extraction (exploration planners: where does observed free space end?) ----
  * The free voxels of an inclusive voxel box [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis) that border never-observed

@@ -231,6 +231,24 @@ class ESDFMap {
                 int32_t *vox_xyz) {
     check(fiesta_nav_paths(f, starts_xyz, n, max_len, status, len, cost, vox_xyz), "NavPaths");
   }
+  // Signed distance of a box for trajectory optimisers (fiesta_signed_* in fiesta_b200.h): FIESTA's distance outside obstacles,
+  // minus the exact depth inside them.  Compute again after UpdateOccupancy / UpdateESDF.  Destroy with fiesta_signed_destroy
+  // before the map.
+  fiesta_signed_field *MakeSignedField() {
+    fiesta_signed_field *f = nullptr;
+    check(fiesta_signed_create(h_, &f), "MakeSignedField");
+    return f;
+  }
+  fiesta_signed_stats ComputeSignedField(fiesta_signed_field *f, const int box_lo[3], const int box_hi[3]) {
+    fiesta_signed_stats st = {};
+    check(fiesta_signed_compute(f, box_lo, box_hi, &st), "ComputeSignedField");
+    return st;
+  }
+  void ExportSignedField(const fiesta_signed_field *f, double *out) { check(fiesta_signed_export(f, out), "ExportSignedField"); }
+  // GetDistWithGradTrilinear on the signed field: S inside the box, the map's distance outside it (host pointers).
+  void SignedDistWithGradTrilinearBatch(fiesta_signed_field *f, const double *pos_xyz, long n, double *dist, double *grad_xyz) {
+    check(fiesta_signed_get_dist_grad_trilinear_batch(f, pos_xyz, n, dist, grad_xyz), "SignedDistWithGradTrilinearBatch");
+  }
   // Frontier extraction for exploration planners (fiesta_frontiers_* in fiesta_b200.h): the free voxels of a box that border
   // unknown space, in 26-connected clusters with statistics and member lists.  Destroy with fiesta_frontiers_destroy before the map.
   fiesta_frontiers *MakeFrontiers() {
