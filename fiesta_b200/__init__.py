@@ -68,6 +68,12 @@ class FrontierStats(C.Structure):
         ("ms_compute", C.c_float), ("reserved_f", C.c_float * 1)]
 
 
+class SkeletonStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("box_voxels", "traversable", "anchors")] + [("iterations", C.c_int64 * 2)] + [
+        (n, C.c_int64) for n in ("prune_rounds", "pruned_voxels", "skeleton_voxels", "vertices", "edges", "edge_voxels")] + [
+        (n, C.c_float) for n in ("ms_compute", "ms_init", "ms_thin", "ms_graph")]
+
+
 class SensorModel(C.Structure):
     _fields_ = [("max_range", C.c_double), ("tan_half_fov", C.c_double * 2)]
 
@@ -120,6 +126,8 @@ SYMBOLS = [
     "fiesta_signed_create", "fiesta_signed_destroy", "fiesta_signed_compute", "fiesta_signed_export",
     "fiesta_signed_get_distance_batch", "fiesta_signed_get_dist_grad_trilinear_batch", "fiesta_signed_get_distance_batch_device",
     "fiesta_signed_get_dist_grad_trilinear_batch_device",
+    "fiesta_skeleton_create", "fiesta_skeleton_destroy", "fiesta_skeleton_compute", "fiesta_skeleton_vertices",
+    "fiesta_skeleton_edges", "fiesta_skeleton_edge_voxels", "fiesta_skeleton_export",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -202,6 +210,14 @@ def load_library():
         L.fiesta_frontiers_export.argtypes = [C.c_void_p, C.c_void_p]
         L.fiesta_frontiers_score_viewpoints.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
                                                         C.POINTER(SensorModel), C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.fiesta_skeleton_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+        L.fiesta_skeleton_destroy.argtypes = [C.c_void_p]
+        L.fiesta_skeleton_destroy.restype = None
+        L.fiesta_skeleton_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_double, C.c_int64, C.c_void_p]
+        L.fiesta_skeleton_vertices.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4
+        L.fiesta_skeleton_edges.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4
+        L.fiesta_skeleton_edge_voxels.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
+        L.fiesta_skeleton_export.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.fiesta_inflate_boxes.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 4
         L.fiesta_corridors.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 7
         L.fiesta_snapshot_save.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
@@ -560,6 +576,76 @@ class Frontiers:
             self._h = None
 
 
+class Skeleton:
+    """fiesta_skeleton: the topological skeleton of a voxel box's free space -- voxels on the generalized Voronoi diagram of the
+    obstacles, thinned to curves -- as a graph of vertices (junctions, ends) and edges (voxel paths).  The buffers grow to the
+    largest box computed; close() it before the map."""
+
+    def __init__(self, m):
+        self._m = m
+        h = C.c_void_p()
+        m._ck(m._L.fiesta_skeleton_create(m._h, C.byref(h)), "fiesta_skeleton_create")
+        self._h = h
+        self.shape = None
+        self.stats = None
+
+    def compute(self, box_lo, box_hi, clearance=0.0, unknown_blocks=False, max_cos=0.5, min_branch=1):
+        """Skeleton of the inclusive voxel box [box_lo, box_hi] at the clearance (metres) -> stats dict (iterations: a list of the
+        two phases' counts)."""
+        lo, hi = np.ascontiguousarray(box_lo, dtype=np.int32), np.ascontiguousarray(box_hi, dtype=np.int32)
+        if lo.shape != (3,) or hi.shape != (3,):
+            raise ValueError("Skeleton.compute: box_lo and box_hi must be 3 voxel coordinates each")
+        st = SkeletonStats()
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        self._m._ck(self._m._L.fiesta_skeleton_compute(self._h, lo.ctypes, hi.ctypes, r, flags, C.c_double(float(max_cos)),
+                                                        C.c_int64(int(min_branch)), C.byref(st)), "Skeleton.compute")
+        self.shape = tuple(int(b - a + 1) for a, b in zip(lo, hi))
+        self.stats = {n: (list(getattr(st, n)) if n == "iterations" else getattr(st, n)) for n, _ in st._fields_}
+        return dict(self.stats)
+
+    def _need(self, what):
+        if self.stats is None:
+            raise FiestaError("Skeleton.%s: no skeleton has been computed" % what)
+
+    def vertices(self, cap=None):
+        """The vertices (the first `cap`): dict of size (V,) int64, rep (V, 3) int32 grid voxels, centroid (V, 3) float64 metres
+        and degree (V,) int32."""
+        self._need("vertices")
+        k = self.stats["vertices"] if cap is None else min(int(cap), self.stats["vertices"])
+        out = dict(size=np.empty(k, np.int64), rep=np.empty((k, 3), np.int32), centroid=np.empty((k, 3)), degree=np.empty(k, np.int32))
+        self._m._ck(self._m._L.fiesta_skeleton_vertices(self._h, C.c_int64(k), *(out[n].ctypes for n in out)), "Skeleton.vertices")
+        return out
+
+    def edges(self, cap=None):
+        """The edges (the first `cap`): dict of uv (E, 2) int32 vertex ids, n_vox (E,) int64, length and min_dist (E,) float64."""
+        self._need("edges")
+        k = self.stats["edges"] if cap is None else min(int(cap), self.stats["edges"])
+        out = dict(uv=np.empty((k, 2), np.int32), n_vox=np.empty(k, np.int64), length=np.empty(k), min_dist=np.empty(k))
+        self._m._ck(self._m._L.fiesta_skeleton_edges(self._h, C.c_int64(k), *(out[n].ctypes for n in out)), "Skeleton.edges")
+        return out
+
+    def edge_voxels(self, cap=None):
+        """The edge paths concatenated in edge order (the first `cap` voxels) as (n, 3) int32 grid voxels."""
+        self._need("edge_voxels")
+        n = self.stats["edge_voxels"] if cap is None else min(int(cap), self.stats["edge_voxels"])
+        out = np.empty((n, 3), np.int32)
+        self._m._ck(self._m._L.fiesta_skeleton_edge_voxels(self._h, C.c_int64(n), out.ctypes), "Skeleton.edge_voxels")
+        return out
+
+    def export(self):
+        """(mask, labels) as (Bx, By, Bz) arrays: uint8 bits 1 traversable, 2 anchor, 4 skeleton; int32 vertex id, -2 - edge id on
+        chain voxels, -1 elsewhere."""
+        self._need("export")
+        mask, lab = np.empty(self.shape, np.uint8), np.empty(self.shape, np.int32)
+        self._m._ck(self._m._L.fiesta_skeleton_export(self._h, mask.ctypes, lab.ctypes), "Skeleton.export")
+        return mask, lab
+
+    def close(self):
+        if self._h:
+            self._m._L.fiesta_skeleton_destroy(self._h)
+            self._h = None
+
+
 class ESDFMap:
     """Mirror of fiesta::ESDFMap (ESDFMap.h:111-164); every method forwards 1:1 to the C ABI."""
 
@@ -848,6 +934,10 @@ class ESDFMap:
     def Frontiers(self):
         """Frontier voxels of a box (free voxels bordering unknown space) in clusters, with statistics (fiesta_frontiers_*)."""
         return Frontiers(self)
+
+    def Skeleton(self):
+        """Topological skeleton of a box's free space as a graph of junctions and edges (fiesta_skeleton_*)."""
+        return Skeleton(self)
 
     def RaycastFrame(self, xyz, T, min_ray_length, max_ray_length):
         """xyz: (n,3) float32 host array, or an integer device pointer paired with `n` as a tuple (ptr, n)."""

@@ -31,7 +31,7 @@ __device__ __forceinline__ void fr_coords(const FbNavBox &b, long long i, int &x
 }
 __host__ __device__ __forceinline__ long long fr_total(const FbNavBox &b) { return (long long)b.n[0] * b.n[1] * b.n[2]; }
 
-// ---- union-find by index in shared memory (one tile, local indices) and in global memory (the box)
+// ---- union-find by index in shared memory (one tile, local indices); the global-memory form is fr_find / fr_union (fb_frontier.cuh)
 __device__ __forceinline__ unsigned fr_find_s(volatile unsigned *s, unsigned x) {
   unsigned p;
   while ((p = s[x]) != x) x = p;
@@ -47,28 +47,6 @@ __device__ void fr_union_s(unsigned *s, unsigned a, unsigned b) {
     b = old;                                      // b was hooked meanwhile: join a with what it was hooked to
   }
 }
-// Root of x, halving the path on the way.  The shortcut is an atomicMin, so it can only lower a parent word to another ancestor
-// and never undo a concurrent hook.
-__device__ unsigned fr_find(uint32_t *P, unsigned x) {
-  unsigned p = __ldcg(&P[x]);
-  while (p != x) {
-    const unsigned gp = __ldcg(&P[p]);
-    if (gp < p) atomicMin(&P[x], gp);
-    x = p; p = gp;
-  }
-  return x;
-}
-__device__ void fr_union(uint32_t *P, unsigned a, unsigned b) {
-  for (;;) {
-    a = fr_find(P, a); b = fr_find(P, b);
-    if (a == b) return;
-    if (a > b) { const unsigned t = a; a = b; b = t; }
-    const unsigned old = atomicMin(&P[b], a);
-    if (old == b) return;
-    b = old;
-  }
-}
-
 __global__ void __launch_bounds__(FR_THREADS) k_fr_tile(FbGeom g, const uint32_t *__restrict__ cobs, const double *__restrict__ occ,
                                                         double l_occ, double r, FbNavBox b, int tn1, int tn2, uint32_t *P, FbFrCtr *ctr) {
   __shared__ unsigned s[FR_THREADS];

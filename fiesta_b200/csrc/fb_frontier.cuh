@@ -4,6 +4,32 @@
 #include "fb_map.h"
 #include "fb_nav.h"       // FbNavBox: the frontier box uses the cost-to-go field's box layout
 
+// Union-find by index in global memory, shared by the frontier's clusters (over the box) and the skeleton's graph (over its
+// compacted voxels, fb_skel.cu).  Parent words only ever decrease and point at a smaller index of the same component, so after
+// the unions every component is one tree rooted at its smallest index, whatever order they ran in.
+//
+// Root of x, halving the path on the way.  The shortcut is an atomicMin, so it can only lower a parent word to another ancestor
+// and never undo a concurrent hook.
+static __device__ unsigned fr_find(uint32_t *P, unsigned x) {
+  unsigned p = __ldcg(&P[x]);
+  while (p != x) {
+    const unsigned gp = __ldcg(&P[p]);
+    if (gp < p) atomicMin(&P[x], gp);
+    x = p; p = gp;
+  }
+  return x;
+}
+static __device__ void fr_union(uint32_t *P, unsigned a, unsigned b) {
+  for (;;) {
+    a = fr_find(P, a); b = fr_find(P, b);
+    if (a == b) return;
+    if (a > b) { const unsigned t = a; a = b; b = t; }
+    const unsigned old = atomicMin(&P[b], a);
+    if (old == b) return;
+    b = old;
+  }
+}
+
 struct FbFrCtr {
   unsigned long long frontier;     // frontier voxels of the box
   unsigned long long roots;        // clusters before the size filter

@@ -504,6 +504,70 @@ int fiesta_frontiers_score_viewpoints(fiesta_frontiers *f, const int32_t *cluste
                                       double clearance, int flags, int32_t *status, int32_t *score /* n * n_orient, row i = candidate i */,
                                       fiesta_viewpoint_stats *stats /* nullable */);
 
+/* ---- topological roadmaps (global, topology-guided and exploration planners: a sparse graph of the free space) ----
+ * The skeleton of the free space of an inclusive voxel box [box_lo, box_hi] (0 <= lo <= hi < grid size on every axis): voxels on the
+ * discrete generalized Voronoi diagram of the map's obstacles (where the closest obstacle changes sharply between neighbours), thinned
+ * to curves that keep the free space's topology, as a graph of junctions and edges.  A snapshot of the integrated records at the time
+ * of the call; nothing in the map or in any other result changes.  Box indices are ((x-lo.x)*By + (y-lo.y))*Bz + (z-lo.z) as in
+ * fiesta_nav_export.
+ *   traversable  a box voxel that does not block at the clearance and flags in the sense of fiesta_check_segments (so a traversable
+ *                voxel of a cost-to-go field at the same clearance and flags).  Voxels outside the box are not.
+ *   o(v)         the voxel's closest obstacle (fiesta_export_closest_obstacle), defined on observed voxels that have one and are not
+ *                under an EXACT local-map reset (their distance reads +10000).
+ *   anchor       a traversable voxel v with o(v) defined and a traversable face neighbour u in the box with o(u) defined and
+ *                different, where, with a = o(v) - v and b = o(u) - u (exact integer dot products, each fp64 operation rounded on its
+ *                own), (double)(a.b) <= max_cos * sqrt((double)(a.a) * (double)(b.b)).
+ *   thinning     from the traversable set, delete simple voxels (26/6 topology) in iterations of 8 passes over the parity subfields
+ *                s = 4((x-lo.x)&1) + 2((y-lo.y)&1) + ((z-lo.z)&1): phase 1 deletes those that are not anchors, phase 2 those with at
+ *                least two 26-neighbours left (endpoints stay), each until an iteration deletes nothing.  The result does not depend
+ *                on any schedule.
+ *   graph        deg(v) = v's 26-neighbours in the set.  Vertex voxels: deg != 2, and the smallest-index voxel of each component that
+ *                is a pure cycle.  Vertices: the 26-components of vertex voxels; chains: the 26-components of the rest, each a simple
+ *                path whose ends attach to one vertex voxel each.  Vertices and edges are numbered by their smallest box index
+ *                (an edge by its chain's).  An edge is the voxel path attach, chain..., attach, oriented so that (vertex id, attach
+ *                box index, adjacent chain voxel box index) is lexicographically smaller at its start.
+ *   pruning      with min_branch >= 2, rounds until one removes nothing, each removing at once (a) every edge of fewer than min_branch
+ *                path voxels (its leaf counted, the other attachment not) from a leaf (a vertex of one voxel with one neighbour) to a
+ *                different vertex that is not a leaf, with its leaf, and (b) every voxel with one neighbour whose neighbour has >= 3.
+ *                No component is removed.  min_branch 0 or 1: no pruning.
+ *   per vertex   size; rep = its first voxel (grid xyz); centroid (metres) = ((double)S / (double)size + 0.5) * resolution + origin
+ *                per axis, as the frontier clusters'; degree = edge ends attached to it (a self-loop counts twice).
+ *   per edge     uv = (start vertex, end vertex); n_vox = the path's voxel count; length = the left fold, from the start, of the
+ *                cost-to-go field's move weights (resolution * sqrt(non-zero components)); min_dist = the least
+ *                GetDistance(Vector3i) over the path.  fiesta_skeleton_edge_voxels: the paths as grid xyz, concatenated in edge order.
+ *   export       mask: one byte per box voxel, bit 1 traversable, bit 2 anchor, bit 4 final skeleton; label: one int32 per box voxel,
+ *                the vertex id on vertex voxels, -2 - e on the chain voxels of edge e, -1 elsewhere.  Either pointer may be null.
+ * Every output is integer or one fixed fp64 expression: the same bits on every run and as the sequential definition
+ * (tests/skeletonref.py; fiesta_b200/csrc/fb_skel.h, DESIGN.md §3.14).  The _vertices / _edges / _edge_voxels reads write the first
+ * min(cap, n) entries (n = stats.vertices / edges / edge_voxels).  The object owns its device buffers, which grow to the largest box
+ * and result used: 5 bytes per box voxel, 164 per voxel left after thinning and 12 per edge path voxel, with the library's 50 %
+ * growth headroom (about 1 GB for a 512^3 box).  It runs on the map's stream; the calls are synchronous.  Destroy it before the map.
+ * Errors: FIESTA_ERR_INVALID for a box outside the grid or inverted, a clearance or flags fiesta_check_segments rejects, a max_cos
+ * that is NaN or outside [-1, 1), min_branch < 0, null buffers, a negative cap, or reads before a compute; nothing is written then.
+ * FIESTA_ERR_CUDA when the buffers cannot be allocated; a new compute is needed before the results can be read. */
+typedef struct fiesta_skeleton fiesta_skeleton;
+typedef struct fiesta_skeleton_stats {
+  int64_t box_voxels;
+  int64_t traversable, anchors;           /* voxels of X0, and the anchors among them */
+  int64_t iterations[2];                  /* thinning iterations of phases 1 and 2, each counting the one that deleted nothing */
+  int64_t prune_rounds;                   /* pruning rounds, counting the one that removed nothing (0 without pruning) */
+  int64_t pruned_voxels;                  /* voxels pruning removed */
+  int64_t skeleton_voxels, vertices, edges;
+  int64_t edge_voxels;                    /* sum of the edges' n_vox: the length of fiesta_skeleton_edge_voxels */
+  float ms_compute;                       /* device time of the compute, and of its three stages */
+  float ms_init, ms_thin, ms_graph;
+} fiesta_skeleton_stats;
+int fiesta_skeleton_create(fiesta_map *m, fiesta_skeleton **out);
+void fiesta_skeleton_destroy(fiesta_skeleton *f);
+int fiesta_skeleton_compute(fiesta_skeleton *f, const int box_lo[3], const int box_hi[3], double clearance, int flags, double max_cos,
+                            int64_t min_branch, fiesta_skeleton_stats *stats /* nullable */);
+int fiesta_skeleton_vertices(const fiesta_skeleton *f, int64_t cap, int64_t *size, int32_t *rep_xyz /* cap * 3 */,
+                             double *centroid_xyz /* cap * 3 */, int32_t *degree);
+int fiesta_skeleton_edges(const fiesta_skeleton *f, int64_t cap, int32_t *uv /* cap * 2 */, int64_t *n_vox, double *length,
+                          double *min_dist);
+int fiesta_skeleton_edge_voxels(const fiesta_skeleton *f, int64_t cap, int32_t *vox_xyz /* cap * 3 */);
+int fiesta_skeleton_export(const fiesta_skeleton *f, uint8_t *mask /* box_voxels, nullable */, int32_t *label /* box_voxels, nullable */);
+
 /* ---- safe flight corridors (corridor-based trajectory planners: free convex regions around a path) ----
  * Free axis-aligned voxel boxes, inflated face by face, and chains of them along paths in which consecutive boxes share a voxel.
  * All boxes are inclusive voxel boxes; the limit box L = [box_lo, box_hi] satisfies 0 <= lo <= hi < grid size on every axis.

@@ -275,6 +275,29 @@ class ESDFMap {
     check(fiesta_frontiers_score_viewpoints(f, cluster, pos_xyz, n, orient, n_orient, &sensor, clearance, flags, status, score, &st), "ScoreViewpoints");
     return st;
   }
+  // Topological roadmaps (fiesta_skeleton_* in fiesta_b200.h): the skeleton of a box's free space on the generalized Voronoi diagram
+  // of the obstacles, as a graph of vertices and edges.  Destroy with fiesta_skeleton_destroy before the map.
+  fiesta_skeleton *MakeSkeleton() {
+    fiesta_skeleton *f = nullptr;
+    check(fiesta_skeleton_create(h_, &f), "MakeSkeleton");
+    return f;
+  }
+  fiesta_skeleton_stats ComputeSkeleton(fiesta_skeleton *f, const int box_lo[3], const int box_hi[3], double clearance, int flags,
+                                        double max_cos, long min_branch) {
+    fiesta_skeleton_stats st = {};
+    check(fiesta_skeleton_compute(f, box_lo, box_hi, clearance, flags, max_cos, min_branch, &st), "ComputeSkeleton");
+    return st;
+  }
+  void SkeletonVertices(const fiesta_skeleton *f, long cap, int64_t *size, int32_t *rep_xyz, double *centroid_xyz, int32_t *degree) {
+    check(fiesta_skeleton_vertices(f, cap, size, rep_xyz, centroid_xyz, degree), "SkeletonVertices");
+  }
+  void SkeletonEdges(const fiesta_skeleton *f, long cap, int32_t *uv, int64_t *n_vox, double *length, double *min_dist) {
+    check(fiesta_skeleton_edges(f, cap, uv, n_vox, length, min_dist), "SkeletonEdges");
+  }
+  void SkeletonEdgeVoxels(const fiesta_skeleton *f, long cap, int32_t *vox_xyz) {
+    check(fiesta_skeleton_edge_voxels(f, cap, vox_xyz), "SkeletonEdgeVoxels");
+  }
+  void ExportSkeleton(const fiesta_skeleton *f, uint8_t *mask, int32_t *label) { check(fiesta_skeleton_export(f, mask, label), "ExportSkeleton"); }
   // Safe flight corridors (fiesta_inflate_boxes / fiesta_corridors in fiesta_b200.h): free axis-aligned voxel boxes in a limit box,
   // and chains of them along paths in which consecutive boxes share a voxel.
   fiesta_corridor_stats InflateBoxes(const int box_lo[3], const int box_hi[3], const int32_t *seed_lo_xyz, const int32_t *seed_hi_xyz,
