@@ -11,8 +11,8 @@
 //  * The doubly linked dependant lists are replaced by a per-voxel link time LS (time of the last relink; every accepted
 //    write relinks at the list front, :24-42): dependants of deleted obstacles are found by a dense scan and ordered by
 //    (position of the obstacle in delete_queue_, link time descending) = the order of the reference's list walk; their
-//    re-seeding ("first valid neighbour in dirs_ order", :308-321, which sees earlier re-seeded dependants) is iterated to
-//    its fixpoint the same way.
+//    re-seeding ("first valid neighbour in dirs_ order", :308-321, which sees earlier re-seeded dependants) is a validity
+//    closure over that order followed by pointer jumping along the chosen sources (k_x_reseed, fb_xrelax.cu).
 //  * occupancy_queue_ order = order of first observation: every observation carries its serial time (host event number,
 //    or point index and position along the ray) and the per-voxel earliest one is kept (fb_touch).  The integration of a
 //    voxel does not depend on its place in the queue, only the order of the insert_queue_ / delete_queue_ pushes does:
@@ -100,9 +100,9 @@ __global__ void k_x_gather64(const unsigned long long *src, const uint32_t *idx,
 __global__ void k_x_gather32(const uint32_t *src, const uint32_t *idx, unsigned n, uint32_t *dst) {
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) dst[i] = src[idx[i]];
 }
-__global__ void k_x_set_ord(const uint32_t *deps, unsigned n, uint32_t *ord, uint32_t *nc, uint8_t *nk) {
+__global__ void k_x_set_ord(const uint32_t *deps, unsigned n, uint32_t *ord) {
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) { ord[deps[i]] = i; nc[i] = FB_INF; nk[i] = 24; }
+  if (i < n) ord[deps[i]] = i;
 }
 __global__ void k_x_fill32(uint32_t *a, size_t n, uint32_t val) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) a[i] = val;
@@ -160,7 +160,7 @@ int fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t s) {
   const size_t c0 = P / 8 > (1u << 20) ? P / 8 : (1u << 20);
   for (FbDevBuf<unsigned long long> *b : {&X->k1, &X->k2, &X->k1b, &X->k2b}) CK(b->grow(c0, s));
   for (FbDevBuf<uint32_t> *b : {&X->dv, &X->idx[0], &X->idx[1], &X->deps, &X->nc[0], &X->nc[1], &X->sel}) CK(b->grow(c0, s));
-  CK(X->flags.grow(c0, s)); CK(X->flags2.grow(c0, s));
+  CK(X->flags.grow(c0, s));
   CK(X->cub_tmp.grow(c0 * 16 + (64u << 20), s));
   CK(X->d_ctl.alloc(1)); CK(cudaMemsetAsync(X->d_ctl, 0, sizeof(FbXCtl), s));
   CK(X->h_ctl.alloc(1));
@@ -283,17 +283,16 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
           k_x_gather32<<<nblk(ndep), 256, 0, s>>>(X->dv, X->idx[0], ndep, X->deps);
           *launches += 5;
         }
-        CK(X->flags2.grow(ndep, s));
-        k_x_set_ord<<<nblk(ndep), 256, 0, s>>>(X->deps, ndep, scratch, X->nc[0], X->flags2);
+        k_x_set_ord<<<nblk(ndep), 256, 0, s>>>(X->deps, ndep, scratch);
         *launches += 1;
-        ndep_run = ndep; ls_deps = X->tclock;                // the fixpoint and the hand-over to E[0] run inside k_x_relax
+        ndep_run = ndep; ls_deps = X->tclock;                // re-seeded and appended to E[0] by k_x_reseed
         X->tclock += ndep;
       }
     }
   }
   // ---- E3: relax (:338-392): one persistent kernel runs every generation
   st->generations = 0;
-  if (xdbg) { cudaStreamSynchronize(s); fprintf(stderr, "[x] seeds+deletes %.2f ms (reseed rounds %u, dependants %u)\n", ms(t_begin, now()), st->reseed_rounds, st->dependants); }
+  if (xdbg) { cudaStreamSynchronize(s); fprintf(stderr, "[x] seeds+deletes %.2f ms (dependants %u)\n", ms(t_begin, now()), st->dependants); }
   if (nE || ndep_run) {
     if (xdbg && !X->d_dbg) CK(X->d_dbg.alloc(FB_X_DBG_WORDS));
     if (xdbg) CK(cudaMemsetAsync(X->d_dbg, 0, FB_X_DBG_WORDS * 8, s));
@@ -302,13 +301,13 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
     if (X->wclock > 0xf0000000u) { CK(cudaMemsetAsync(X->wstamp, 0, P * 4, s)); X->wclock = 0; }
     FbXCtl *h = X->h_ctl;
     memset(h, 0, sizeof(*h));
-    h->gen_id = X->gen_id; h->wclock = X->wclock; h->tclock = X->tclock; h->sclock = X->sclock;
+    h->gen_id = X->gen_id; h->wclock = X->wclock; h->tclock = X->tclock; h->sclock = X->sclock; h->nE0 = nE;
     CK(cudaMemcpyAsync(X->d_ctl, h, sizeof(FbXCtl), cudaMemcpyHostToDevice, s));
-    CK(fb_xrelax_launch(X, g, cobs, nE, X->deps, ndep_run, scratch, X->nc[0], X->flags2, occbits, ls_deps, xdbg ? X->d_dbg.p : nullptr, s));
+    CK(fb_xrelax_launch(X, g, cobs, X->deps, ndep_run, scratch, X->nc[0], X->nc[1], occbits, ls_deps, xdbg ? X->d_dbg.p : nullptr, s));
     if (ndep_run) k_x_unset<<<nblk(ndep_run), 256, 0, s>>>(X->deps, ndep_run, scratch);
     CK(cudaMemcpyAsync(h, X->d_ctl, sizeof(FbXCtl), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    *launches += 1;
+    *launches += ndep_run ? 2 : 1;                             // k_x_reseed, k_x_relax
     if (h->err) {
       if (h->err == 3u) {                                      // an abandoned work queue may leave marked ring slots and queue
         for (int k = 0; k < 3; ++k) CK(cudaMemsetAsync(X->W[k], 0, P * 4, s));   // states above the saved clock behind
@@ -327,11 +326,12 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
       static double cyc_per_us = 0;                            // clock64 counts SM cycles: convert with this device's SM clock
       if (cyc_per_us == 0) { int dev = 0, khz = 0; CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev)); cyc_per_us = khz / 1000.0; }
       CK(cudaMemcpy(hd, X->d_dbg, sizeof(hd), cudaMemcpyDeviceToHost));
-      // phase categories of k_x_relax (14 and 15 are list-length counters, printed below)
-      static const char *cat[20] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top", "empty-barrier",
-                                    "reseed.rounds", "reseed.assemble", "", "", "async", "", "refresh", "s.async"};
+      // phase categories of k_x_reseed and k_x_relax (14 and 15 are counters, printed below)
+      static const char *cat[FB_XDBG_NCAT] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
+                                              "empty-barrier", "reseed.classify", "reseed.assemble", "", "", "async", "", "refresh", "s.async",
+                                              "reseed.closure", "reseed.choose", "reseed.resolve", ""};
       fprintf(stderr, "[x] reseed rounds %u; phases (us, count):", st->reseed_rounds);
-      for (int c = 0; c < 20; ++c)
+      for (int c = 0; c < FB_XDBG_NCAT; ++c)
         if (*cat[c]) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[FB_XDBG_PHASE + 2 * c] / cyc_per_us, hd[FB_XDBG_PHASE + 2 * c + 1]);
       fprintf(stderr, "\n");
       fprintf(stderr, "[x] round work (summed longest CTA work time us / summed list length):");
@@ -345,7 +345,9 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
       fprintf(stderr, "[x] async: evaluations %llu dirty %llu pushes %llu spin %.0f us\n", hd[FB_XDBG_Q + 0], hd[FB_XDBG_Q + 1], hd[FB_XDBG_Q + 2],
               hd[FB_XDBG_Q + 3] / cyc_per_us);
       for (int gq = 0; gq < 2; ++gq) { fprintf(stderr, "[x] gen %d work lists:", gq); for (int r = 0; r < 512 && hd[FB_XDBG_ROUNDS + gq * 512 + r]; ++r) fprintf(stderr, " %llu", hd[FB_XDBG_ROUNDS + gq * 512 + r]); fprintf(stderr, "\n"); }
-      fprintf(stderr, "[x] work-list entries: evaluated %llu refreshed %llu reseeded %llu\n", hd[FB_XDBG_PHASE + 2 * 14], hd[FB_XDBG_PHASE + 2 * 14 + 1], hd[FB_XDBG_PHASE + 2 * 15]);
+      fprintf(stderr, "[x] work-list entries: evaluated %llu refreshed %llu\n", hd[FB_XDBG_PHASE + 2 * 14], hd[FB_XDBG_PHASE + 2 * 14 + 1]);
+      fprintf(stderr, "[x] reseed: dependants %u final after classify %llu closure rounds %llu list entries %llu resolve passes %llu\n", st->dependants,
+              hd[FB_XDBG_PHASE + 2 * 15], hd[FB_XDBG_PHASE + 2 * 20 + 1], hd[FB_XDBG_PHASE + 2 * 15 + 1], hd[FB_XDBG_PHASE + 2 * 22 + 1]);
       fprintf(stderr, "[x] gens %u rounds %u dense %u deps %u nE0 %u |", st->generations, st->eval_rounds, st->dense_rounds, st->dependants, nE);
       for (unsigned q = 0; q < st->generations && q < FB_XDBG_GENS; ++q) fprintf(stderr, " %llu/%llu/%.1fus", hd[3 * q], hd[3 * q + 1], hd[3 * q + 2] / cyc_per_us);
       fprintf(stderr, "\n");

@@ -5,9 +5,11 @@
 
 #define FB_X_MAX_BLOCKS 256
 #define FB_X_SMALL_DEFAULT 32768u   // (from a sweep on the 512^3 LIDAR frames; FIESTA_X_SMALL / FIESTA_X_DENSE override)
-// Trace layout of k_x_relax (FIESTA_DEBUG_X): [3 * FB_XDBG_GENS] per generation {nE, rounds, cycles}; FB_XDBG_NCAT x {cycles,
-// count} per phase category; 2 x 512 work-list sizes per round (first two generations); 4096 per-round slots for the longest
-// CTA work time of the round (cycles, reset once added up); FB_XDBG_NCAT x {summed longest CTA work time, summed list
+// Trace layout of k_x_reseed and k_x_relax (FIESTA_DEBUG_X): [3 * FB_XDBG_GENS] per generation {nE, rounds, cycles};
+// FB_XDBG_NCAT x {cycles, count} per phase category (re-seeding: 12 classify, 20 closure, 21 choose, 22 resolve, 13 assemble;
+// the counts of 20 and 22 are the closure rounds and the resolve passes; 15 holds the dependants final after the
+// classification and the summed closure list lengths instead); 2 x 512 work-list sizes per round (first two generations);
+// 4096 per-round slots for the longest CTA work time of the round (cycles, reset once added up); FB_XDBG_NCAT x {summed longest CTA work time, summed list
 // length} per round category; 2 x 32 log2 histograms of the list lengths of BIG short-list rounds and SMALL later rounds;
 // FB_XDBG_NQ counters of the asynchronous schedule.
 #define FB_XDBG_GENS 1024
@@ -24,13 +26,16 @@
 struct FbExactStats {
   unsigned long long expansions;      // == the reference's "Expanding N nodes" (ESDFMap.cpp:347,394)
   unsigned long long voxels_changed;  // accepted final writes over all generations
-  unsigned generations, eval_rounds, dense_rounds, reseed_rounds, dependants;
+  unsigned generations, eval_rounds, dense_rounds, dependants;
+  unsigned reseed_rounds;             // re-seeding of the dependants (k_x_reseed): closure rounds + pointer-jumping passes
 };
 
 // Control block of k_x_relax (device memory; the host writes it before and reads it after every launch).
 struct FbXCtl {
   unsigned bar, err;                  // grid barrier arrivals; 1 = a generation exceeded 2^27 entries
-  unsigned sclock, pad1;              // stamp of the last summary pass (SUMg dedupe; persists across launches)
+  unsigned sclock;                    // stamp of the last summary pass (SUMg dedupe; persists across launches)
+  unsigned rbar;                      // grid barrier arrivals of k_x_reseed
+  unsigned nE0;                       // entries of generation 0: the insert seeds, plus the re-seeded dependants k_x_reseed appends
   unsigned nW[3], nF[3];              // work / flip list lengths, rotating per round
   unsigned gen_id, wclock;            // stamps for SUMg / wstamp dedupe (persist across launches)
   unsigned generations, rounds, dense_rounds, reseed_rounds;
@@ -73,7 +78,7 @@ struct FbExact {
   FbDevBuf<uint32_t> E[2], sel;
   FbDevBuf<unsigned long long> k1, k2, k1b, k2b;
   FbDevBuf<uint32_t> dv, idx[2], deps, nc[2];
-  FbDevBuf<uint8_t> flags, flags2;
+  FbDevBuf<uint8_t> flags;
   FbDevBuf<char> cub_tmp;
 };
 
@@ -88,5 +93,5 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
 // fb_xrelax.cu
 cudaError_t fb_xrelax_init();
 int fb_xrelax_blocks(int device);
-cudaError_t fb_xrelax_launch(FbExact *X, const FbGeom &g, uint32_t *cobs, unsigned nE0, const uint32_t *deps, unsigned ndep, uint32_t *ord, uint32_t *nc, uint8_t *nk,
+cudaError_t fb_xrelax_launch(FbExact *X, const FbGeom &g, uint32_t *cobs, const uint32_t *deps, unsigned ndep, uint32_t *ord, uint32_t *nc, uint32_t *M,
                              const uint32_t *occbits, unsigned long long ls_deps, unsigned long long *dbg, cudaStream_t s);

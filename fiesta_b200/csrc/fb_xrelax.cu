@@ -24,9 +24,9 @@
 //  * Hand-over: element i owns slot k iff the final state of its k-th target carries the timestamp 32*i + k; the owned slots in
 //    timestamp order (per-element masks, exclusive scan over CTA-contiguous ranges) are the next generation; old words are
 //    retired by compare-and-swap (a generation-parity bit tells old from new).
-//  * Before generation 0 the same kernel iterates the delete loop's re-seeding ("first valid neighbour in dirs_ order",
-//    earlier dependants expose their new value, :308-321) to its fixpoint over work lists and appends the re-seeded
-//    dependants, in list-walk order, to the insert seeds.
+//  * Before it, k_x_reseed re-seeds the dependants of the deleted obstacles (:308-321) in four stages (see there) and appends
+//    the re-seeded ones, in list-walk order, to the insert seeds in E[0]; k_x_relax reads generation 0's length from
+//    ctl->nE0.
 #include <stdio.h>
 #include "fb_common.cuh"
 #include "fb_exact.h"
@@ -42,9 +42,8 @@
 #define X_NOFF 129
 #define X_MAX_ROUNDS 4000000u
 #define XGB 8                         // writer words loaded per batch by a gather (24 / XGB batches)
-#define XRC 8                         // directions listed per chunk after a re-seeding change (24 / XRC chunks)
-// trace layout (FIESTA_DEBUG_X): fb_exact.h.  Phase categories 14 and 15 hold summed work / flip list lengths and summed
-// re-seeding list lengths instead of times.
+// trace layout (FIESTA_DEBUG_X): fb_exact.h.  Phase categories 14 and 15 hold summed work / flip list lengths, and the
+// dependants final after the classification / summed closure list lengths, instead of times.
 #define XDBG_PHASE FB_XDBG_PHASE
 #define XDBG_ROUNDS FB_XDBG_ROUNDS
 #define XDBG_WMAX FB_XDBG_WMAX
@@ -212,12 +211,12 @@ struct XArgs {
   uint32_t *wstamp;
   uint32_t *slotc;          // SMALL mode: winner codes, [small_max][32]
   FbXCtl *ctl;
-  unsigned nE0, small_max, dense_min;  // nE0: insert seeds already in E[0]
+  unsigned small_max, dense_min;
   // E2 (delete loop): dependants of deleted obstacles in the order of the reference's list walk
   const uint32_t *deps; unsigned ndep;
   uint32_t *ord;            // per voxel: position in deps, or XNONE
-  uint32_t *nc;             // per dependant: re-seeded code (FB_INF at start)
-  uint8_t *nk;              // per dependant: direction of the neighbour the code was taken from (24 = none)
+  uint32_t *nc;             // per dependant: re-seeded code (k_x_reseed: or X_PAR | parent dependant)
+  uint32_t *M;              // per dependant: k_x_reseed's mask of earlier dependant neighbours | X_STATIC | X_VALID
   const uint32_t *occbits;
   unsigned long long ls_deps;   // link time of dependant 0 (InsertIntoList order, :333)
   unsigned long long *dbg;  // optional per-generation trace {nE, rounds, ns} (FIESTA_DEBUG_X)
@@ -477,24 +476,6 @@ __device__ __forceinline__ unsigned x_block_scan(XShared &sh, unsigned c, unsign
   return __shfl_sync(0xffffffffu, s - v, (int)wid) + incl - c;
 }
 
-// Reserves n (< 16) consecutive slots per lane of the lanes active here behind `counter`: one atomic per warp.  The exclusive
-// prefix of n over the active lanes is built from one ballot per bit of n.
-__device__ __forceinline__ unsigned x_warp_append_n(unsigned *counter, unsigned n, unsigned lane) {
-  const unsigned act = __activemask(), below = (1u << lane) - 1u;
-  unsigned pre = 0, total = 0;
-#pragma unroll
-  for (int bit = 0; bit < 4; ++bit) {
-    const unsigned m = __ballot_sync(act, (n >> bit) & 1u);
-    pre += (unsigned)__popc(m & below) << bit;
-    total += (unsigned)__popc(m) << bit;
-  }
-  if (total == 0u) return 0u;
-  const int leader = __ffs(act) - 1;
-  unsigned base = 0;
-  if ((int)lane == leader) base = atomicAdd(counter, total);
-  return __shfl_sync(act, base, leader) + pre;
-}
-
 // ---- asynchronous schedule of the short work lists ------------------------------------------------------------------------
 // Rounds are a scheduling device: element i's behaviour depends only on the words of earlier elements, so the fixpoint is
 // unique and every fair schedule that re-evaluates an element after each change of its inputs reaches it (by induction on
@@ -720,29 +701,248 @@ __device__ void x_async_small(const XArgs &a, XShared &sh, XNb &stg, unsigned la
   }
 }
 
-// One evaluation of the re-seeding rule: dependant i takes the closest obstacle of the FIRST neighbour in dirs_ order that
-// has a valid one (:308-321); dependants processed earlier expose their new value, later ones their (deleted) old one.
-__device__ __forceinline__ uint32_t x_reseed_eval(const XArgs &a, unsigned i, int x, int y, int z, unsigned &kc) {
-  const FbGeom &g = a.g;
-  kc = 24u;
-  for (int k = 0; k < 24; ++k) {
-    const int nx = x + x_dirs[k][0], ny = y + x_dirs[k][1], nz = z + x_dirs[k][2];
-    if (!x_in_range(g, nx, ny, nz) || !x_in_grid(g, nx, ny, nz)) continue;
-    const unsigned nv = x_vi(g, nx, ny, nz);
-    const unsigned o = __ldcg(&a.ord[nv]);
-    uint32_t c;
-    if (o != XNONE) { if (o < i) c = __ldcg(&a.nc[o]); else continue; }
-    else c = __ldcg(&a.cobs[nv]) & FB_CODE_MASK;
-    if (c >= 2u) {
-      int ox, oy, oz; fb_unpack(c, ox, oy, oz);
-      const unsigned oi = x_vi(g, ox, oy, oz);
-      if ((__ldg(&a.occbits[oi >> 5]) >> (oi & 31)) & 1u) { kc = (unsigned)k; return c; }   // Exist(closest obstacle) (:312), then `break` (:319)
-    }
+extern __shared__ __align__(16) unsigned char x_dyn_smem[];
+
+// ---- E2, second half: re-seeding of the dependants of the deleted obstacles (:301-334) ----------------------------------
+// The reference walks the dependants in list order and gives dependant i the closest obstacle of the FIRST neighbour, in
+// dirs_ order and inside the update box, whose closest obstacle exists (:308-321); earlier dependants show their new value,
+// later ones are skipped.  So i's final code is INF or a code copied, through a chain of earlier dependants, from a
+// non-dependant neighbour that passed the Exist test (a static source).  It follows that
+//  * validity is monotone: i ends valid iff it has a static source or an earlier dependant neighbour that ends valid.  This
+//    is an OR closure over a DAG (o -> i only for o < i): each dependant turns valid at most once;
+//  * once validity is known, i's source is local: its first direction, in dirs_ order, whose neighbour is a static source
+//    or a valid earlier dependant (its parent);
+//  * parents have smaller indices, so pointer jumping resolves every code in ceil(log2(longest chain)) + 1 passes.
+// By induction on i this is the sequential rule, whatever the dependant order.  k_x_reseed runs it in four stages separated
+// by grid barriers (CPU model checked against the sequential rule: scripts/reseed_model.c):
+//  A classify  one thread per dependant walks its neighbours up to the first static source: nc[i] = its code, or INF;
+//              M[i] = the mask of the earlier dependant neighbours before it | X_STATIC | X_VALID if there is one.  An empty
+//              mask is final.
+//  B closure   round 1: every dependant with no static source and a non-empty mask becomes X_VALID if a masked neighbour
+//              is (pull); each later round: every dependant made valid in the round before marks its later dependant
+//              neighbours that have no static source (push, atomicOr: each enters a list once).  Until a round lists none.
+//  C choose    a valid dependant with a non-empty mask takes its first masked valid neighbour as parent: nc[i] = X_PAR | o.
+//  D resolve   nc[i] = nc[parent] over the dependants still holding a parent, until none does.  In place: a concurrent
+//              write only moves a parent further up its chain, and a 32-bit word never tears.
+// ctl->reseed_rounds = the rounds of B plus the passes of D.
+#define X_STATIC 0x20000000u
+#define X_VALID 0x40000000u
+#define X_PAR 0x80000000u                // codes use 31 bits (FB_CODE_MASK)
+#define X_LAP(cat) do { if (DBG && gtid == 0) { const long long t_now = clock64(); a.dbg[XDBG_PHASE + 2 * (cat)] += (unsigned long long)(t_now - t_ph); a.dbg[XDBG_PHASE + 2 * (cat) + 1] += 1ull; t_ph = t_now; } } while (0)
+
+// The dependant at the in-grid, in-box voxel x + dirs_[k] (XNONE: none, or outside the grid or the box) for the directions
+// k = K0..K0+7 set in `want`: all loads of a chunk are issued before any is looked at.
+template <int K0>
+__device__ __forceinline__ void x_dep_nb(const XArgs &a, int x, int y, int z, unsigned want, unsigned (&nv)[8], unsigned (&o)[8]) {
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+    const int nx = x + x_dc(K0 + t, 0), ny = y + x_dc(K0 + t, 1), nz = z + x_dc(K0 + t, 2);
+    nv[t] = ((want >> (K0 + t)) & 1u) && x_in_grid(a.g, nx, ny, nz) && x_in_range(a.g, nx, ny, nz) ? x_vi(a.g, nx, ny, nz) : XNONE;
+    o[t] = nv[t] != XNONE ? __ldcg(&a.ord[nv[t]]) : XNONE;
   }
-  return FB_INF;
+}
+// first masked direction of chunk K0 whose dependant is valid (24: none)
+template <int K0>
+__device__ __forceinline__ unsigned x_first_valid(const XArgs &a, int x, int y, int z, unsigned mask, unsigned &par) {
+  unsigned nv[8], o[8], m[8];
+  x_dep_nb<K0>(a, x, y, z, mask, nv, o);                     // a masked direction holds an earlier dependant
+#pragma unroll
+  for (int t = 0; t < 8; ++t) m[t] = o[t] != XNONE ? __ldcg(&a.M[o[t]]) : 0u;
+#pragma unroll
+  for (int t = 0; t < 8; ++t) if (m[t] & X_VALID) { par = o[t]; return (unsigned)(K0 + t); }
+  return 24u;
+}
+// A for dependant i: directions K0..K0+7 (until `done`)
+template <int K0>
+__device__ __forceinline__ void x_classify(const XArgs &a, unsigned i, int x, int y, int z, unsigned &mask, uint32_t &sc, bool &done) {
+  unsigned nv[8], o[8];
+  uint32_t c[8];
+  x_dep_nb<K0>(a, x, y, z, 0xffffffu, nv, o);
+#pragma unroll
+  for (int t = 0; t < 8; ++t) c[t] = (nv[t] != XNONE && o[t] == XNONE) ? __ldcg(&a.cobs[nv[t]]) & FB_CODE_MASK : 0u;
+  unsigned e[8];
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+    e[t] = 0u;
+    if (c[t] >= 2u) { int ox, oy, oz; fb_unpack(c[t], ox, oy, oz); const unsigned oi = x_vi(a.g, ox, oy, oz); e[t] = (__ldg(&a.occbits[oi >> 5]) >> (oi & 31)) & 1u; }
+  }
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+    if (done || nv[t] == XNONE) continue;
+    if (o[t] != XNONE) { if (o[t] < i) mask |= 1u << (K0 + t); }
+    else if (e[t]) { sc = c[t]; done = true; }                // Exist(closest obstacle) (:312), then `break` (:319)
+  }
+}
+// B, push (if `act`): the later dependants without a static source next to the newly valid dependant o at (x,y,z), directions
+// K0..K0+7, turn valid and are listed in W[out].  Called by whole warps (the appends are warp-aggregated).
+template <int K0>
+__device__ __forceinline__ void x_mark_later(const XArgs &a, bool act, unsigned o, int x, int y, int z, unsigned out) {
+  unsigned j[8], m[8];
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+    const int nx = x + x_dc(K0 + t, 0), ny = y + x_dc(K0 + t, 1), nz = z + x_dc(K0 + t, 2);
+    j[t] = act && x_in_grid(a.g, nx, ny, nz) ? __ldcg(&a.ord[x_vi(a.g, nx, ny, nz)]) : XNONE;
+  }
+#pragma unroll
+  for (int t = 0; t < 8; ++t) m[t] = (j[t] != XNONE && j[t] > o) ? __ldcg(&a.M[j[t]]) : X_VALID;
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+    const bool push = !(m[t] & (X_STATIC | X_VALID)) && !(atomicOr(&a.M[j[t]], X_VALID) & X_VALID);
+    const unsigned slot = fb_warp_append(&a.ctl->nW[out], push);
+    if (push) a.W[out][slot] = j[t];
+  }
 }
 
-extern __shared__ __align__(16) unsigned char x_dyn_smem[];
+template <bool DBG>
+__global__ void __launch_bounds__(XT, 1) k_x_reseed(const XArgs a) {
+  __shared__ XShared sh;
+  FbXCtl *ctl = a.ctl;
+  const unsigned tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5, G = gridDim.x, b = blockIdx.x;
+  const unsigned gtid = b * XT + tid, gthreads = G * XT;
+  unsigned bar_target = 0;
+  long long t_ph = DBG ? clock64() : 0;
+  // A: classify; the dependants with a non-empty mask and no static source are the list of B's first round (W[1])
+  for (unsigned i0 = 0; i0 < a.ndep; i0 += gthreads) {
+    const unsigned i = i0 + gtid;
+    unsigned mask = 0;
+    uint32_t sc = FB_INF;
+    bool done = true;
+    if (i < a.ndep) {
+      int x, y, z; x_coords(a, __ldcg(&a.deps[i]), x, y, z);
+      done = false;
+      x_classify<0>(a, i, x, y, z, mask, sc, done);
+      if (!done) x_classify<8>(a, i, x, y, z, mask, sc, done);
+      if (!done) x_classify<16>(a, i, x, y, z, mask, sc, done);
+      a.nc[i] = sc;
+      a.M[i] = mask | (done ? X_STATIC | X_VALID : 0u);
+    }
+    const bool pull = !done && mask;
+    const unsigned slot = fb_warp_append(&ctl->nW[1], pull);
+    if (pull) a.W[1][slot] = i;
+    if (DBG) { const unsigned f = __popc(__ballot_sync(0xffffffffu, i < a.ndep && !mask)); if ((threadIdx.x & 31u) == 0 && f) atomicAdd(&a.dbg[XDBG_PHASE + 2 * 15], (unsigned long long)f); }
+  }
+  x_gsync(&ctl->rbar, bar_target);
+  X_LAP(12);
+  // B: closure rounds over the lists W[r % 3] (the list counters rotate as in k_x_relax's rounds)
+  unsigned r = 1, rounds = 0;
+  for (;; ++r) {
+    const unsigned in = r % 3u, out = (r + 1u) % 3u, zz = (r + 2u) % 3u;
+    const unsigned nw = __ldcg(&ctl->nW[in]);
+    if (gtid == 0) ctl->nW[zz] = 0;
+    if (nw == 0u) break;
+    ++rounds;
+    if (DBG && gtid == 0) a.dbg[XDBG_PHASE + 2 * 15 + 1] += nw;
+    for (unsigned q0 = 0; q0 < nw; q0 += gthreads) {          // (every warp runs the same iterations: its appends are collective)
+      const unsigned q = q0 + gtid;
+      const bool act = q < nw;
+      const unsigned i = act ? __ldcg(&a.W[in][q]) : 0u;
+      int x = 0, y = 0, z = 0;
+      if (act) x_coords(a, __ldcg(&a.deps[i]), x, y, z);
+      if (r == 1u) {                                           // pull: a masked neighbour is valid
+        unsigned k = 24u, par;
+        if (act) {
+          const unsigned mask = __ldcg(&a.M[i]);
+          k = x_first_valid<0>(a, x, y, z, mask, par);
+          if (k == 24u) k = x_first_valid<8>(a, x, y, z, mask, par);
+          if (k == 24u) k = x_first_valid<16>(a, x, y, z, mask, par);
+          if (k != 24u) a.M[i] = mask | X_VALID;               // nobody else writes M[i] in this round
+        }
+        const unsigned slot = fb_warp_append(&ctl->nW[out], k != 24u);
+        if (k != 24u) a.W[out][slot] = i;
+      } else {                                                 // push; later dependants see this one only inside the box
+        const bool push = act && x_in_range(a.g, x, y, z);
+        x_mark_later<0>(a, push, i, x, y, z, out);
+        x_mark_later<8>(a, push, i, x, y, z, out);
+        x_mark_later<16>(a, push, i, x, y, z, out);
+      }
+    }
+    x_gsync(&ctl->rbar, bar_target);
+    X_LAP(20);
+  }
+  // C: choose the parents; the dependants that took one are the list of D's first pass
+  {
+    const unsigned out = (r + 1u) % 3u;
+    for (unsigned i0 = 0; i0 < a.ndep; i0 += gthreads) {
+      const unsigned i = i0 + gtid;
+      const unsigned m = i < a.ndep ? __ldcg(&a.M[i]) : 0u;
+      unsigned k = 24u, par = 0;
+      if ((m & X_VALID) && (m & 0xffffffu)) {
+        int x, y, z; x_coords(a, __ldcg(&a.deps[i]), x, y, z);
+        k = x_first_valid<0>(a, x, y, z, m, par);
+        if (k == 24u) k = x_first_valid<8>(a, x, y, z, m, par);
+        if (k == 24u) k = x_first_valid<16>(a, x, y, z, m, par);
+        if (k != 24u) a.nc[i] = X_PAR | par;                   // else the static code stays
+      }
+      const unsigned slot = fb_warp_append(&ctl->nW[out], k != 24u);
+      if (k != 24u) a.W[out][slot] = i;
+    }
+    x_gsync(&ctl->rbar, bar_target);
+    X_LAP(21);
+  }
+  // D: resolve by pointer jumping
+  unsigned passes = 0;
+  for (++r;; ++r) {
+    const unsigned in = r % 3u, out = (r + 1u) % 3u, zz = (r + 2u) % 3u;
+    const unsigned nw = __ldcg(&ctl->nW[in]);
+    if (gtid == 0) ctl->nW[zz] = 0;
+    if (nw == 0u) break;
+    ++passes;
+    for (unsigned q0 = 0; q0 < nw; q0 += gthreads) {
+      const unsigned q = q0 + gtid;
+      bool again = false;
+      unsigned i = 0;
+      if (q < nw) {
+        i = __ldcg(&a.W[in][q]);
+        const uint32_t c = __ldcg(&a.nc[__ldcg(&a.nc[i]) & ~X_PAR]);
+        a.nc[i] = c;
+        again = (c & X_PAR) != 0u;
+      }
+      const unsigned slot = fb_warp_append(&ctl->nW[out], again);
+      if (again) a.W[out][slot] = i;
+    }
+    x_gsync(&ctl->rbar, bar_target);
+    X_LAP(22);
+  }
+  // Hand-over: the re-seeded dependants, in list-walk order, follow the insert seeds in E[0] (:329-333): per-CTA counts over
+  // CTA-contiguous ranges, then an exclusive scan
+  const unsigned per = (a.ndep + G - 1u) / G;
+  const unsigned lo = min(a.ndep, b * per), hi = min(a.ndep, lo + per);
+  unsigned mine = 0;
+  for (unsigned i = lo + tid; i < hi; i += XT) mine += __ldcg(&a.nc[i]) >= 2u ? 1u : 0u;
+  unsigned tot;
+  x_block_scan(sh, mine, lane, wid, tot);
+  if (tid == 0) ctl->partial[b] = tot;
+  const unsigned nE = __ldcg(&ctl->nE0);                       // the insert seeds
+  x_gsync(&ctl->rbar, bar_target);
+  if (wid == 0) {
+    unsigned before = 0, all = 0;
+    for (unsigned k = lane; k < G; k += 32u) { const unsigned c = __ldcg(&ctl->partial[k]); all += c; if (k < b) before += c; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { before += __shfl_xor_sync(0xffffffffu, before, o); all += __shfl_xor_sync(0xffffffffu, all, o); }
+    if (lane == 0) { sh.base = before; sh.total = all; }
+  }
+  __syncthreads();
+  unsigned run = nE + sh.base;
+  for (unsigned i0 = lo; i0 < hi; i0 += XT) {
+    const unsigned i = i0 + tid;
+    uint32_t c = FB_INF, v = 0;
+    if (i < hi) {
+      c = __ldcg(&a.nc[i]); v = __ldcg(&a.deps[i]);
+      a.cobs[v] = c;
+      a.LS[v] = a.ls_deps + i;                                 // InsertIntoList(new_obs_idx, obs_idx) (:333)
+    }
+    unsigned ctot;
+    const unsigned pos = x_block_scan(sh, (i < hi && c >= 2u) ? 1u : 0u, lane, wid, ctot);
+    if (i < hi && c >= 2u) a.E[0][run + pos] = v;              // `if (distance < infinity_) update_queue_.push` (:329-331)
+    run += ctot;
+  }
+  if (gtid == 0) {                                             // (every CTA has read nE0 and the list counters)
+    ctl->nE0 = nE + sh.total;
+    ctl->reseed_rounds = rounds + passes;
+    ctl->nW[0] = ctl->nW[1] = ctl->nW[2] = 0;
+  }
+  X_LAP(13);
+}
 
 // DBG: the FIESTA_DEBUG_X trace (a.dbg != nullptr).  The production instance carries none of its clocks and counters, which
 // would otherwise stay live across the generation loop and the queue phases (spills at the 64-register limit).
@@ -774,7 +974,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
   XNb &stg = reinterpret_cast<XNb *>(x_dyn_smem)[wid];
 
   // grid-uniform state (every CTA computes the same values)
-  unsigned nE = a.nE0, bar_target = 0;
+  unsigned nE = ctl->nE0, bar_target = 0;
   int cur = 0;
   unsigned gen = ctl->gen_id, wclock = ctl->wclock;
   unsigned long long tclock = ctl->tclock;
@@ -786,137 +986,6 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
     if (gtid == 0) a.dbg[XDBG_PHASE + 2 * 11] = (unsigned long long)(clock64() - t0) / 32ull;
   }
   long long t_ph = DBG ? clock64() : 0;
-#define X_LAP(cat) do { if (DBG && gtid == 0) { const long long t_now = clock64(); a.dbg[XDBG_PHASE + 2 * (cat)] += (unsigned long long)(t_now - t_ph); a.dbg[XDBG_PHASE + 2 * (cat) + 1] += 1ull; t_ph = t_now; } } while (0)
-  // ---- E2, second half: re-seed the dependants of the deleted obstacles (fixpoint over work lists, in place), then append
-  // the re-seeded ones, in list-walk order, to the insert seeds in E[0] (:301-334).
-  unsigned reseed_rounds = 0;
-  if (a.ndep) {
-    for (unsigned r = 1;; ++r) {
-      const unsigned in = r % 3u, out = (r + 1u) % 3u, zz = (r + 2u) % 3u;
-      const unsigned nw = r == 1u ? a.ndep : __ldcg(&ctl->nW[in]);
-      if (gtid == 0) ctl->nW[zz] = 0;
-      if (r > 1u && nw == 0u) break;
-      if (DBG && gtid == 0) a.dbg[XDBG_PHASE + 2 * 15] += nw;
-      ++reseed_rounds; ++wclock;
-      if (nw <= 2u * gwarps) {
-        // short list: one WARP per dependant, lane k = neighbour k -- the 24 look-ups (position in deps, code, Exist bit) run side
-        // by side (three round trips instead of up to 72 one after the other); the round's length is what the sweep costs
-        for (unsigned q = gwarp; q < nw; q += gwarps) {
-          const unsigned i = r == 1u ? q : __ldcg(&a.W[in][q]);
-          int x, y, z; x_coords(a, __ldcg(&a.deps[i]), x, y, z);
-          int dx = 0, dy = 0, dz = 0;
-          if (lane < 24u) x_unpack_off(sh.dir[lane], dx, dy, dz);
-          const int nx = x + dx, ny = y + dy, nz = z + dz;
-          const bool ing = lane < 24u && x_in_grid(g, nx, ny, nz);
-          const unsigned nv = ing ? x_vi(g, nx, ny, nz) : 0u;
-          const unsigned o = ing ? __ldcg(&a.ord[nv]) : XNONE;
-          uint32_t c = 0;
-          if (ing && x_in_range(g, nx, ny, nz)) {
-            if (o != XNONE) { if (o < i) c = __ldcg(&a.nc[o]); }
-            else c = __ldcg(&a.cobs[nv]) & FB_CODE_MASK;
-          }
-          bool ok = false;
-          if (c >= 2u) { int px, py, pz; fb_unpack(c, px, py, pz); const unsigned oi = x_vi(g, px, py, pz); ok = (__ldg(&a.occbits[oi >> 5]) >> (oi & 31)) & 1u; }
-          const unsigned vm = __ballot_sync(0xffffffffu, ok);
-          const unsigned kc = vm ? (unsigned)(__ffs(vm) - 1) : 24u;                 // first valid neighbour in dirs_ order (:308-321)
-          const uint32_t res = vm ? __shfl_sync(0xffffffffu, c, (int)kc) : FB_INF;
-          uint32_t was = 0;
-          if (lane == 0) { was = __ldcg(&a.nc[i]); a.nk[i] = (uint8_t)kc; }
-          was = __shfl_sync(0xffffffffu, was, 0);
-          if (res == was) continue;
-          if (lane == 0) a.nc[i] = res;
-          bool push = ing && o != XNONE && o > i;                                  // later dependants that look at this one
-          if (push) {
-            const unsigned so = __ldcg(&a.wstamp[o]);
-            push = so != wclock;
-            if (push && r > 1u && so != wclock - 1u) {                              // stable choice of a dependant not evaluated this round (see below)
-              const unsigned ko = __ldcg(&a.nk[o]), kd = lane ^ 1u;
-              push = kd == ko || (kd < ko && res >= 2u);
-            }
-            push = push && atomicExch(&a.wstamp[o], wclock) != wclock;
-          }
-          const unsigned slot2 = fb_warp_append(&ctl->nW[out], push);
-          if (push) a.W[out][slot2] = o;
-        }
-      } else
-      for (unsigned q = gtid; q < nw; q += gthreads) {
-        const unsigned i = r == 1u ? q : __ldcg(&a.W[in][q]);
-        int x, y, z; x_coords(a, __ldcg(&a.deps[i]), x, y, z);
-        unsigned kc;
-        const uint32_t res = x_reseed_eval(a, i, x, y, z, kc);
-        const uint32_t was = __ldcg(&a.nc[i]);
-        a.nk[i] = (uint8_t)kc;
-        if (res == was) continue;
-        a.nc[i] = res;
-        // later dependants that look at this one, XRC directions at a time: every stage issues its loads (or atomics) for
-        // all of them before the next stage looks at the results, and the chunk ends with one append per warp -- a few
-        // round trips per chunk instead of up to five per direction, one after the other
-#pragma unroll
-        for (int k0 = 0; k0 < 24; k0 += XRC) {
-          unsigned o[XRC], so[XRC], ko[XRC];
-#pragma unroll
-          for (int t = 0; t < XRC; ++t) {
-            const int k = k0 + t, nx = x + x_dc(k, 0), ny = y + x_dc(k, 1), nz = z + x_dc(k, 2);
-            o[t] = x_in_grid(g, nx, ny, nz) ? __ldcg(&a.ord[x_vi(g, nx, ny, nz)]) : XNONE;
-          }
-#pragma unroll
-          for (int t = 0; t < XRC; ++t) so[t] = (o[t] != XNONE && o[t] > i) ? __ldcg(&a.wstamp[o[t]]) : wclock;   // wclock = not a candidate
-          // A dependant that is NOT being evaluated in this round holds a stable choice: it looks at this voxel through
-          // direction k^1 and only cares if that direction comes before its current source (and this one became valid) or
-          // is its current source.  One that is being evaluated right now may have missed the new value: always listed.
-#pragma unroll
-          for (int t = 0; t < XRC; ++t) ko[t] = (so[t] != wclock && r > 1u && so[t] != wclock - 1u) ? __ldcg(&a.nk[o[t]]) : XNONE;
-          unsigned pm = 0;
-#pragma unroll
-          for (int t = 0; t < XRC; ++t) {
-            const unsigned kd = (unsigned)(k0 + t) ^ 1u;
-            bool push = so[t] != wclock;                       // not listed for the next round yet
-            if (push && ko[t] != XNONE) push = kd == ko[t] || (kd < ko[t] && res >= 2u);
-            if (push && atomicExch(&a.wstamp[o[t]], wclock) != wclock) pm |= 1u << t;
-          }
-          unsigned slot2 = x_warp_append_n(&ctl->nW[out], (unsigned)__popc(pm), lane);
-#pragma unroll
-          for (int t = 0; t < XRC; ++t) if ((pm >> t) & 1u) a.W[out][slot2++] = o[t];
-        }
-      }
-      x_gsync(&ctl->bar, bar_target);
-    }
-    X_LAP(12);
-    const unsigned per = (a.ndep + G - 1u) / G;
-    const unsigned lo = min(a.ndep, b * per), hi = min(a.ndep, lo + per);
-    unsigned mine = 0;
-    for (unsigned i = lo + tid; i < hi; i += XT) mine += __ldcg(&a.nc[i]) >= 2u ? 1u : 0u;
-    unsigned tot;
-    x_block_scan(sh, mine, lane, wid, tot);
-    if (tid == 0) ctl->partial[b] = tot;
-    if (gtid == 0) { ctl->nW[0] = ctl->nW[1] = ctl->nW[2] = 0; }
-    x_gsync(&ctl->bar, bar_target);
-    if (wid == 0) {
-      unsigned before = 0, all = 0;
-      for (unsigned k = lane; k < G; k += 32u) { const unsigned c = __ldcg(&ctl->partial[k]); all += c; if (k < b) before += c; }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) { before += __shfl_xor_sync(0xffffffffu, before, o); all += __shfl_xor_sync(0xffffffffu, all, o); }
-      if (lane == 0) { sh.base = before; sh.total = all; }
-    }
-    __syncthreads();
-    unsigned run = nE + sh.base;
-    for (unsigned i0 = lo; i0 < hi; i0 += XT) {
-      const unsigned i = i0 + tid;
-      uint32_t c = FB_INF, v = 0;
-      if (i < hi) {
-        c = __ldcg(&a.nc[i]); v = __ldcg(&a.deps[i]);
-        a.cobs[v] = c;
-        a.LS[v] = a.ls_deps + i;                               // InsertIntoList(new_obs_idx, obs_idx) (:333)
-      }
-      unsigned ctot;
-      const unsigned pos = x_block_scan(sh, (i < hi && c >= 2u) ? 1u : 0u, lane, wid, ctot);
-      if (i < hi && c >= 2u) a.E[0][run + pos] = v;            // `if (distance < infinity_) update_queue_.push` (:329-331)
-      run += ctot;
-    }
-    nE += sh.total;
-    x_gsync(&ctl->bar, bar_target);
-    X_LAP(13);
-  }
   bool big = nE > a.small_max;
 
   // generation 0: words.  Initial guess of the fixpoint: every entry pushes its snapshot code.
@@ -1154,7 +1223,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
   }
   if (gtid == 0) {
     ctl->gen_id = gen; ctl->wclock = wclock; ctl->tclock = tclock; ctl->sclock = sclock;
-    ctl->generations = generations; ctl->reseed_rounds = reseed_rounds; ctl->rounds = rounds_total; ctl->dense_rounds = dense_total; ctl->voxels_changed = changed_total;
+    ctl->generations = generations; ctl->rounds = rounds_total; ctl->dense_rounds = dense_total; ctl->voxels_changed = changed_total;
   }
 }
 
@@ -1186,14 +1255,16 @@ int fb_xrelax_blocks(int device) {
   int per_sm = 0, sms = 0;
   for (const void *k : {(const void *)k_x_relax<false>, (const void *)k_x_relax<true>})
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, XT, sizeof(XNb) * XW) != cudaSuccess || per_sm < 1) return -1;
+  for (const void *k : {(const void *)k_x_reseed<false>, (const void *)k_x_reseed<true>})
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, XT, 0) != cudaSuccess || per_sm < 1) return -1;
   if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return -1;
   return sms;                                                  // one CTA per SM: the barrier is cheapest with few arrivals
 }
 
-cudaError_t fb_xrelax_launch(FbExact *X, const FbGeom &g, uint32_t *cobs, unsigned nE0, const uint32_t *deps, unsigned ndep, uint32_t *ord, uint32_t *nc, uint8_t *nk,
+cudaError_t fb_xrelax_launch(FbExact *X, const FbGeom &g, uint32_t *cobs, const uint32_t *deps, unsigned ndep, uint32_t *ord, uint32_t *nc, uint32_t *M,
                              const uint32_t *occbits, unsigned long long ls_deps, unsigned long long *dbg, cudaStream_t s) {
   XArgs a;
-  a.deps = deps; a.ndep = ndep; a.ord = ord; a.nc = nc; a.nk = nk; a.occbits = occbits; a.ls_deps = ls_deps;
+  a.deps = deps; a.ndep = ndep; a.ord = ord; a.nc = nc; a.M = M; a.occbits = occbits; a.ls_deps = ls_deps;
   fb_div_make((unsigned)g.pz, a.div_pz_m, a.div_pz_s);
   fb_div_make((unsigned)g.gy, a.div_gy_m, a.div_gy_s);
   a.g = g;
@@ -1202,9 +1273,13 @@ cudaError_t fb_xrelax_launch(FbExact *X, const FbGeom &g, uint32_t *cobs, unsign
   a.cobs = cobs; a.MB = X->MB; a.LS = X->LS; a.SUM = X->SUM; a.SUMg = X->SUMg;
   a.E[0] = X->E[0]; a.E[1] = X->E[1]; a.emask = X->emask;
   for (int k = 0; k < 3; ++k) { a.W[k] = X->W[k]; a.F[k] = X->F[k]; }
-  a.wstamp = X->wstamp; a.slotc = X->slotc; a.ctl = X->d_ctl; a.nE0 = nE0; a.small_max = X->small_max; a.dense_min = X->dense_min; a.dbg = dbg;
+  a.wstamp = X->wstamp; a.slotc = X->slotc; a.ctl = X->d_ctl; a.small_max = X->small_max; a.dense_min = X->dense_min; a.dbg = dbg;
   a.async_on = X->async ? 1u : 0u;
   a.small_async_on = X->small_async ? 1u : 0u;
   void *args[] = {(void *)&a};
+  if (ndep) {
+    const cudaError_t e = cudaLaunchCooperativeKernel(dbg ? (void *)k_x_reseed<true> : (void *)k_x_reseed<false>, dim3(X->relax_blocks), dim3(XT), args, 0, s);
+    if (e != cudaSuccess) return e;
+  }
   return cudaLaunchCooperativeKernel(dbg ? (void *)k_x_relax<true> : (void *)k_x_relax<false>, dim3(X->relax_blocks), dim3(XT), args, sizeof(XNb) * XW, s);
 }

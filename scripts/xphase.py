@@ -4,8 +4,10 @@
 
 Runs frames 0 .. warmup+steps-1 of the workload in EXACT mode with FIESTA_DEBUG_X=1 (the kernel then times its phases with
 clock64; the library converts cycles with the device's SM clock) and sums, over the timed frames warmup .. warmup+steps-1:
-the time of every phase, the evaluation rounds, the work-list entries evaluated and refreshed, and the re-seeding list
-entries.  It also prints, per frame, the (nE, rounds) list of every generation.  The numbers of generations and every nE
+the time of every phase, the evaluation rounds and the work-list entries evaluated and refreshed.  The re-seeding of the
+dependants of deleted obstacles (k_x_reseed) is split into its stages: classify, closure, choose, resolve and the hand-over
+to generation 0 (assemble); per frame it prints the dependants, those final after the classification, the closure rounds,
+the closure list entries and the resolve passes.  It also prints, per frame, the (nE, rounds) list of every generation.  The numbers of generations and every nE
 are fixed by the sequential result; rounds and list lengths vary from run to run (a round reads words flipped in the same
 round).  For the evaluation-round categories it also splits the time into the summed longest CTA work time of every round
 and the rest (grid barrier plus waiting for the slowest CTA), with a log2 histogram of the list lengths of the short-list
@@ -24,7 +26,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PHASES = ["S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
-          "empty-barrier", "reseed.rounds", "reseed.assemble", "async", "refresh", "s.async"]
+          "empty-barrier", "reseed.classify", "reseed.closure", "reseed.choose", "reseed.resolve", "reseed.assemble", "async",
+          "refresh", "s.async"]
 ROUND_CATS = ["round1", "rounds", "dense", "s.round1", "s.rounds"]
 
 
@@ -91,7 +94,9 @@ def main():
     small_max = int(os.environ.get("FIESTA_X_SMALL", "32768"))
     small = {}                                                 # log2 bucket of nE -> [generations, rounds, us]
     us = {k: 0.0 for k in PHASES}
-    tot = dict(rounds=0, evaluated=0, refreshed=0, reseeded=0, reseed_rounds=0, generations=0, expansions=0)
+    tot = dict(rounds=0, evaluated=0, refreshed=0, reseed_rounds=0, dependants=0, final_after_classify=0, closure_rounds=0,
+               closure_entries=0, resolve_passes=0, generations=0, expansions=0)
+    reseed = {}                                                # frame -> (dependants, final, closure rounds, entries, passes)
     work = {k: [0.0, 0] for k in ROUND_CATS}
     hist = {"rounds": {}, "s.rounds": {}}
     aq = dict(evaluations=0, dirty=0, pushes=0, spin_us=0.0)
@@ -123,8 +128,13 @@ def main():
             aq["evaluations"] += int(mm.group(1)); aq["dirty"] += int(mm.group(2)); aq["pushes"] += int(mm.group(3))
             aq["spin_us"] += float(mm.group(4))
         elif line.startswith("[x] work-list entries:"):
-            mm = re.search(r"evaluated (\d+) refreshed (\d+) reseeded (\d+)", line)
-            tot["evaluated"] += int(mm.group(1)); tot["refreshed"] += int(mm.group(2)); tot["reseeded"] += int(mm.group(3))
+            mm = re.search(r"evaluated (\d+) refreshed (\d+)", line)
+            tot["evaluated"] += int(mm.group(1)); tot["refreshed"] += int(mm.group(2))
+        elif line.startswith("[x] reseed:"):
+            v = tuple(int(t) for t in re.findall(r"\d+", line))
+            reseed[f] = v
+            for k, n in zip(("dependants", "final_after_classify", "closure_rounds", "closure_entries", "resolve_passes"), v):
+                tot[k] += n
         elif line.startswith("[x] gens "):
             mm = re.match(r"\[x\] gens (\d+) rounds (\d+)", line)
             tot["generations"] += int(mm.group(1)); tot["rounds"] += int(mm.group(2))
@@ -158,8 +168,11 @@ def main():
         out.append("  b %2d: %6d gens %6.2f rounds %8.1f us" % (b, g, r / g, t / g))
     g, r, t = (sum(v[k] for v in small.values()) for k in range(3))
     out.append("  all : %6d gens %6.2f rounds %8.1f us (%.2f ms)" % (g, r / max(1, g), t / max(1, g), t / 1000.0))
-    for k in ("generations", "rounds", "evaluated", "refreshed", "reseed_rounds", "reseeded", "expansions"):
+    for k in ("generations", "rounds", "evaluated", "refreshed", "reseed_rounds", "dependants", "final_after_classify",
+              "closure_rounds", "closure_entries", "resolve_passes", "expansions"):
         out.append("total %s %d" % (k, tot[k]))
+    for fr in sorted(reseed):
+        out.append("frame %d reseed: dependants %d final after classify %d closure rounds %d list entries %d resolve passes %d" % ((fr,) + reseed[fr]))
     for fr in sorted(gens):
         out.append("frame %d nE %s" % (fr, " ".join(str(n) for n, _ in gens[fr])))
     for fr in sorted(gens):
