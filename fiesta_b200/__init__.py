@@ -74,6 +74,11 @@ class SkeletonStats(C.Structure):
         (n, C.c_float) for n in ("ms_compute", "ms_init", "ms_thin", "ms_graph")]
 
 
+class MeshStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("box_voxels", "blocking", "vertices", "quads", "triangles")] + [
+        (n, C.c_float) for n in ("ms_compute", "ms_classify", "ms_vertices", "ms_faces")]
+
+
 class SensorModel(C.Structure):
     _fields_ = [("max_range", C.c_double), ("tan_half_fov", C.c_double * 2)]
 
@@ -128,6 +133,7 @@ SYMBOLS = [
     "fiesta_signed_get_dist_grad_trilinear_batch_device",
     "fiesta_skeleton_create", "fiesta_skeleton_destroy", "fiesta_skeleton_compute", "fiesta_skeleton_vertices",
     "fiesta_skeleton_edges", "fiesta_skeleton_edge_voxels", "fiesta_skeleton_export",
+    "fiesta_mesh_create", "fiesta_mesh_destroy", "fiesta_mesh_compute", "fiesta_mesh_vertices", "fiesta_mesh_triangles",
 ]
 
 SEGMENT_UNKNOWN_BLOCKS = 1     # FIESTA_SEGMENT_UNKNOWN_BLOCKS
@@ -218,6 +224,12 @@ def load_library():
         L.fiesta_skeleton_edges.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 4
         L.fiesta_skeleton_edge_voxels.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
         L.fiesta_skeleton_export.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.fiesta_mesh_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+        L.fiesta_mesh_destroy.argtypes = [C.c_void_p]
+        L.fiesta_mesh_destroy.restype = None
+        L.fiesta_mesh_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p]
+        L.fiesta_mesh_vertices.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
+        L.fiesta_mesh_triangles.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
         L.fiesta_inflate_boxes.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 4
         L.fiesta_corridors.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_double, C.c_int] + [C.c_void_p] * 7
         L.fiesta_snapshot_save.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
@@ -646,6 +658,71 @@ class Skeleton:
             self._h = None
 
 
+class Mesh:
+    """fiesta_mesh: the triangle mesh of the boundary of what blocks at a clearance in a voxel box -- float32 vertices in metres
+    placed on the records' exact distances, int32 triangles with normals from blocking to free space, closed at the box faces.
+    The buffers grow to the largest box computed; close() it before the map."""
+
+    def __init__(self, m):
+        self._m = m
+        h = C.c_void_p()
+        m._ck(m._L.fiesta_mesh_create(m._h, C.byref(h)), "fiesta_mesh_create")
+        self._h = h
+        self.stats = None
+
+    def compute(self, box_lo, box_hi, clearance=0.0, unknown_blocks=False):
+        """Mesh of the inclusive voxel box [box_lo, box_hi] at the clearance (metres) -> stats dict."""
+        lo, hi = np.ascontiguousarray(box_lo, dtype=np.int32), np.ascontiguousarray(box_hi, dtype=np.int32)
+        if lo.shape != (3,) or hi.shape != (3,):
+            raise ValueError("Mesh.compute: box_lo and box_hi must be 3 voxel coordinates each")
+        st = MeshStats()
+        r, flags = _segment_flags(clearance, unknown_blocks)
+        rc = self._m._L.fiesta_mesh_compute(self._h, lo.ctypes, hi.ctypes, r, flags, C.byref(st))
+        if rc not in (0, 1):                                                # only FIESTA_ERR_INVALID keeps the last result
+            self.stats = None
+        self._m._ck(rc, "Mesh.compute")
+        self.stats = {n: getattr(st, n) for n, _ in st._fields_}
+        return dict(self.stats)
+
+    def _need(self, what):
+        if self.stats is None:
+            raise FiestaError("Mesh.%s: no mesh has been computed" % what)
+
+    def vertices(self, cap=None):
+        """The vertex positions (the first `cap`) as (V, 3) float32 metres."""
+        self._need("vertices")
+        n = self.stats["vertices"] if cap is None else min(int(cap), self.stats["vertices"])
+        out = np.empty((n, 3), np.float32)
+        self._m._ck(self._m._L.fiesta_mesh_vertices(self._h, C.c_int64(n), out.ctypes), "Mesh.vertices")
+        return out
+
+    def triangles(self, cap=None):
+        """The triangles (the first `cap`) as (T, 3) int32 vertex ids, counter-clockwise seen from free space."""
+        self._need("triangles")
+        n = self.stats["triangles"] if cap is None else min(int(cap), self.stats["triangles"])
+        out = np.empty((n, 3), np.int32)
+        self._m._ck(self._m._L.fiesta_mesh_triangles(self._h, C.c_int64(n), out.ctypes), "Mesh.triangles")
+        return out
+
+    def save_ply(self, path):
+        """Write the mesh as binary little-endian PLY (float x y z; list uchar int vertex_indices)."""
+        v, t = self.vertices(), self.triangles()
+        face = np.empty(len(t), dtype=[("n", "u1"), ("ijk", "<i4", (3,))])
+        face["n"] = 3
+        face["ijk"] = t
+        head = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
+                "element face %d\nproperty list uchar int vertex_indices\nend_header\n" % (len(v), len(t)))
+        with open(path, "wb") as f:
+            f.write(head.encode("ascii"))
+            f.write(v.astype("<f4").tobytes())
+            f.write(face.tobytes())
+
+    def close(self):
+        if self._h:
+            self._m._L.fiesta_mesh_destroy(self._h)
+            self._h = None
+
+
 class ESDFMap:
     """Mirror of fiesta::ESDFMap (ESDFMap.h:111-164); every method forwards 1:1 to the C ABI."""
 
@@ -938,6 +1015,10 @@ class ESDFMap:
     def Skeleton(self):
         """Topological skeleton of a box's free space as a graph of junctions and edges (fiesta_skeleton_*)."""
         return Skeleton(self)
+
+    def Mesh(self):
+        """Triangle mesh of the surface of what blocks at a clearance in a box (fiesta_mesh_*)."""
+        return Mesh(self)
 
     def RaycastFrame(self, xyz, T, min_ray_length, max_ray_length):
         """xyz: (n,3) float32 host array, or an integer device pointer paired with `n` as a tuple (ptr, n)."""

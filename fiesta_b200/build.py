@@ -7,8 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libfiesta_b200.so")
-SOURCES = ["fb_map.cu", "fb_esdf.cu", "fb_raycast.cu", "fb_exact.cu", "fb_xrelax.cu", "fb_vis.cu", "fb_depth.cu", "fb_segment.cu", "fb_nav.cu", "fb_navmatrix.cu", "fb_frontier.cu", "fb_view.cu", "fb_corridor.cu", "fb_pose.cu", "fb_snapshot.cu", "fb_signed.cu", "fb_skel.cu"]
-HEADERS = ["fb_common.cuh", "fb_map.h", "fb_nav.cuh", "fb_frontier.cuh", "fb_host.h", "fb_record.h", "fb_segment.h", "fb_nav.h", "fb_frontier.h", "fb_view.h", "fb_corridor.h", "fb_pose.h", "fb_snapshot.h", "fb_signed.h", "fb_skel.cuh", "fb_skel.h", "fb_exact.h", "fb_divmagic.h", os.path.join("..", "..", "include", "fiesta_b200.h")]
+SOURCES = ["fb_map.cu", "fb_esdf.cu", "fb_raycast.cu", "fb_exact.cu", "fb_xrelax.cu", "fb_vis.cu", "fb_depth.cu", "fb_segment.cu", "fb_nav.cu", "fb_navmatrix.cu", "fb_frontier.cu", "fb_view.cu", "fb_corridor.cu", "fb_pose.cu", "fb_snapshot.cu", "fb_signed.cu", "fb_skel.cu", "fb_mesh.cu"]
+HEADERS = ["fb_common.cuh", "fb_map.h", "fb_nav.cuh", "fb_frontier.cuh", "fb_host.h", "fb_record.h", "fb_segment.h", "fb_nav.h", "fb_frontier.h", "fb_view.h", "fb_corridor.h", "fb_pose.h", "fb_snapshot.h", "fb_signed.h", "fb_skel.cuh", "fb_skel.h", "fb_mesh.h", "fb_exact.h", "fb_divmagic.h", os.path.join("..", "..", "include", "fiesta_b200.h")]
 # -fmad=false: the ray-casting, query and occupancy code must round every fp64 operation exactly like the reference's
 # separate multiply and add (ESDFMap.cpp:122-123, 519-537; raycast.cpp:100-107).
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -568,6 +568,52 @@ int fiesta_skeleton_edges(const fiesta_skeleton *f, int64_t cap, int32_t *uv /* 
 int fiesta_skeleton_edge_voxels(const fiesta_skeleton *f, int64_t cap, int32_t *vox_xyz /* cap * 3 */);
 int fiesta_skeleton_export(const fiesta_skeleton *f, uint8_t *mask /* box_voxels, nullable */, int32_t *label /* box_voxels, nullable */);
 
+/* ---- surface meshes (viewers, simulators, other collision libraries: the map, or what the planners treat as blocked, as geometry) ----
+ * The triangle mesh of the boundary of the voxels that block at a clearance in an inclusive voxel box [box_lo, box_hi]
+ * (0 <= lo <= hi < grid size on every axis).  A snapshot of the integrated records at the time of the call; nothing in the map or in
+ * any other result changes.
+ *   blocking     a box voxel that blocks at the clearance and flags in the sense of fiesta_check_segments (GetDistance(Vector3i) <=
+ *                clearance; with FIESTA_SEGMENT_UNKNOWN_BLOCKS also a never-observed voxel).  Voxels outside the box never block, so
+ *                every mesh is closed and caps the box faces.
+ *   distance     a box voxel whose record holds an obstacle not under an EXACT local-map reset has d(v) = GetDistance(Vector3i).
+ *   E            the extended box [lo - 1, hi] on every axis, indexed ((x-lo.x+1)*(By+1) + (y-lo.y+1))*(Bz+1) + (z-lo.z+1).
+ *   crossing     on a grid edge (u, w = u + e_a) with exactly one blocking endpoint: t = (clearance - d(u)) / (d(w) - d(u)) in fp64
+ *                when both have a distance, else 0.5; the point u + t e_a (voxel units).
+ *   vertices     one per active cell c in E (its corners c + {0,1}^3 neither all block nor all fail to), numbered in E-index order:
+ *                the fp64 mean of the crossing points on its sign-changing edges (x-edges, then y-edges, then z-edges, each axis'
+ *                four ordered lexicographically by the other offsets), in metres as ((m + 0.5) * resolution) + origin, rounded to
+ *                float32.
+ *   triangles    one quad per sign-changing grid edge (v, v + e_a), v in E: with (a, b, c) cyclic, the cells v + (0,-1,-1),
+ *                v + (0,0,-1), v, v + (0,-1,0) (offsets along a, b, c) in that order when v blocks and reversed after the first
+ *                otherwise, so normals point from blocking to free space; split along p0-p2 when |p0-p2|^2 <= |p1-p3|^2 (fp64 on the
+ *                float32 positions) into (p0,p1,p2), (p0,p2,p3), else into (p1,p2,p3), (p1,p3,p0).  Written in order of (v's E-index,
+ *                axis x, y, z), two per quad, as int32 vertex ids.
+ * The mesh is closed (every directed edge meets its reverse) and combinatorially the boundary of the union of the blocking voxels'
+ * cubes; voxels touching only along an edge or a corner share vertices there.  Clearance 0 puts the surface through obstacle voxel
+ * centres, 0.5 * resolution on the obstacle cubes' faces.  A vertex depends only on its cell's 8 corners, so adjacent boxes agree bit
+ * for bit on the cells whose corners both boxes hold.  Every output is one fixed fp64 expression rounded once: the same bits on every
+ * run and as the sequential definition (tests/meshref.py; fiesta_b200/csrc/fb_mesh.h, DESIGN.md §3.15).  The reads write the first
+ * min(cap, n) entries (n = stats.vertices / triangles).  The object owns its device buffers, which grow to the largest box and
+ * result used: about 1 byte per extended-box position, plus 12 bytes per vertex and 12 per triangle, with the library's 50 % growth
+ * headroom.  It runs on the map's stream; the calls are synchronous.  Destroy it before the map.  Errors: FIESTA_ERR_INVALID for a
+ * box outside the grid or inverted, a clearance or flags fiesta_check_segments rejects, a null buffer with cap > 0, a negative cap,
+ * or reads before a compute; nothing is written then.  FIESTA_ERR_LIMIT when the mesh would have more than 2^31 - 1 vertices (only
+ * possible for boxes near the largest grid; mesh them in chunks).  FIESTA_ERR_CUDA when the buffers cannot be allocated.  After
+ * either of the last two a new compute is needed before the results can be read. */
+typedef struct fiesta_mesh fiesta_mesh;
+typedef struct fiesta_mesh_stats {
+  int64_t box_voxels, blocking;           /* voxels of the box, and those that block */
+  int64_t vertices, quads, triangles;     /* triangles = 2 * quads */
+  float ms_compute;                       /* device time of the compute, and of its three stages: */
+  float ms_classify, ms_vertices, ms_faces;   /* bitmap, cell and edge counts and their scans; vertices; triangles */
+} fiesta_mesh_stats;
+int fiesta_mesh_create(fiesta_map *m, fiesta_mesh **out);
+void fiesta_mesh_destroy(fiesta_mesh *f);
+int fiesta_mesh_compute(fiesta_mesh *f, const int box_lo[3], const int box_hi[3], double clearance, int flags,
+                        fiesta_mesh_stats *stats /* nullable */);
+int fiesta_mesh_vertices(const fiesta_mesh *f, int64_t cap, float *xyz /* cap * 3 */);
+int fiesta_mesh_triangles(const fiesta_mesh *f, int64_t cap, int32_t *ijk /* cap * 3 */);
+
 /* ---- safe flight corridors (corridor-based trajectory planners: free convex regions around a path) ----
  * Free axis-aligned voxel boxes, inflated face by face, and chains of them along paths in which consecutive boxes share a voxel.
  * All boxes are inclusive voxel boxes; the limit box L = [box_lo, box_hi] satisfies 0 <= lo <= hi < grid size on every axis.

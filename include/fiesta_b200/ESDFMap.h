@@ -298,6 +298,20 @@ class ESDFMap {
     check(fiesta_skeleton_edge_voxels(f, cap, vox_xyz), "SkeletonEdgeVoxels");
   }
   void ExportSkeleton(const fiesta_skeleton *f, uint8_t *mask, int32_t *label) { check(fiesta_skeleton_export(f, mask, label), "ExportSkeleton"); }
+  // Surface meshes (fiesta_mesh_* in fiesta_b200.h): the triangle mesh of the boundary of what blocks at a clearance in a box, float32
+  // vertices in metres and int32 triangles.  Destroy with fiesta_mesh_destroy before the map.
+  fiesta_mesh *MakeMesh() {
+    fiesta_mesh *f = nullptr;
+    check(fiesta_mesh_create(h_, &f), "MakeMesh");
+    return f;
+  }
+  fiesta_mesh_stats ComputeMesh(fiesta_mesh *f, const int box_lo[3], const int box_hi[3], double clearance, int flags) {
+    fiesta_mesh_stats st = {};
+    check(fiesta_mesh_compute(f, box_lo, box_hi, clearance, flags, &st), "ComputeMesh");
+    return st;
+  }
+  void MeshVertices(const fiesta_mesh *f, long cap, float *xyz) { check(fiesta_mesh_vertices(f, cap, xyz), "MeshVertices"); }
+  void MeshTriangles(const fiesta_mesh *f, long cap, int32_t *ijk) { check(fiesta_mesh_triangles(f, cap, ijk), "MeshTriangles"); }
   // Safe flight corridors (fiesta_inflate_boxes / fiesta_corridors in fiesta_b200.h): free axis-aligned voxel boxes in a limit box,
   // and chains of them along paths in which consecutive boxes share a voxel.
   fiesta_corridor_stats InflateBoxes(const int box_lo[3], const int box_hi[3], const int32_t *seed_lo_xyz, const int32_t *seed_hi_xyz,
