@@ -150,8 +150,6 @@ int fb_exact_init(FbExact *X, const FbGeom &g, int device, cudaStream_t s) {
   for (int k = 0; k < 2; ++k) CK(X->E[k].alloc(P));
   X->dense_min = 16384u;
   if (const char *e = getenv("FIESTA_X_DENSE")) { long v = atol(e); if (v >= 0 && v <= (1 << 24)) X->dense_min = (unsigned)v; }
-  if (const char *e = getenv("FIESTA_X_ASYNC")) X->async = atol(e) != 0;                  // 0: no work queue anywhere
-  if (const char *e = getenv("FIESTA_X_SMALL_ASYNC")) X->small_async = atol(e) != 0;      // 1: SMALL generations from the queue
   X->small_max = FB_X_SMALL_DEFAULT;
   if (const char *e = getenv("FIESTA_X_SMALL")) { long v = atol(e); if (v >= 0 && v <= 65536) X->small_max = (unsigned)v; }
   CK(X->slotc.alloc(((size_t)X->small_max + 1) * 32));
@@ -326,22 +324,20 @@ int fb_exact_update_esdf(FbExact *X, const FbGeom &g, uint32_t *cobs, uint32_t *
       static double cyc_per_us = 0;                            // clock64 counts SM cycles: convert with this device's SM clock
       if (cyc_per_us == 0) { int dev = 0, khz = 0; CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev)); cyc_per_us = khz / 1000.0; }
       CK(cudaMemcpy(hd, X->d_dbg, sizeof(hd), cudaMemcpyDeviceToHost));
-      // phase categories of k_x_reseed and k_x_relax (14 and 15 are counters, printed below)
-      static const char *cat[FB_XDBG_NCAT] = {"S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
-                                              "empty-barrier", "reseed.classify", "reseed.assemble", "", "", "async", "", "refresh", "s.async",
+      // phase categories of k_x_reseed and k_x_relax (14 and 15 are counters, printed below; 2 and 19 are retired)
+      static const char *cat[FB_XDBG_NCAT] = {"S", "round1", "", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
+                                              "empty-barrier", "reseed.classify", "reseed.assemble", "", "", "async", "", "refresh", "",
                                               "reseed.closure", "reseed.choose", "reseed.resolve", ""};
       fprintf(stderr, "[x] reseed rounds %u; phases (us, count):", st->reseed_rounds);
       for (int c = 0; c < FB_XDBG_NCAT; ++c)
         if (*cat[c]) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[FB_XDBG_PHASE + 2 * c] / cyc_per_us, hd[FB_XDBG_PHASE + 2 * c + 1]);
       fprintf(stderr, "\n");
       fprintf(stderr, "[x] round work (summed longest CTA work time us / summed list length):");
-      for (int c : {1, 2, 3, 6, 7}) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[FB_XDBG_WORK + 2 * c] / cyc_per_us, hd[FB_XDBG_WORK + 2 * c + 1]);
+      for (int c : {1, 3, 6, 7}) fprintf(stderr, " %s %.0f/%llu", cat[c], hd[FB_XDBG_WORK + 2 * c] / cyc_per_us, hd[FB_XDBG_WORK + 2 * c + 1]);
       fprintf(stderr, "\n");
-      for (int h = 0; h < 2; ++h) {
-        fprintf(stderr, "[x] list-length histogram %s (log2 bucket=rounds):", h ? "s.rounds" : "rounds");
-        for (int b = 0; b < 32; ++b) if (hd[FB_XDBG_NWH + 32 * h + b]) fprintf(stderr, " %d=%llu", b, hd[FB_XDBG_NWH + 32 * h + b]);
-        fprintf(stderr, "\n");
-      }
+      fprintf(stderr, "[x] list-length histogram s.rounds (log2 bucket=rounds):");
+      for (int b = 0; b < 32; ++b) if (hd[FB_XDBG_NWH + 32 + b]) fprintf(stderr, " %d=%llu", b, hd[FB_XDBG_NWH + 32 + b]);
+      fprintf(stderr, "\n");
       fprintf(stderr, "[x] async: evaluations %llu dirty %llu pushes %llu spin %.0f us\n", hd[FB_XDBG_Q + 0], hd[FB_XDBG_Q + 1], hd[FB_XDBG_Q + 2],
               hd[FB_XDBG_Q + 3] / cyc_per_us);
       for (int gq = 0; gq < 2; ++gq) { fprintf(stderr, "[x] gen %d work lists:", gq); for (int r = 0; r < 512 && hd[FB_XDBG_ROUNDS + gq * 512 + r]; ++r) fprintf(stderr, " %llu", hd[FB_XDBG_ROUNDS + gq * 512 + r]); fprintf(stderr, "\n"); }

@@ -10,8 +10,9 @@
 // the counts of 20 and 22 are the closure rounds and the resolve passes; 15 holds the dependants final after the
 // classification and the summed closure list lengths instead); 2 x 512 work-list sizes per round (first two generations);
 // 4096 per-round slots for the longest CTA work time of the round (cycles, reset once added up); FB_XDBG_NCAT x {summed longest CTA work time, summed list
-// length} per round category; 2 x 32 log2 histograms of the list lengths of BIG short-list rounds and SMALL later rounds;
-// FB_XDBG_NQ counters of the asynchronous schedule.
+// length} per round category; 2 x 32 log2 histograms of the list lengths of later rounds (the first retired, the second
+// SMALL generations'); FB_XDBG_NQ counters of the asynchronous schedule.  Categories 2 and 19 are retired (BIG short-list
+// rounds, SMALL generations from the work queue); their slots stay so that the offsets do not move.
 #define FB_XDBG_GENS 1024
 #define FB_XDBG_NCAT 24
 #define FB_XDBG_NQ 8
@@ -69,8 +70,6 @@ struct FbExact {
   FbDevBuf<uint32_t> slotc;           // SMALL generations: codes of the owned slots
   unsigned dense_min = 0;             // work lists longer than this are evaluated through refreshed summaries (one wave of warps)
   unsigned small_max = 0;             // generations up to this many entries run without summaries
-  bool async = true;                  // short work lists resolved from a work queue instead of in rounds (FIESTA_X_ASYNC=0: rounds)
-  bool small_async = false;           // SMALL generations resolved from the queue, seeded with every element (FIESTA_X_SMALL_ASYNC=1)
   FbDevBuf<FbXCtl> d_ctl;
   FbHostBuf<FbXCtl> h_ctl;
   FbDevBuf<unsigned long long> d_dbg;

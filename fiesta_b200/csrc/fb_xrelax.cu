@@ -14,13 +14,12 @@
 //  * An element's behaviour (stale / pulled code / pushes code, :345-373) depends only on states at its own pop time, i.e.
 //    on the words at the 129 offsets a+b (a,b in {0} u dirs_) around it.  Round 1 evaluates every element against the guess
 //    "everybody pushes its snapshot code"; a flip lists every LATER element it can touch for the next round (all 129 offsets
-//    if pushing is involved, else only the 24 neighbours: just the offer to its own voxel changed).  Short lists are evaluated
-//    from a per-warp shared-memory stage filled by one round of loads (x_stage) while last round's flips refresh the
-//    summaries of their targets; long lists first refresh, then evaluate through the summaries.  Element i is right once all
+//    if pushing is involved, else only the 24 neighbours: just the offer to its own voxel changed).  SMALL generations
+//    evaluate from a per-warp shared-memory stage filled by one round of loads (x_stage); the later rounds of BIG
+//    generations first refresh the summaries of last round's flips' targets, then evaluate through them.  Element i is right once all
 //    earlier ones are, so the fixpoint -- reached by a round without flips, which has only read final words -- is the
 //    sequential execution.  In BIG generations, once a list is short, the rest of the fixpoint runs without rounds from a
-//    work queue (x_async), followed by one summary refresh.  With FIESTA_X_SMALL_ASYNC=1, SMALL generations seed that
-//    queue with every element and run no rounds at all (slower on the measured workloads, DESIGN §6, so off by default).
+//    work queue (x_async), followed by one summary refresh.
 //  * Hand-over: element i owns slot k iff the final state of its k-th target carries the timestamp 32*i + k; the owned slots in
 //    timestamp order (per-element masks, exclusive scan over CTA-contiguous ranges) are the next generation; old words are
 //    retired by compare-and-swap (a generation-parity bit tells old from new).
@@ -57,16 +56,17 @@ static __constant__ int x_off_c[X_NOFF];     // the distinct sums a+b, packed (d
 
 // Index arithmetic was a third of this kernel's instruction stream (ncu source view): 64-bit linear
 // indices, six-compare box tests and divisions by the run-time pitch.  The forms below are exact for every grid the library
-// accepts (< 2^30 voxels): 32-bit indices, unsigned range tests, multiply-high divisions with host-made constants.
+// accepts (< 2^30 voxels): 32-bit indices, unsigned grid tests, multiply-high divisions with host-made constants.
 __device__ __forceinline__ unsigned x_vi(const FbGeom &g, int x, int y, int z) { return (unsigned)((x * g.gy + y) * g.pz + z); }
 __device__ __forceinline__ bool x_in_grid(const FbGeom &g, int x, int y, int z) {
   return (unsigned)x < (unsigned)g.gx && (unsigned)y < (unsigned)g.gy && (unsigned)z < (unsigned)g.gz;
 }
 // VoxInRange (ESDFMap.cpp:63-72); fb_xrelax_launch makes min_vec / max_vec of the kernel's copy an unreachable box when the
-// update box is empty, so max - min >= 0 here
+// update box is empty.  Compared with the bounds as they are, which stay kernel parameters: the extents max - min of an
+// unsigned test are loop-invariant values that the compiler keeps in registers, and at k_x_relax's 64-register limit they
+// spill inside the per-element loops.
 __device__ __forceinline__ bool x_in_range(const FbGeom &g, int x, int y, int z) {
-  return (unsigned)(x - g.min_vec[0]) <= (unsigned)(g.max_vec[0] - g.min_vec[0]) && (unsigned)(y - g.min_vec[1]) <= (unsigned)(g.max_vec[1] - g.min_vec[1]) &&
-         (unsigned)(z - g.min_vec[2]) <= (unsigned)(g.max_vec[2] - g.min_vec[2]);
+  return x >= g.min_vec[0] && x <= g.max_vec[0] && y >= g.min_vec[1] && y <= g.max_vec[1] && z >= g.min_vec[2] && z <= g.max_vec[2];
 }
 // dirs_[j][k] for a compile-time j (unrolled loops): folded into immediates, unlike a read of the constant-memory table
 __device__ __forceinline__ int x_dc(int j, int k) {
@@ -90,6 +90,11 @@ struct XShared {
   unsigned char self[32];             // index in off[] of target t itself (entry 24 = 0)
   unsigned red[XW], red2[XW];
   unsigned base, total;
+  // thread 0's alone: the grid barrier's arrival target and k_x_relax's totals.  They stay live across the whole generation
+  // loop, which runs at the 64-register limit, so they are kept here rather than in registers that would spill.
+  unsigned bar_target;
+  unsigned generations, rounds, dense_rounds;
+  unsigned long long changed;
   unsigned qdone;                     // the work queue of the current asynchronous phase is done (copy of ctl->qdone)
 };
 
@@ -221,8 +226,6 @@ struct XArgs {
   unsigned long long ls_deps;   // link time of dependant 0 (InsertIntoList order, :333)
   unsigned long long *dbg;  // optional per-generation trace {nE, rounds, ns} (FIESTA_DEBUG_X)
   unsigned div_pz_m, div_pz_s, div_gy_m, div_gy_s;   // n / d = umulhi(n, m) >> s for n < 2^31 (fb_div_make, fb_divmagic.h); m == 0: d == 1
-  unsigned async_on;        // resolve short work lists from the work queue (x_async) instead of in rounds
-  unsigned small_async_on;  // SMALL generations: the whole fixpoint from the work queue, seeded with every element
 };
 // voxel index -> coordinates: two divisions by run-time constants, as multiply-high + shift
 __device__ __forceinline__ unsigned x_div(unsigned n, unsigned m, unsigned s) { return m ? (__umulhi(n, m) >> s) : n; }
@@ -601,30 +604,25 @@ __device__ __forceinline__ unsigned x_q_list(const XArgs &a, XShared &sh, const 
   for (int t = 0; t < 5; ++t) if ((pm >> t) & 1u) x_q_put(a, sh, ring, cap, base++, j[t]);
   return total;
 }
-// One element of an asynchronous phase, taken from the queue (RUNNING set here) or claimed by its owner (`claimed`: RUNNING
-// and fenced already): evaluated from its stage, its word stored on a flip (BIG: and recorded in F[fout]) and the later
-// elements it can touch listed; evaluated again while a lister marked it dirty meanwhile.
-template <bool BIG, bool DBG>
+// One element of an asynchronous phase, taken from the queue: evaluated from its stage, its word stored on a flip and
+// recorded in F[fout], and the later elements it can touch listed; evaluated again while a lister marked it dirty meanwhile.
+template <bool DBG>
 __device__ __forceinline__ void x_q_run(const XArgs &a, XShared &sh, XNb &stg, unsigned lane, const uint32_t *E, unsigned nE, uint32_t *ring,
-                                        unsigned gen, unsigned A, unsigned fout, unsigned i, bool claimed) {
+                                        unsigned gen, unsigned A, unsigned fout, unsigned i) {
   const uint32_t p = __ldcg(&E[i]);
   int x, y, z; x_coords(a, p, x, y, z);
-  for (;; claimed = false) {
+  for (;;) {
     if (DBG && lane == 0) atomicAdd(&a.dbg[FB_XDBG_Q + 0], 1ull);
-    if (!claimed) {
-      if (lane == 0) atomicExch(&a.wstamp[i], A);              // RUNNING (from MARKED: queued, or dirty)
-      __syncwarp();
-      __threadfence();
-    }
+    if (lane == 0) atomicExch(&a.wstamp[i], A);                // RUNNING (from MARKED: queued, or dirty)
+    __syncwarp();
+    __threadfence();
     x_stage(a, sh, stg, lane, x, y, z);
     const unsigned long long old = stg.w[0], nw2 = x_eval_nb(a, sh, stg, lane, gen, i, x, y, z);
     if (nw2 != old) {                                          // flip
       if (lane == 0) {
         a.MB[p] = nw2;
-        if (BIG) {
-          const unsigned f = atomicAdd(&a.ctl->nF[fout], 1u);
-          if (f < (unsigned)a.g.ptotal) a.F[fout][f] = i;
-        }
+        const unsigned f = atomicAdd(&a.ctl->nF[fout], 1u);
+        if (f < (unsigned)a.g.ptotal) a.F[fout][f] = i;
       }
       __syncwarp();
       __threadfence();
@@ -662,45 +660,10 @@ __device__ void x_async(const XArgs &a, XShared &sh, XNb &stg, unsigned lane, un
     if (lane == 0) i = x_q_take<DBG>(a, sh, ring, nE, h);
     i = __shfl_sync(0xffffffffu, i, 0);
     if (i == XNONE) break;
-    x_q_run<true, DBG>(a, sh, stg, lane, E, nE, ring, gen, A, fout, i, false);
+    x_q_run<DBG>(a, sh, stg, lane, E, nE, ring, gen, A, fout, i);
     if (lane == 0) x_q_count(a, sh, 0ull - (1ull << 32));
   }
 }
-// The asynchronous phase of one SMALL generation (FIESTA_X_SMALL_ASYNC=1): its whole behaviour fixpoint, seeded with every
-// element; no summaries, so nothing is recorded for a refresh (the commit re-stages the final words).  A seed's first
-// evaluation is round 1's, so seeds do not go through the ring: warp w takes the elements w, w + nwk, ... itself, 32 at a
-// time, IDLE -> RUNNING with one atomicMax each and one fence for the 32 (an element a lister marked first is already
-// queued and skipped here), and evaluates them in order under its seeding token, as if it had pushed and popped them.
-// Only the first nwk = min(warps, nE) warps take part (at most nE elements are ever queued): warp 0 drops the other
-// warps' tokens at once, and those warps leave, so a short generation does not pay for every warp's token and pop.
-template <bool DBG>
-__device__ void x_async_small(const XArgs &a, XShared &sh, XNb &stg, unsigned lane, unsigned gwarp, unsigned gwarps, const uint32_t *E, unsigned nE,
-                              uint32_t *ring, unsigned gen, unsigned A) {
-  const unsigned nwk = min(gwarps, nE);
-  if (gwarp >= nwk) return;
-  if (gwarp == 0u && lane == 0 && nwk < gwarps) x_q_count(a, sh, 0ull - ((unsigned long long)(gwarps - nwk) << 32));   // warp 0's own token stays
-  for (unsigned s0 = gwarp; s0 < nE; s0 += 32u * nwk) {
-    const unsigned e = s0 + lane * nwk;
-    unsigned om = __ballot_sync(0xffffffffu, e < nE && atomicMax(&a.wstamp[e], A) < A);   // IDLE -> RUNNING, else queued by a lister
-    __threadfence();                                           // RUNNING before any of their stages
-    while (om) {
-      const unsigned i = s0 + (unsigned)(__ffs(om) - 1) * nwk;
-      om &= om - 1u;
-      x_q_run<false, DBG>(a, sh, stg, lane, E, nE, ring, gen, A, 0u, i, true);
-    }
-  }
-  if (lane == 0) x_q_count(a, sh, 0ull - (1ull << 32));
-  unsigned h = XNONE;
-  for (;;) {
-    unsigned i = 0;
-    if (lane == 0) i = x_q_take<DBG>(a, sh, ring, nE, h);
-    i = __shfl_sync(0xffffffffu, i, 0);
-    if (i == XNONE) break;
-    x_q_run<false, DBG>(a, sh, stg, lane, E, nE, ring, gen, A, 0u, i, false);
-    if (lane == 0) x_q_count(a, sh, 0ull - (1ull << 32));
-  }
-}
-
 extern __shared__ __align__(16) unsigned char x_dyn_smem[];
 
 // ---- E2, second half: re-seeding of the dependants of the deleted obstacles (:301-334) ----------------------------------
@@ -957,7 +920,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
   const unsigned gwarp = gtid >> 5, gwarps = gthreads >> 5;
   for (unsigned k = tid; k < X_NOFF; k += XT) sh.off[k] = x_off_c[k];
   if (tid < 32) sh.self[tid] = 0;
-  if (tid == 0) sh.qdone = 0u;
+  if (tid == 0) { sh.qdone = 0u; sh.bar_target = 0u; }
   if (gtid == 0) a.ctl->qtail = (unsigned long long)gwarps << 32;   // one seeding token per warp (x_async)
   if (tid < 32) sh.dir[tid] = tid < 24 ? ((x_dirs[tid][0] + 4) | ((x_dirs[tid][1] + 4) << 4) | ((x_dirs[tid][2] + 4) << 8)) : (4 | (4 << 4) | (4 << 8));
   __syncthreads();
@@ -974,15 +937,14 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
   XNb &stg = reinterpret_cast<XNb *>(x_dyn_smem)[wid];
 
   // grid-uniform state (every CTA computes the same values)
-  unsigned nE = ctl->nE0, bar_target = 0;
+  unsigned nE = ctl->nE0;
   int cur = 0;
   unsigned gen = ctl->gen_id, wclock = ctl->wclock;
   unsigned long long tclock = ctl->tclock;
-  unsigned generations = 0, rounds_total = 0, dense_total = 0;
-  unsigned long long changed_total = 0;
+  if (tid == 0) { sh.generations = 0; sh.rounds = 0; sh.dense_rounds = 0; sh.changed = 0; }
   if (DBG) {                                                 // cost of an empty grid barrier
     const long long t0 = clock64();
-    for (int q = 0; q < 32; ++q) x_gsync(&ctl->bar, bar_target);
+    for (int q = 0; q < 32; ++q) x_gsync(&ctl->bar, sh.bar_target);
     if (gtid == 0) a.dbg[XDBG_PHASE + 2 * 11] = (unsigned long long)(clock64() - t0) / 32ull;
   }
   long long t_ph = DBG ? clock64() : 0;
@@ -998,12 +960,12 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
     const uint32_t v = __ldcg(&a.E[0][i]);
     a.MB[v] = x_mb(gen, i, X_PUSH, __ldcg(&a.cobs[v]) & FB_CODE_MASK);
   }
-  x_gsync(&ctl->bar, bar_target);
+  x_gsync(&ctl->bar, sh.bar_target);
 
   while (nE) {
     const long long t_gen = DBG ? clock64() : 0;
     X_LAP(10);
-    ++generations;
+    if (tid == 0) ++sh.generations;
     const uint32_t *E = a.E[cur];
     // ---- behaviour fixpoint
     unsigned rounds = 0;
@@ -1011,7 +973,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
     if (big) {
       ++sclock;
       for (unsigned i = gwarp; i < nE; i += gwarps) { int x, y, z; x_coords(a, __ldcg(&E[i]), x, y, z); x_claim_summaries(a, sh, lane, x, y, z, sclock); }
-      x_gsync(&ctl->bar, bar_target);
+      x_gsync(&ctl->bar, sh.bar_target);
       X_LAP(0);
     }
     for (unsigned r = 1;; ++r) {
@@ -1022,23 +984,19 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       if (r > 1u && nw == 0u && nf == 0u) break;
       if (r > X_MAX_ROUNDS) { if (gtid == 0) ctl->err = 2u; break; }   // cannot happen (element i is final after i+1 rounds at the latest); never spin forever on the GPU
       if (DBG && gtid == 0) { a.dbg[XDBG_PHASE + 2 * 14] += nw; a.dbg[XDBG_PHASE + 2 * 14 + 1] += nf; }
-      if (a.async_on && (big ? r > 1u && nw <= a.dense_min : r == 1u && a.small_async_on)) {
-        // BIG: the rest of the fixpoint from the work queue, with W[out] as its ring; then the summaries of the targets of
-        // every flip since the last refresh: last round's (F[in]) and the queue's (F[out]).  A summary's offer timestamps
-        // 32*i+k are fixed, so the refresh rule needs only the final word and the summary's first / best, however often the
-        // element flipped in between.  SMALL: the whole fixpoint from the queue, seeded with every element instead of round
-        // 1 (the words start as "everybody pushes its snapshot code", as for round 1); no summaries, so no refresh: the
-        // commit follows the barrier, and the queue's reset below happens in the commit phase, behind the commit's barrier.
+      if (big && r > 1u && nw <= a.dense_min) {
+        // the rest of the fixpoint from the work queue, with W[out] as its ring; then the summaries of the targets of every
+        // flip since the last refresh: last round's (F[in]) and the queue's (F[out]).  A summary's offer timestamps 32*i+k
+        // are fixed, so the refresh rule needs only the final word and the summary's first / best, however often the element
+        // flipped in between.
         ++rounds; wclock += 3u;
         const unsigned A = wclock - 1u;                        // RUNNING; MARKED = wclock; the stamps of the next rounds are above
-        if (big) x_async<DBG>(a, sh, stg, lane, gwarp, gwarps, E, nE, a.W[in], nw, a.W[out], gen, A, out);
-        else x_async_small<DBG>(a, sh, stg, lane, gwarp, gwarps, E, nE, a.W[out], gen, A);
-        x_gsync(&ctl->bar, bar_target);
-        X_LAP(big ? 16 : 19);
+        x_async<DBG>(a, sh, stg, lane, gwarp, gwarps, E, nE, a.W[in], nw, a.W[out], gen, A, out);
+        x_gsync(&ctl->bar, sh.bar_target);
+        X_LAP(16);
         if (tid == 0) sh.qdone = 0u;
         if (gtid == 0) { ctl->qtail = (unsigned long long)gwarps << 32; ctl->qhead = 0u; ctl->qdone = 0u; }
         if (__ldcg(&ctl->err)) { aborted = true; break; }
-        if (!big) break;
         const unsigned nfa = __ldcg(&ctl->nF[out]);
         if (nfa > (unsigned)g.ptotal) {                        // flip list overflowed: summarise every target again
           ++sclock;
@@ -1051,14 +1009,14 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
             x_refresh_summaries(a, sh, lane, i, p, x, y, z);
           }
         }
-        x_gsync(&ctl->bar, bar_target);
+        x_gsync(&ctl->bar, sh.bar_target);
         X_LAP(18);
         break;
       }
       ++rounds; ++wclock;
-      const bool dense = big && r > 1u && nw > a.dense_min;   // more than one wave of warps: evaluate through the summaries
+      const bool dense = big && r > 1u;                        // (shorter lists went to the queue): through the summaries
       if (dense) {                                             // bring the summaries up to date first, then evaluate through them
-        ++dense_total;
+        if (tid == 0) ++sh.dense_rounds;
         if (nf < nE / 4u) {                                    // few flips: only the targets of last round's flips
           for (unsigned q = gwarp; q < nf; q += gwarps) {
             const unsigned i = __ldcg(&a.F[in][q]);
@@ -1070,31 +1028,19 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
           ++sclock;
           for (unsigned i = gwarp; i < nE; i += gwarps) { int x, y, z; x_coords(a, __ldcg(&E[i]), x, y, z); x_claim_summaries(a, sh, lane, x, y, z, sclock); }
         }
-        x_gsync(&ctl->bar, bar_target);
+        x_gsync(&ctl->bar, sh.bar_target);
       }
-      const bool use_sum = big && (r == 1u || dense);
-      const unsigned nref = (big && !dense) ? nf : 0u;
       const uint32_t *wl = a.W[in];
       const long long t_w0 = DBG ? clock64() : 0;
-      for (unsigned q = gwarp; q < nw + nref; q += gwarps) {
-        if (q >= nw) {                                         // summaries of the targets of an element that flipped last round
-          const unsigned i = __ldcg(&a.F[in][q - nw]);
-          const uint32_t p = __ldcg(&E[i]);
-          int x, y, z; x_coords(a, p, x, y, z);
-          x_refresh_summaries(a, sh, lane, i, p, x, y, z);
-          continue;
-        }
+      for (unsigned q = gwarp; q < nw; q += gwarps) {
         const unsigned i = r == 1u ? q : __ldcg(&wl[q]);
         const uint32_t p = __ldcg(&E[i]);
         int x, y, z; x_coords(a, p, x, y, z);
-        if (!use_sum) {                                        // gathering evaluation: everything from one staged round of loads
+        if (!big) {                                            // gathering evaluation: everything from one staged round of loads
           x_stage(a, sh, stg, lane, x, y, z);
           const unsigned long long old = stg.w[0], nw2 = x_eval_nb(a, sh, stg, lane, gen, i, x, y, z);
           if (nw2 == old) continue;
-          if (lane == 0) {                                     // flip
-            a.MB[p] = nw2;
-            if (big) a.F[out][atomicAdd(&ctl->nF[out], 1u)] = i;
-          }
+          if (lane == 0) a.MB[p] = nw2;                        // flip
           x_list_affected_nb(a, stg, lane, i, (x_mb_kind(old) == X_PUSH || x_mb_kind(nw2) == X_PUSH) ? (unsigned)X_NOFF : 25u, wclock, out);
           continue;
         }
@@ -1105,27 +1051,27 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
         if (nb == old) continue;
         if (lane == 0) {                                       // flip
           a.MB[p] = nb;
-          if (big) a.F[out][atomicAdd(&ctl->nF[out], 1u)] = i;
+          a.F[out][atomicAdd(&ctl->nF[out], 1u)] = i;
         }
         // later elements whose inputs this element can touch: a pushing element offers to its 24 neighbours, which the elements
         // within the 129 offsets a+b read; a flip between "stale" and "pulls" (or of the pulled code) only changes the
         // element's offer to its own voxel, which only its 24 neighbours read (the table starts with 0 and dirs_)
         x_list_affected(a, sh, lane, i, x, y, z, (x_mb_kind(old) == X_PUSH || x_mb_kind(nb) == X_PUSH) ? (unsigned)X_NOFF : 25u, wclock, out);
       }
-      if (DBG) { __syncthreads(); if (tid == 0) atomicMax(&a.dbg[XDBG_WMAX + ((rounds_total + rounds) & 4095u)], (unsigned long long)(clock64() - t_w0)); }
-      x_gsync(&ctl->bar, bar_target);
-      X_LAP(big ? (r == 1u ? 1 : (dense ? 3 : 2)) : (r == 1u ? 6 : 7));
+      if (DBG) { __syncthreads(); if (tid == 0) atomicMax(&a.dbg[XDBG_WMAX + ((sh.rounds + rounds) & 4095u)], (unsigned long long)(clock64() - t_w0)); }
+      x_gsync(&ctl->bar, sh.bar_target);
+      X_LAP(big ? (r == 1u ? 1 : 3) : (r == 1u ? 6 : 7));
       if (DBG && gtid == 0) {
-        if (generations <= 2u && rounds <= 512u) a.dbg[XDBG_ROUNDS + (generations - 1u) * 512u + (rounds - 1u)] = nw;
+        if (sh.generations <= 2u && rounds <= 512u) a.dbg[XDBG_ROUNDS + (sh.generations - 1u) * 512u + (rounds - 1u)] = nw;
         // the round's longest CTA work time and list length, summed per category: the rest of the category's time is barrier
         // and waiting for the slowest CTA
-        const unsigned cat = big ? (r == 1u ? 1u : (dense ? 3u : 2u)) : (r == 1u ? 6u : 7u);
-        unsigned long long *wm = &a.dbg[XDBG_WMAX + ((rounds_total + rounds) & 4095u)];
+        const unsigned cat = big ? (r == 1u ? 1u : 3u) : (r == 1u ? 6u : 7u);
+        unsigned long long *wm = &a.dbg[XDBG_WMAX + ((sh.rounds + rounds) & 4095u)];
         a.dbg[FB_XDBG_WORK + 2 * cat] += __ldcg(wm); a.dbg[FB_XDBG_WORK + 2 * cat + 1] += nw; *wm = 0;
-        if (cat == 2u || cat == 7u) a.dbg[FB_XDBG_NWH + (cat == 7u ? 32u : 0u) + (nw ? 32u - __clz(nw) : 0u)] += 1ull;
+        if (cat == 7u) a.dbg[FB_XDBG_NWH + 32u + (nw ? 32u - __clz(nw) : 0u)] += 1ull;
       }
     }
-    rounds_total += rounds;
+    if (tid == 0) sh.rounds += rounds;
     if (rounds > X_MAX_ROUNDS || aborted) break;
 
     // ---- commit: per-element masks of owned slots, winner counts per CTA (CTA-contiguous ranges keep the order)
@@ -1167,7 +1113,7 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       if (lane == 0) { ctl->partial[b] = c; if (l) atomicAdd(&ctl->expansions, (unsigned long long)l); }   // `times++` (:347)
     }
     if (gtid == 0) { ctl->nW[0] = ctl->nW[1] = ctl->nW[2] = 0; ctl->nF[0] = ctl->nF[1] = ctl->nF[2] = 0; }
-    x_gsync(&ctl->bar, bar_target);
+    x_gsync(&ctl->bar, sh.bar_target);
     X_LAP(big ? 4 : 8);
 
     // ---- apply: exclusive scan of the counts -> queue positions of the next generation; words + targets of the new entries
@@ -1212,18 +1158,18 @@ __global__ void __launch_bounds__(XT, 1) k_x_relax(const XArgs a) {
       }
       run += ctot;
     }
-    if (DBG && gtid == 0 && generations <= FB_XDBG_GENS) { a.dbg[3 * (generations - 1u)] = nE; a.dbg[3 * (generations - 1u) + 1] = rounds; a.dbg[3 * (generations - 1u) + 2] = (unsigned long long)(clock64() - t_gen); }
+    if (DBG && gtid == 0 && sh.generations <= FB_XDBG_GENS) { a.dbg[3 * (sh.generations - 1u)] = nE; a.dbg[3 * (sh.generations - 1u) + 1] = rounds; a.dbg[3 * (sh.generations - 1u) + 2] = (unsigned long long)(clock64() - t_gen); }
     tclock += (unsigned long long)nE * 32ull + 1ull;
-    changed_total += n2;
+    if (tid == 0) sh.changed += n2;
     if (n2 >= (1u << 27)) { if (gtid == 0) ctl->err = 1u; break; }
     const bool was_big = big;
     nE = n2; cur ^= 1; big = big2; ++gen;
-    x_gsync(&ctl->bar, bar_target);
+    x_gsync(&ctl->bar, sh.bar_target);
     X_LAP(was_big ? 5 : 9);
   }
   if (gtid == 0) {
     ctl->gen_id = gen; ctl->wclock = wclock; ctl->tclock = tclock; ctl->sclock = sclock;
-    ctl->generations = generations; ctl->rounds = rounds_total; ctl->dense_rounds = dense_total; ctl->voxels_changed = changed_total;
+    ctl->generations = sh.generations; ctl->rounds = sh.rounds; ctl->dense_rounds = sh.dense_rounds; ctl->voxels_changed = sh.changed;
   }
 }
 
@@ -1274,8 +1220,6 @@ cudaError_t fb_xrelax_launch(FbExact *X, const FbGeom &g, uint32_t *cobs, const 
   a.E[0] = X->E[0]; a.E[1] = X->E[1]; a.emask = X->emask;
   for (int k = 0; k < 3; ++k) { a.W[k] = X->W[k]; a.F[k] = X->F[k]; }
   a.wstamp = X->wstamp; a.slotc = X->slotc; a.ctl = X->d_ctl; a.small_max = X->small_max; a.dense_min = X->dense_min; a.dbg = dbg;
-  a.async_on = X->async ? 1u : 0u;
-  a.small_async_on = X->small_async ? 1u : 0u;
   void *args[] = {(void *)&a};
   if (ndep) {
     const cudaError_t e = cudaLaunchCooperativeKernel(dbg ? (void *)k_x_reseed<true> : (void *)k_x_reseed<false>, dim3(X->relax_blocks), dim3(XT), args, 0, s);

@@ -2,25 +2,21 @@
 // The CPU model of k_x_relax (oracle/exact_model.c) with the asynchronous schedule of fb_xrelax.cu's x_async added: the
 // same replays, checked against the sequential oracle in the same process, voxel for voxel and expansion for expansion.
 //   gcc -O2 -ffp-contract=off -o /tmp/exact_async_model scripts/exact_async_model.c -lm
-//   /tmp/exact_async_model WORKERS SMALL_ASYNC G obs rounds nops seed [small [local [dense_min]]]
-// (the arguments after SMALL_ASYNC are exact_model.c's).  WORKERS = 0 runs exact_model.c's round schedule unchanged.
+//   /tmp/exact_async_model WORKERS G obs rounds nops seed [small [local [dense_min]]]
+// (the arguments after WORKERS are exact_model.c's).  WORKERS = 0 runs exact_model.c's round schedule unchanged.
 // Built with -DNO_DIRTY_RULE, a running element that gets marked is not evaluated again (a mutation the replays must catch).
 //
 // In BIG generations the first work list of at most dense_min entries after round 1 is not evaluated in rounds: it seeds a
-// queue.  SMALL generations: SMALL_ASYNC = 0 keeps their rounds, 1 seeds the queue with the list after round 1, 2 (what
-// k_x_relax does with FIESTA_X_SMALL_ASYNC=1) seeds it with every element of the generation instead of round 1: there,
-// worker w of nwk = min(WORKERS drawn, nE) owns the elements w, w + nwk, ...; it claims up to CLAIM of them at a time,
-// IDLE -> RUNNING (an element a lister already queued is skipped), evaluates them in order, and pops from the queue once
-// its own are done.  Each element is IDLE, PENDING
+// queue; every later round before it is dense.  SMALL generations keep their rounds.  Each element is IDLE, PENDING
 // (queued), RUNNING or DIRTY (running, and an input flipped since it was marked running).  WORKERS simulated workers take
 // steps, one at a time, chosen at random:
 //   pop    take a random queued element, PENDING -> RUNNING;
 //   read   evaluate it from the current words (the kernel's stage);
-//   store  write its word if it flipped (BIG: and record the flip);
+//   store  write its word if it flipped, and record the flip;
 //   list   for every later element it can touch: IDLE -> PENDING and push, RUNNING -> DIRTY, otherwise nothing;
 //   finish DIRTY -> RUNNING and read again, else RUNNING -> IDLE.
 // Other workers' steps fall between a read and its store, so evaluations from stale words happen and must be repaired
-// by the DIRTY rule.  Once the queue is empty and every worker waits, BIG generations refresh the summaries of every flip
+// by the DIRTY rule.  Once the queue is empty and every worker waits, the generation refreshes the summaries of every flip
 // since the last refresh (last round's and every flip of the queue, repeats included) with exact_model.c's
 // refresh_targets rule, in random order, exactly once each; the commit then reads the summaries.  The run prints, over
 // all queue phases, evaluations per seeded entry, dirty re-runs and the longest chain of dependent evaluations (an
@@ -36,13 +32,12 @@ static void relax_dispatch(void);
 #undef main
 #undef relax
 
-static int WORKERS = 8, SMALL_ASYNC = 0;
+static int WORKERS = 8;
 static long a_phases = 0, a_seeds = 0, a_evals = 0, a_dirty = 0, a_maxchain = 0, a_refreshed = 0;
 enum { A_IDLE = 0, A_PEND, A_RUN, A_DIRTY };
 static unsigned char *astate; static u32 *adepth; static u32 *bag; static long nbag;
-typedef struct { int step; u32 i, depth; u64 nb, old; long next; int ncl, pcl; u32 cl[32]; } worker_t;
+typedef struct { int step; u32 i, depth; u64 nb, old; } worker_t;
 #define MAXW 64
-#define CLAIM 4
 
 static void a_mark(u32 j) {
   if (astate[j] == A_IDLE) { astate[j] = A_PEND; bag[nbag++] = j; }
@@ -60,31 +55,22 @@ static u32 a_depth(u32 i) {
   }
   return d + 1;
 }
-// the rest of a generation's fixpoint from the nw elements of wl (wl == NULL: the whole generation, owned by the workers);
-// BIG generations record every flip in F[fout]
-static void async_phase(u32 *wl, long nw, int big, int fout) {
+// the rest of a BIG generation's fixpoint from the nw elements of wl; every flip is recorded in F[fout]
+static void async_phase(u32 *wl, long nw, int fout) {
   a_phases++; a_seeds += nw;
   memset(astate, 0, (size_t)nE); memset(adepth, 0, 4 * (size_t)nE); nbag = 0;
-  if (wl) for (long q = 0; q < nw; q++) a_mark(wl[q]);
+  for (long q = 0; q < nw; q++) a_mark(wl[q]);
   int nwk = 1 + rand() % WORKERS; worker_t wk[MAXW];
-  if (!wl && nwk > nw) nwk = (int)nw;
-  for (int k = 0; k < nwk; k++) { wk[k].step = 0; wk[k].next = wl ? nw : k; wk[k].ncl = wk[k].pcl = 0; }
+  for (int k = 0; k < nwk; k++) wk[k].step = 0;
   for (;;) {
     int en[MAXW], ne = 0;
-    for (int k = 0; k < nwk; k++) if (wk[k].step != 0 || nbag > 0 || wk[k].pcl < wk[k].ncl || wk[k].next < nw) en[ne++] = k;
+    for (int k = 0; k < nwk; k++) if (wk[k].step != 0 || nbag > 0) en[ne++] = k;
     if (!ne) break;                                            // queue empty and every worker waiting: quiescence
     worker_t *w = &wk[en[rand() % ne]];
     for (int t = 0; t < 8 && w->step == 2; t++) w = &wk[en[rand() % ne]];   // stores lag behind: more reads of stale words
     long p;
     switch (w->step) {
       case 0:
-        if (w->pcl < w->ncl) { w->i = w->cl[w->pcl++]; w->step = 1; break; }            // next claimed own seed (RUNNING)
-        if (w->next < nw) {                                                             // claim own seeds: IDLE -> RUNNING
-          w->ncl = w->pcl = 0;
-          for (int c = 0; c < CLAIM && w->next < nw; c++, w->next += nwk)
-            if (astate[w->next] == A_IDLE) { astate[w->next] = A_RUN; w->cl[w->ncl++] = (u32)w->next; }
-          break;
-        }
         if (nbag == 0) break;                                                           // waits for the queue
         { long q = rand() % nbag; w->i = bag[q]; bag[q] = bag[--nbag]; astate[w->i] = A_RUN; w->step = 1; }
         break;
@@ -93,7 +79,8 @@ static void async_phase(u32 *wl, long nw, int big, int fout) {
         p = E[cur][w->i]; w->old = MB[p];
         if (w->nb != w->old) {
           MB[p] = w->nb; adepth[w->i] = w->depth; if (w->depth > a_maxchain) a_maxchain = w->depth;
-          if (big) { if (nF[fout] < N) F[fout][nF[fout]] = w->i; nF[fout]++; }
+          if (nF[fout] < N) F[fout][nF[fout]] = w->i;
+          nF[fout]++;
           w->step = 3;
         } else w->step = 4;
         break;
@@ -127,26 +114,23 @@ static void relax_async(void) {
       long nf = (big && r > 1) ? nF[in] : 0;
       if (r > 1 && nw == 0 && nf == 0) break;
       rounds++;
-      if (big ? r > 1 && nw <= DENSE_MIN : SMALL_ASYNC == 2 ? r == 1 : r > 1 && SMALL_ASYNC) {
-        async_phase(r == 1 ? NULL : wl, nw, big, out);
-        if (big) {                                             // one refresh of every flip since the last one, in random order
-          long nfa = nF[out];
-          if (nfa > N) { sclock++; for (long i = 0; i < nE; i++) claim_summaries(i); }
-          else {
-            u32 *ord = malloc(4 * (nf + nfa + 1)); for (long q = 0; q < nf; q++) ord[q] = F[in][q]; for (long q = 0; q < nfa; q++) ord[nf + q] = F[out][q];
-            shuffle(ord, nf + nfa); for (long q = 0; q < nf + nfa; q++) refresh_targets(ord[q]); a_refreshed += nf + nfa; free(ord);
-          }
+      if (big && r > 1 && nw <= DENSE_MIN) {
+        async_phase(wl, nw, out);
+        long nfa = nF[out];                                    // one refresh of every flip since the last one, in random order
+        if (nfa > N) { sclock++; for (long i = 0; i < nE; i++) claim_summaries(i); }
+        else {
+          u32 *ord = malloc(4 * (nf + nfa + 1)); for (long q = 0; q < nf; q++) ord[q] = F[in][q]; for (long q = 0; q < nfa; q++) ord[nf + q] = F[out][q];
+          shuffle(ord, nf + nfa); for (long q = 0; q < nf + nfa; q++) refresh_targets(ord[q]); a_refreshed += nf + nfa; free(ord);
         }
         break;
       }
-      int dense = big && r > 1 && nw > DENSE_MIN; int use_sum = big && (r == 1 || dense);
+      int dense = big && r > 1;
       if (dense) { totdense++;
         if (nf < nE / 4) { for (long q = 0; q < nf; q++) refresh_targets(F[in][q]); } else { sclock++; for (long i = 0; i < nE; i++) claim_summaries(i); } }
-      long nref = (big && !dense) ? nf : 0; long tot = nw + nref; u32 *ord = malloc(4 * (tot + 1)); for (long q = 0; q < tot; q++) ord[q] = (u32)q; shuffle(ord, tot);
-      for (long q = 0; q < tot; q++) { long a = ord[q];
-        if (a >= nw) { refresh_targets(F[in][a - nw]); continue; }
-        long i = wl[a]; totevals++;
-        u64 nb = eval(i, use_sum); long p = E[cur][i];
+      u32 *ord = malloc(4 * (nw + 1)); for (long q = 0; q < nw; q++) ord[q] = (u32)q; shuffle(ord, nw);
+      for (long q = 0; q < nw; q++) {
+        long i = wl[ord[q]]; totevals++;
+        u64 nb = eval(i, big); long p = E[cur][i];
         if (nb != MB[p]) { int wide = mb_kind(MB[p]) == K_PUSH || mb_kind(nb) == K_PUSH;
           MB[p] = nb; if (big) F[out][nF[out]++] = (u32)i;
           int x, y, z; vxyz(p, &x, &y, &z);
@@ -177,11 +161,11 @@ static void relax_dispatch(void) {
   relax_async();
 }
 int main(int argc, char **argv) {
-  if (argc < 3) { fprintf(stderr, "usage: %s WORKERS SMALL_ASYNC [exact_model.c arguments]\n", argv[0]); return 2; }
-  WORKERS = atoi(argv[1]); SMALL_ASYNC = atoi(argv[2]);
+  if (argc < 2) { fprintf(stderr, "usage: %s WORKERS [exact_model.c arguments]\n", argv[0]); return 2; }
+  WORKERS = atoi(argv[1]);
   if (WORKERS < 0 || WORKERS > MAXW) { fprintf(stderr, "WORKERS: 0..%d\n", MAXW); return 2; }
-  argv[2] = argv[0];
-  const int rc = exact_model_main(argc - 2, argv + 2);
+  argv[1] = argv[0];
+  const int rc = exact_model_main(argc - 1, argv + 1);
   printf("async: workers <= %d, phases %ld, seeded entries %ld, evaluations %ld (%.2f per seeded entry), dirty re-runs %ld, "
          "longest chain of dependent evaluations %ld, flips refreshed %ld\n", WORKERS, a_phases, a_seeds, a_evals,
          a_seeds ? (double)a_evals / a_seeds : 0.0, a_dirty, a_maxchain, a_refreshed);

@@ -10,9 +10,9 @@ to generation 0 (assemble); per frame it prints the dependants, those final afte
 the closure list entries and the resolve passes.  It also prints, per frame, the (nE, rounds) list of every generation.  The numbers of generations and every nE
 are fixed by the sequential result; rounds and list lengths vary from run to run (a round reads words flipped in the same
 round).  For the evaluation-round categories it also splits the time into the summed longest CTA work time of every round
-and the rest (grid barrier plus waiting for the slowest CTA), with a log2 histogram of the list lengths of the short-list
-rounds, and it sums the counters of the asynchronous schedule (FIESTA_X_ASYNC; the queue of BIG generations is phase
-"async", the whole-generation queue of SMALL generations "s.async", FIESTA_X_SMALL_ASYNC).  SMALL generations (at most
+and the rest (grid barrier plus waiting for the slowest CTA), with a log2 histogram of the list lengths of SMALL
+generations' later rounds, and it sums the counters of the asynchronous schedule (the work queue of BIG generations,
+phase "async").  SMALL generations (at most
 FIESTA_X_SMALL entries, default 32768) are summarised over the timed frames by log2 size bucket: count, rounds (a queue
 phase counts as one) and time per generation.  The card, its power limit and the SM clock are printed first.  The output is
 plain text, one item per line, so two runs can be diffed.  Needs a GPU, except with --from-trace FILE, which reads the
@@ -25,10 +25,10 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PHASES = ["S", "round1", "rounds", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
+PHASES = ["S", "round1", "dense", "commit", "apply", "s.round1", "s.rounds", "s.commit", "s.apply", "top",
           "empty-barrier", "reseed.classify", "reseed.closure", "reseed.choose", "reseed.resolve", "reseed.assemble", "async",
-          "refresh", "s.async"]
-ROUND_CATS = ["round1", "rounds", "dense", "s.round1", "s.rounds"]
+          "refresh"]
+ROUND_CATS = ["round1", "dense", "s.round1", "s.rounds"]
 
 
 def card():
@@ -98,7 +98,7 @@ def main():
                closure_entries=0, resolve_passes=0, generations=0, expansions=0)
     reseed = {}                                                # frame -> (dependants, final, closure rounds, entries, passes)
     work = {k: [0.0, 0] for k in ROUND_CATS}
-    hist = {"rounds": {}, "s.rounds": {}}
+    hist = {"s.rounds": {}}
     aq = dict(evaluations=0, dirty=0, pushes=0, spin_us=0.0)
     gens = {}
     f = -1
@@ -145,7 +145,6 @@ def main():
                     b = small.setdefault(int(n).bit_length(), [0, 0, 0.0])
                     b[0] += 1; b[1] += int(r); b[2] += float(t_us[:-2])
     out = ["card: " + card() if not args.from_trace else "trace: " + args.from_trace,
-           "FIESTA_X_ASYNC=%s FIESTA_X_SMALL_ASYNC=%s" % (os.environ.get("FIESTA_X_ASYNC", "(default)"), os.environ.get("FIESTA_X_SMALL_ASYNC", "(default)")),
            "workload %s, frames %d-%d, phase totals of k_x_relax (ms):" % (args.workload, lo, hi - 1)]
     for k in PHASES:
         if k != "empty-barrier":

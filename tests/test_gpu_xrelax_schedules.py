@@ -1,7 +1,7 @@
 """Every schedule of k_x_relax against the sequential reference, on small adversarial maps.
 
 k_x_relax (fiesta_b200/csrc/fb_xrelax.cu) chooses its code paths by list sizes, and at the default thresholds the small maps
-of the other GPU tests only reach SMALL generations and the one-warp-per-dependant re-seeding loop.  Three environment
+of the other GPU tests only reach SMALL generations and the one-warp-per-dependant re-seeding loop.  Two environment
 variables, read once per map when it is created (fb_exact_init), move the thresholds so that small maps run every path:
 
   FIESTA_X_SMALL=n    a generation of more than n entries is BIG: summaries of its targets (x_claim_summaries), round 1
@@ -10,9 +10,8 @@ variables, read once per map when it is created (fb_exact_init), move the thresh
   FIESTA_X_DENSE=n    a later round of a BIG generation whose work list has more than n entries is dense: it refreshes the
                       summaries first (only the targets of last round's flips if these are fewer than nE/4, else it claims
                       every target again), then evaluates through them.  Default 16384; 0 makes every round with work dense.
-  FIESTA_X_ASYNC=0|1  1 (default): in a BIG generation the first later list of at most n entries seeds the device work
-                      queue (x_async), which is followed by one refresh of the targets of the last round's flips (F[in]) and
-                      the queue's (F[out]).  0: such lists run in rounds that refresh the last round's flips concurrently.
+                      The first later list of at most n entries seeds the device work queue (x_async) instead, which is
+                      followed by one refresh of the targets of the last round's flips (F[in]) and the queue's (F[out]).
 
 Whatever the schedule, the result must be the reference's, bit for bit: distance_, closest_obstacle_ (ties included),
 occupancy and the expansion count after every update, and the trilinear queries at the end.  Run this file after every
@@ -39,15 +38,14 @@ from tests import scenes
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-X_ENV = ("FIESTA_X_SMALL", "FIESTA_X_DENSE", "FIESTA_X_ASYNC", "FIESTA_X_TWO_SORTS")
+X_ENV = ("FIESTA_X_SMALL", "FIESTA_X_DENSE", "FIESTA_X_TWO_SORTS")
 
 SCHEDULES = {
     "default": {},                                                              # SMALL generations on these maps
     "big-queue": {"FIESTA_X_SMALL": "0"},                                       # every generation BIG, the queue from round 2
-    "big-rounds": {"FIESTA_X_SMALL": "0", "FIESTA_X_ASYNC": "0"},               # BIG short rounds with concurrent refresh
-    "big-dense": {"FIESTA_X_SMALL": "0", "FIESTA_X_DENSE": "0", "FIESTA_X_ASYNC": "0"},   # every later round dense
-    # dense rounds until only flips are left (nw == 0, nf > 0): then a queue phase seeded with an empty list
-    "dense-then-empty-queue": {"FIESTA_X_SMALL": "0", "FIESTA_X_DENSE": "0", "FIESTA_X_ASYNC": "1"},
+    # every later round with work dense, until only flips are left (nw == 0, nf > 0): then a queue phase seeded with an
+    # empty list
+    "dense-then-empty-queue": {"FIESTA_X_SMALL": "0", "FIESTA_X_DENSE": "0"},
     # dense rounds, then the queue: the last dense round's flips (F[in]) are refreshed after it
     "dense-then-queue": {"FIESTA_X_SMALL": "0", "FIESTA_X_DENSE": "64"},
     "mixed": {"FIESTA_X_SMALL": "256", "FIESTA_X_DENSE": "64"},                # SMALL <-> BIG hand-overs within one UpdateESDF
@@ -399,11 +397,9 @@ GENS = re.compile(r"^\[x\] gens .*\|(.*)$", re.M)
 # schedule -> (scenario, required phase counts); the names are the trace's categories
 COVERAGE = {
     "default": ("salt-and-pepper", {"round1": 0}),             # the gap this file closes: no BIG generation by default
-    "big-queue": ("salt-and-pepper", {"round1": ">0", "async": ">0", "s.round1": 0}),
-    "big-rounds": ("salt-and-pepper", {"rounds": ">0", "async": 0}),
-    "big-dense": ("salt-and-pepper", {"dense": ">0"}),
+    "big-queue": ("salt-and-pepper", {"round1": ">0", "async": ">0", "s.round1": 0, "rounds": 0}),
     "dense-then-empty-queue": ("salt-and-pepper", {"dense": ">0", "async": ">0"}),   # with DENSE=0 the queue only runs when nw == 0
-    "dense-then-queue": ("salt-and-pepper", {"dense": ">0", "async": ">0"}),
+    "dense-then-queue": ("salt-and-pepper", {"dense": ">0", "async": ">0", "rounds": 0}),
     "mixed": ("salt-and-pepper", {"round1": ">0", "s.round1": ">0"}),
     "all-small": ("mass-delete", {"s.round1": ">0"}),           # and generations of 32769..65536 entries (below)
 }
